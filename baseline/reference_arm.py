@@ -1,7 +1,7 @@
 """Reference arm of bench.py: the UNMODIFIED reference (facebookresearch/mbrl-lib) on the host CPUs.
 
-``baseline/_ref`` holds ``pip install --no-deps --target baseline/_ref /root/reference`` (git-ignored, travels to the
-GPU box with the snapshot); in the build container ``/root/reference`` works too.  mbrl-lib imports hydra, omegaconf,
+``oracle/_ref`` holds a copy of the reference's ``mbrl`` package made by ``oracle/install_ref.py`` (git-ignored: it is
+not part of this project).  mbrl-lib imports hydra, omegaconf,
 gymnasium and termcolor at module level; none of them is installed in this image and there is no index, so the
 API shims under ``oracle/ref_shims`` (a dict-backed DictConfig, ``hydra.utils.instantiate``, ``gymnasium.spaces.Box``)
 stand in for them.  They are configuration plumbing only: every tensor operation on the timed path
@@ -34,7 +34,7 @@ def import_reference():
         except ImportError:
             if shims not in sys.path:
                 sys.path.insert(0, shims)
-    for cand in (os.path.join(ROOT, "baseline", "_ref"), "/root/reference"):
+    for cand in (os.path.join(ROOT, "oracle", "_ref"),):
         if os.path.isdir(os.path.join(cand, "mbrl")):
             sys.path.insert(0, cand)
             try:
@@ -51,7 +51,7 @@ def import_reference():
                     del sys.modules[k]
                 last = f"{cand}: {type(e).__name__}: {e}"
                 continue
-    return None, locals().get("last", "no baseline/_ref and no /root/reference")
+    return None, locals().get("last", "no oracle/_ref (see oracle/install_ref.py)")
 
 
 def _proc_fn(name):

@@ -14,11 +14,10 @@ population, ONE all-gather of local top-k records per CEM iteration (mbrl_lib_b2
 The same run also reports BASELINE config 5 (fixed global populations 8 000 ... 64 000 sharded over the N GPUs,
 strong scaling) with the collective's share of an iteration, in ``config5_population_scan_sharded``.
 
-``--impl reference``: the UNMODIFIED reference (mbrl-lib from ``baseline/_ref``) timed on the host CPUs through
+``--impl reference``: the UNMODIFIED reference (mbrl-lib from ``oracle/_ref``) timed on the host CPUs through
 its own ``TrajectoryOptimizerAgent.act`` (rank 0 only); the oracle port is the fallback when it cannot be imported.
 """
 import argparse
-import csv
 import json
 import os
 import statistics
@@ -37,7 +36,7 @@ from mbrl_lib_b200 import synthetic as syn  # noqa: E402
 
 WORKLOAD = "halfcheetah"  # BASELINE.json configs[1]
 CEM_ITERS, ELITE_RATIO, ALPHA = 5, 0.1, 0.1
-FLOP_PER_SEQ = 157.68e6  # SURVEY.md section 8d: 2 * sum K*N (true dims) * P * H = 262 800 * 20 * 30
+FLOP_PER_SEQ = 157.68e6  # 2 * sum K*N (true dims) * P * H = 262 800 * 20 * 30
 METRIC = "candidate action-sequences/sec, PETS HalfCheetah CEM"
 # identical on both arms (ours and --impl reference): what is computed per step
 CONFIG = {
@@ -45,31 +44,22 @@ CONFIG = {
                  "per plan, horizon 30, 20 particles, TS1"),
     "step": "one 5-iteration CEM plan = one TrajectoryOptimizerAgent.act(): 2 500 candidate sequences per GPU",
 }
-NCU_SUMMARIES = ["profiles/r2_rollout_tc_ncu_full_summary.csv", "profiles/r1_rollout_tc_final_ncu_full_summary.csv"]
+# NVIDIA H100 SXM data sheet, dense BF16 (700 W card): the denominator of the roofline fraction, not a reached rate
+H100_BF16_DENSE_TFLOPS = 989.0
 
 
 def measured_peak_tflops():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["bf16_tflops"]), "measured (MEASURED_PEAKS.json bf16_tflops, burst)"
-    return 1590.0, "fallback (B200_PROFILING.md 1.59 PFLOP/s)"
+    return H100_BF16_DENSE_TFLOPS, "H100 SXM data sheet, dense BF16 (989 TFLOP/s at 700 W)"
 
 
-def ncu_dram_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum of ONE rollout launch from the newest committed ncu --set full summary."""
-    unit = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-    for rel in NCU_SUMMARIES:
-        path = os.path.join(ROOT, rel)
-        if not os.path.exists(path):
-            continue
-        tot, seen = 0.0, 0
-        for row in csv.reader(open(path)):
-            if len(row) >= 3 and row[0] in ("dram__bytes_read.sum", "dram__bytes_write.sum") and row[1] in unit:
-                tot += float(row[2]) * unit[row[1]]
-                seen += 1
-        if seen == 2:
-            return int(tot), rel
-    return None, None
+def dump_outputs(directory, arrays):
+    """Writes what the timed path returned in its last step, one float32 .npy per array."""
+    os.makedirs(directory, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(directory, f"{name}.npy"), t.detach().float().cpu().numpy())
 
 
 class ClockSampler:
@@ -318,6 +308,7 @@ def run_ours(args):
     local = int(os.environ.get("LOCAL_RANK", "0"))
     torch.cuda.set_device(local)
     device = f"cuda:{local}"
+    torch.manual_seed(0)  # the optimisers' Philox seed: identical populations from run to run
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device(device))
     spec, arrays, env = build_problem(device)
@@ -372,9 +363,11 @@ def run_ours(args):
     for s, e in evs:
         flush.fill_(1)
         s.record()
-        step()
+        solution = step()
         e.record()
     barrier()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"solution": solution})  # the plan (horizon x action dim) of the last timed step
     step_ms = [s.elapsed_time(e) for s, e in evs]
     total_ms = torch.tensor([sum(step_ms)], device=device, dtype=torch.float64)
     if world > 1:
@@ -510,7 +503,6 @@ def run_ours(args):
 
     if rank == 0:
         achieved = N * FLOP_PER_SEQ / (kern_ms_avg * 1e-3) / 1e12
-        traffic, traffic_src = ncu_dram_traffic()
         line = {
             "metric": METRIC, "value": seqs_per_step * args.steps / (total_ms * 1e-3), "unit": "sequences/s",
             "n_gpus": world, "steps": args.steps, "warmup": warmup, "ms_per_step": total_ms / args.steps,
@@ -523,8 +515,7 @@ def run_ours(args):
                            "precision": env.precision},
             "gpu_launches": launches_per_step * args.steps,
             "roofline": {"bound": "tensor", "achieved": achieved, "peak": peak_tf, "unit": "TFLOP/s", "frac": achieved / peak_tf,
-                         "traffic": traffic, "traffic_source": f"ncu --set full dram__bytes_read.sum + dram__bytes_write.sum of one launch ({traffic_src}); "
-                         "algorithmic: 1.3 MB bf16 weights + 0.36 MB actions + 2 KB returns",
+                         "traffic_source": "algorithmic: 1.3 MB bf16 weights + 0.36 MB actions + 2 KB returns",
                          "kernel": "rollout_tc_kernel (one CEM iteration: 500 sequences x 20 particles x 30 steps)",
                          "kernel_ms": kern_ms_avg, "peak_source": peak_src, "algorithmic_flop_per_launch": N * FLOP_PER_SEQ},
             "clocks": clocks,
@@ -652,6 +643,7 @@ if __name__ == "__main__":
     ap.add_argument("--no-cpu", action="store_true", help="skip the CPU baseline leg")
     ap.add_argument("--no-scan5", action="store_true", help="skip the sharded config-5 population scan (N > 1)")
     ap.add_argument("--no-scan", action="store_true", help="skip the population scan / extra configurations")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's plan to DIR/solution.npy (float32)")
     a = ap.parse_args()
     if a.impl == "reference":
         run_reference(a)

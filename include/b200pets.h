@@ -1,5 +1,5 @@
 /*
- * b200pets.h -- C ABI of the B200-native PETS planning hot path.
+ * b200pets.h -- C ABI of the H100-native PETS planning hot path.
  *
  * The reference (facebookresearch/mbrl-lib) has no FFI: its plugin boundary is Python duck typing
  * (SURVEY.md section 8b).  This header is the boundary a native binding would target; every entry point
@@ -67,7 +67,7 @@ extern "C" {
 
 /* arithmetic of the ensemble MLP */
 #define B200PETS_PREC_F32 0     /* fp32 SIMT: parity anchor (~1e-5 of the reference) */
-#define B200PETS_PREC_BF16_TC 1 /* bf16 operands, fp32 accumulate on tcgen05 tensor cores */
+#define B200PETS_PREC_BF16_TC 1 /* bf16 operands, fp32 accumulate on the tensor cores (wgmma) */
 
 /* how TS1 assigns rows to members when no permutation is injected */
 #define B200PETS_TS1_PERMS 0        /* explicit permutations (one per step), reference semantics */
@@ -309,20 +309,11 @@ int b200pets_cem_plan(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, 
                       const float* z, const float* eps, const int64_t* perms, float* solution,
                       float* values_out, void* workspace, size_t workspace_bytes, void* stream);
 
-/* Diagnostics: when stamps [dev] int64[128] is non-NULL, CTA 0 of every tensor-core rollout launch writes clock64()
- * stamps of one horizon step (epilogue thread: slots 0.., MMA thread: slots 64 + 4 * layer ..); NULL disables. */
-int b200pets_debug_timeline(int64_t* stamps);
-
-/* Diagnostics: cycles [dev] int64[2] <- (issue, issue+complete) clock64 cycles of reps x (k/16) back-to-back
- * tcgen05.mma M=128 x n with operand layout `mode` (0 = the rollout kernel's no-swizzle layout, 1 = SWIZZLE_128B,
- * 2 = no-swizzle with adjacent K halves).  Timing only. */
-int b200pets_debug_umma_bench(int32_t mode, int32_t k, int32_t n, int32_t reps, int64_t* cycles, void* stream);
-
-/* Self test of the tcgen05 building block: D[128][n] = A[128][k] * B[n][k]^T with bf16 operands staged in
- * the no-swizzle canonical layout the rollout kernel uses.  a, b [dev] float (rounded to bf16 inside),
- * d [dev] float[128][n].  k, n multiples of 16, n <= 256.  A negative k runs the A-from-TMEM (tcgen05.st -> .ts MMA)
- * form with |k|. */
-int b200pets_selftest_umma(int32_t k, int32_t n, const float* a, const float* b, float* d, void* stream);
+/* Self test of the wgmma building block: D[128][n] = A[128][k] * B[n][k]^T with bf16 operands staged in the
+ * no-swizzle canonical layouts, the weight ring and the accumulator fragments the rollout kernel uses.  a, b [dev] float
+ * (rounded to bf16 inside), d [dev] float[128][n].  k, n multiples of 16, <= 256.  A negative k writes A as bf16 pairs
+ * per thread and row (the hidden-layer epilogue's stores) with |k|. */
+int b200pets_selftest_wgmma(int32_t k, int32_t n, const float* a, const float* b, float* d, void* stream);
 
 #ifdef __cplusplus
 }

@@ -1,4 +1,4 @@
-"""b200pets: a Blackwell-native PETS planning inner loop behind mbrl-lib's Agent / Optimizer / ModelEnv API.
+"""b200pets: an H100-native PETS planning inner loop behind mbrl-lib's Agent / Optimizer / ModelEnv API.
 
 Sub-modules are imported lazily so that the seeded synthetic-input helpers (``synthetic``) can be used
 without the CUDA library; every compute entry point fails loudly when ``libb200pets.so`` is missing.

@@ -1,6 +1,6 @@
 """ctypes binding of ``libb200pets.so`` (the C ABI in ``include/b200pets.h``).
 
-The library is built in-tree by ``build.py`` (nvcc, sm_100a).  There is no CPU fallback: if the shared
+The library is built in-tree by ``build.py`` (nvcc, sm_90a).  There is no CPU fallback: if the shared
 object is missing or a call fails, a ``RuntimeError`` carrying ``b200pets_last_error()`` is raised.
 """
 from __future__ import annotations
@@ -92,9 +92,7 @@ _SIGNATURES = {
     "b200pets_cem_elites_refit": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_int32, C.c_int32,
                                             C.c_int32, C.c_uint32, C.POINTER(C.c_void_p), _P, _P, _P, _P, _P, C.c_int32, _P, _P,
                                             C.c_uint64, C.c_uint64, C.c_int32, _P, _P, _P]),
-    "b200pets_debug_timeline": (C.c_int, [_P]),
-    "b200pets_debug_umma_bench": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P]),
-    "b200pets_selftest_umma": (C.c_int, [C.c_int32, C.c_int32, _P, _P, _P, _P]),
+    "b200pets_selftest_wgmma": (C.c_int, [C.c_int32, C.c_int32, _P, _P, _P, _P]),
 }
 
 _lib = None

@@ -1,4 +1,4 @@
-"""Build libb200pets.so in-tree with nvcc for sm_100a (no GPU needed: nvcc cross-compiles)."""
+"""Build libb200pets.so in-tree with nvcc for sm_90a (no GPU needed: nvcc cross-compiles)."""
 import os
 import subprocess
 import sys
@@ -7,7 +7,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200pets.so")
 SOURCES = ["api.cu", "rollout_f32.cu", "rollout_tc.cu", "cem.cu", "mbpo.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 
@@ -32,7 +32,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             print(" ".join(cmd), flush=True)
         subprocess.check_call(cmd)
         objs.append(obj)
-    subprocess.check_call([nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"])
+    subprocess.check_call([nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-lcudart"])
     return LIB
 
 

@@ -13,7 +13,7 @@
 // launchers defined in the kernel translation units
 int launch_rollout_f32(const ModelDev& m, const RolloutArgs& a, cudaStream_t stream);
 int launch_rollout_tc(const ModelDev& m, const RolloutArgs& a, cudaStream_t stream);
-int launch_umma_selftest(int k, int n, const float* a, const float* b, float* d, cudaStream_t stream);
+int launch_wgmma_selftest(int k, int n, const float* a, const float* b, float* d, cudaStream_t stream);
 int launch_particle_mean(int N, int P, const float* total, float* returns, cudaStream_t stream);
 bool cem_refit_sample_supported(int population, int dims, int elite_num);
 int launch_cem_refit_sample(int population, int dims, int elite_num, float alpha, int use_std, const float* row_totals,
@@ -26,7 +26,6 @@ int launch_cem_update_rows(int population, int dims, int elite_num, float alpha,
                            float* dispersion, float* best_value, float* best_solution, void* workspace,
                            size_t workspace_bytes, void* stream);
 bool tc_supported(const ModelDev& m);
-int launch_umma_bench(int mode, int k, int n, int reps, long long* out, cudaStream_t stream);
 
 // ---------------------------------------------------------------------------------------------------------
 // errors
@@ -68,7 +67,7 @@ __global__ void gather_members_kernel(const float* __restrict__ src, float* __re
   dst[idx] = src[(long long)members[m] * per_member + idx % per_member];
 }
 
-// bf16 UMMA image of one layer for every member: [m][Kp/8][Np/8][8 n][8 k]; rows K, K+1 carry the split bias;
+// bf16 tensor-core image of one layer for every member: [m][Kp/8][Np/8][8 n][8 k]; rows K, K+1 carry the split bias;
 // the output layer's logvar columns are moved to start at column outp.
 __global__ void pack_image_kernel(const float* __restrict__ Wg, const float* __restrict__ bg, unsigned char* __restrict__ img,
                                   unsigned member_stride, unsigned layer_off, int M, int K, int N, int Kp, int Np,
@@ -289,7 +288,6 @@ int b200pets_model_supports_tc(b200pets_model_t model) { return model && model->
 // ---------------------------------------------------------------------------------------------------------
 // rollouts
 // ---------------------------------------------------------------------------------------------------------
-static long long* g_timeline = nullptr;
 
 static int shard_of(const b200pets_rollout_cfg* cfg, int* seq0, int* n_glob) {
   *seq0 = cfg->first_sequence;
@@ -302,7 +300,6 @@ static int shard_of(const b200pets_rollout_cfg* cfg, int* seq0, int* n_glob) {
 
 static int dispatch(const b200pets_model_s* mdl, int precision, const RolloutArgs& a_in, cudaStream_t stream) {
   RolloutArgs a = a_in;
-  a.timeline = g_timeline;
   if (precision == B200PETS_PREC_BF16_TC) {
     if (!mdl->tc_ok) return b200pets_set_error(B200PETS_EUNSUPPORTED, "tensor-core path does not cover this model; use B200PETS_PREC_F32");
     return launch_rollout_tc(mdl->dev, a, stream);
@@ -477,10 +474,9 @@ int b200pets_cem_plan(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, 
 
   cem_init_kernel<<<(dims + 255) / 256, 256, 0, stream>>>(dims, x0, lower, upper, ccfg->clipped_normal, mu, disp, best_val);
   CUDA_TRY(cudaGetLastError());
-  // Default: sample -> rollout -> refit (3 launches per iteration; the refit kernel fuses the particle mean).  B200PETS_CEM_FUSED=1 selects the fused variants, kept because they are parity-tested but measured
-  // SLOWER on B200: refit by the last CTA of the rollout kernel (2 launches / iteration, 2.01 ms) and, with
-  // B200PETS_CEM_SAMPLE_IN_KERNEL=1, the population drawn inside the rollout kernel too (1 launch / iteration,
-  // 2.68 ms: every particle row re-derives its sequence's actions on the epilogue's critical path).
+  // Default: sample -> rollout -> refit (3 launches per iteration; the refit kernel fuses the particle mean).  B200PETS_CEM_FUSED=1 selects the fused variants (parity-tested, not the default): refit by the last CTA of the
+  // rollout kernel (2 launches / iteration) and, with B200PETS_CEM_SAMPLE_IN_KERNEL=1, the population drawn inside the
+  // rollout kernel too (1 launch / iteration: every particle row re-derives its sequence's actions).
   const char* env_fuse = getenv("B200PETS_CEM_FUSED");
   const bool fuse = (env_fuse && env_fuse[0] == '1') && rcfg->precision == B200PETS_PREC_BF16_TC && model->tc_ok && !z &&
                     !perms && N <= 2048 && dims <= 1024 && ccfg->elite_num >= 2 && ccfg->elite_num <= N &&
@@ -617,17 +613,8 @@ int b200pets_shuffle_member_map(const b200pets_rollout_cfg* cfg, int32_t num_mem
   return B200PETS_OK;
 }
 
-int b200pets_debug_timeline(int64_t* stamps) {
-  g_timeline = reinterpret_cast<long long*>(stamps);
-  return B200PETS_OK;
-}
-
-int b200pets_debug_umma_bench(int32_t mode, int32_t k, int32_t n, int32_t reps, int64_t* cycles, void* stream) {
-  return launch_umma_bench(mode, k, n, reps, reinterpret_cast<long long*>(cycles), (cudaStream_t)stream);
-}
-
-int b200pets_selftest_umma(int32_t k, int32_t n, const float* a, const float* b, float* d, void* stream) {
-  return launch_umma_selftest(k, n, a, b, d, (cudaStream_t)stream);
+int b200pets_selftest_wgmma(int32_t k, int32_t n, const float* a, const float* b, float* d, void* stream) {
+  return launch_wgmma_selftest(k, n, a, b, d, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -1,4 +1,4 @@
-// Shared device-side definitions of the PETS planning kernels (sm_100a).
+// Shared device-side definitions of the PETS planning kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -25,7 +25,7 @@ struct ModelDev {
   const float* min_lv;                  // [out]
   const float* max_lv;
   const uint8_t* no_delta;              // [D] mask
-  // tensor-core images (bf16, UMMA no-swizzle K-major canonical layout), see rollout_tc.cu
+  // tensor-core images (bf16, no-swizzle K-major canonical layout of wgmma), see rollout_tc.cu
   const uint8_t* img;                   // base of member 0
   uint32_t img_member_stride;           // bytes between members
   uint32_t img_replica_stride;          // bytes between replicas of the whole image set
@@ -65,7 +65,6 @@ struct RolloutArgs {
   // step outputs (b200pets_step): next_obs = obs_out, reward, done
   float* reward_out;       // [B] or NULL
   uint8_t* done_out;       // [B] or NULL
-  long long* timeline;     // diagnostics: clock64 stamps of CTA 0 (b200pets_debug_timeline) or NULL
   // ---- fused CEM iteration (tensor-core kernel only): population sampled in-kernel, refit by the last CTA ----
   const float* cem_mu;     // [H*A] sampling mean; non-NULL switches the action source to in-kernel sampling
   const float* cem_disp;   // [H*A] variance (truncated normal) or std (clipped normal)
@@ -313,7 +312,7 @@ static inline unsigned long long rng_key(unsigned long long seed, unsigned long 
 // ------------------------------------------------------------------------------------------------------
 // Programmatic dependent launch (PDL).  The kernels of a plan form a chain  sample -> rollout -> refit -> sample ..
 // on one stream.  Launched with the programmatic-stream-serialization attribute, a kernel may become resident as soon
-// as its predecessor has executed pdl_trigger() in all its CTAs; it then runs its prologue (barrier / TMEM set-up,
+// as its predecessor has executed pdl_trigger() in all its CTAs; it then runs its prologue (barrier set-up,
 // constant tables, the first weight prefetches -- memory no kernel of the chain writes) and blocks in pdl_wait() until
 // the predecessor grid has completed and flushed, BEFORE its first access to anything the chain produces.  Every
 // kernel of the chain waits before it finishes, so completion is transitive along the chain.  Launch gaps and the

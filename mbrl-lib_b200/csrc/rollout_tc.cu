@@ -1,20 +1,21 @@
-// Tensor-core rollout of the ensemble MLP on sm_100a: bf16 operands, fp32 accumulation in TMEM.
+// Tensor-core rollout of the ensemble MLP on sm_90a: bf16 operands, fp32 accumulation in registers (wgmma).
 //
 // One persistent CTA per SM walks 128-row tiles through steps [t0, t1) of the horizon without leaving the chip:
 //  * row state (observation, return, dead flag, actions) stays in shared memory / registers;
-//  * each layer is a chain of tcgen05.mma (M=128, K=16) in the A-from-TMEM form: the activations are written by the
-//    epilogue warps as bf16 pairs with tcgen05.st into a TMEM buffer and never touch shared memory;
-//  * the B operand (weights) is streamed from the L2-resident packed image into two shared-memory layer slots by
-//    1-D TMA bulk copies (cp.async.bulk + mbarrier expect_tx), one slot in use while the next layer is in flight;
-//  * hidden layers are split in two N halves (128 + 80 columns at width 208) so that epilogue, MMAs of the other half
-//    and the next layer's first K steps overlap (see the kernel's header comment);
-//  * without an observation pre-processor the output-layer epilogue also writes the next step's layer-0 operand
-//    (no barrier, no builder pass between two steps); propagation "expectation" runs M member passes per step.
+//  * two consumer warpgroups own 64 rows each.  A layer is a chain of wgmma.mma_async (M=64, K=16, N <= 128 per
+//    instruction, two instructions per K step for layers wider than 128) that reads the warpgroup's activations from
+//    its own shared-memory operand buffer; the accumulators stay in registers until the layer's last K step, then the
+//    epilogue writes the activated, bf16-packed columns back into the same buffer (the next layer's A operand) or, for
+//    the output layer, the fp32 accumulators into a staging area that aliases it;
+//  * the B operand (weights) is streamed from the L2-resident packed image in K slices of up to 4 x 16 rows
+//    by 1-D TMA bulk copies (cp.async.bulk + mbarrier expect_tx) into a ring of shared-memory slots: a producer warp
+//    keeps the ring full across layers, steps and tiles, and a slot is released as soon as both warpgroups' MMAs that
+//    read it have completed (wgmma.wait_group 1);
+//  * propagation "expectation" runs M member passes per step.
 //
-// Warp roles (64 + 128 * CS threads):  warp 0 = weight producer (one elected lane),
-//                            warp 1 = TMEM allocator + MMA issuer (converged warp, MMAs under elect.sync),
-//                            warps 2.. = 4 * CS epilogue warps: warp (q, cs) <-> TMEM lanes 32q..32q+31 (tile rows)
-//                            and every CS-th 16-column chunk; thread (row, cs == 0) owns the row's scalar state.
+// Warp roles (256 + 32 threads): warps 0-3 = warpgroup 0 (tile rows 0-63), warps 4-7 = warpgroup 1 (rows 64-127),
+// warp 8 = weight producer (one lane).  Thread (row r, half h) of a warpgroup builds / samples half of the row's
+// columns; half 0 owns the row's scalar state.
 //
 // Bias is folded into the GEMM: every A tile carries two constant-one columns after the real inputs and the
 // packed weight image carries bf16(b) and bf16(b - bf16(b)) in the matching K rows (api.cu pack kernel).
@@ -23,32 +24,33 @@
 #include <stdlib.h>
 
 #include "common.cuh"
-#include "sm100.cuh"
+#include "sm90.cuh"
 
-using namespace sm100;
+using namespace sm90;
 
 struct TcPlan {
   int nlayers;
-  int nblk[B200PETS_MAX_LAYERS];  // K-blocks (64 K-elements) per layer
-  uint32_t stage_bytes;
+  int kp_max;           // widest layer input (K columns of the operand buffers)
+  int kslice;           // K steps (16 rows of the weight image each) per ring slot
+  uint32_t slot_bytes;  // one ring slot: kslice K steps of the widest layer
   int nstages;
-  uint32_t off_A, off_ring, off_obs, off_act, off_tail, off_const, off_cout, off_bar;
-  int tail_ld;
-  uint32_t tmem_cols;
+  uint32_t wg_bytes;    // operand buffer / output staging of one warpgroup
+  int stg_ld;           // row stride (floats) of the output staging
+  uint32_t off_A, off_ring, off_obs, off_act, off_const, off_cout, off_bar;
   int obs_ld, act_ld;
-  int h0n;  // columns of the first N half of the hidden layers
   uint32_t smem_bytes;
   uint32_t off_exp;  // [128][exp_ld] member sums of mean / log2-variance terms (propagation "expectation" launches only)
   int exp_ld;
-  int tail_split;  // fast tail chunk: 1 = two columns per column-split warp, 0 = one warp takes all eight
 };
 
 namespace {
 
-constexpr int kEpiSplit = 4;  // column splits of the epilogue (16 epilogue warps)
 constexpr int kTileM = 128;
-constexpr int kMaxStages = 8;
+constexpr int kThreads = 256 + 32;
+constexpr int kSliceK16 = 4;       // longest ring slot in K steps (16 rows of the weight image each)
+constexpr int kMaxStages = 16;
 constexpr int kCemTabDims = 1024;  // horizon * act_dim supported by the fused CEM iteration
+constexpr uint32_t kTailScratch = 256 + 2048 * 9 + (kThreads / 32 + 1) * kCemTabDims * 4;  // cem_tail_refit's scratch
 
 __device__ __forceinline__ float tanh_approx(float x) {
   float y;
@@ -86,51 +88,123 @@ __device__ __forceinline__ float act_tc(float x, float slope) {
   return x > 0.f ? x : x * slope;
 }
 
-// byte offset of the 16-byte chunk (row i, k-chunk kc) in the A tile: [kc][i / 8][i % 8][8 x bf16]
-__device__ __forceinline__ uint32_t a_chunk_off(int i, int kc) { return (uint32_t)((kc * 16 + (i >> 3)) * 128 + (i & 7) * 16); }
+// Byte offset of (row r, column k) in a warpgroup's operand buffer: 64 rows, K-major core matrices of 8 rows x 16 bytes,
+// [k / 8][r / 8][r % 8][k % 8] -> LBO (K direction) = 1024 B, SBO (row direction) = 128 B.
+__device__ __forceinline__ uint32_t a_off(int r, int k) {
+  return (uint32_t)((k >> 3) * 1024 + (r >> 3) * 128 + (r & 7) * 16 + (k & 7) * 2);
+}
 
+__device__ __forceinline__ void wg_bar(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
 
-// layer-0 operand of one step -> activation buffer in TMEM: normalise(cat(proc(obs), act)), two constant-one bias
-// columns, zero pad.  Branch-free for obs_process == NONE (clamped loads + selects), generic otherwise.  Not inlined:
-// executed once per horizon step, and the kernel's code size matters (instruction cache).
-// The model dimensions come in BY VALUE: a `const ModelDev&` here made the compiler keep a per-thread copy of the
-// whole parameter struct in local memory (464 B x 576 threads, far more than the L1 left beside 200 KB of shared
-// memory), and every field read in the step loop became an L2 round trip.
-struct InDims {
-  int Kp0, D, Dp, A, in, obs_process;
+// One layer of one warpgroup: D (64 x np) = A (64 x 16 nk, shared memory) * W^T, W streamed through the ring in slices
+// of kslice K steps.  The accumulator is split in two register chunks of W0 and W1 (0 or more) columns, np = W0 + W1.
+// mode 0 (hidden layer): activation, bias-one columns n_true and n_true + 1, zero pad up to kp_next, bf16 pairs back into
+// the operand buffer; mode 1 (output layer / self test): fp32 accumulators to the staging rows (stride stg_ld floats) that
+// alias the operand buffer.  Returns the advanced ring position (stage | phase << 16).
+struct LayerArgs {
+  uint32_t a_addr;  // shared address of the warpgroup's operand buffer
+  uint8_t* a_ptr;   // same, generic
+  uint32_t ring_addr, slot_bytes;
+  int nstages, kslice, nk, np, mode, n_true, kp_next, stg_ld;
+  float leaky;
 };
-static __device__ __noinline__ void build_input_tmem(const InDims m, const float* my_obs, const float* tail,
-                                                     const float2* c_norm, uint32_t a_out, int cs, int CS,
-                                                     uint64_t* bar_ar) {
-  const int Kp0 = m.Kp0;
-  // Work unit = 8 operand columns (4 TMEM columns, one tcgen05.st.x4), dealt round-robin to the CS column-split warps
-  // of the row: with Kp0 = 32 every warp has exactly one unit.  Columns past the processed observation come from the
-  // row's `tail` words (this step's actions, the two bias ones, zero pad, already in operand order) and c_norm holds
-  // {mean, 1/std} pairs ((0, 1) past the real inputs), so every element is "load, subtract, scale" with independent
-  // loads (a branchy form serialised ~8 x (3 dependent LDS + branches) ~ 1.3 k cycles on the step's critical path).
-  for (int gi = cs; gi < Kp0 / 8; gi += CS) {
-    float raw[8];
-    float2 nm[8];
+
+template <int ACT, int W0, int W1>
+static __device__ __noinline__ uint32_t wg_layer(const LayerArgs la, uint32_t ring_pos, uint64_t* bar_full, uint64_t* bar_empty) {
+  constexpr int R1 = W1 > 0 ? W1 / 2 : 1;
+  float d0[W0 / 2], d1[R1];
 #pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      const int j = gi * 8 + e;
-      if (m.obs_process == B200PETS_PROC_NONE) raw[e] = j < m.Dp ? my_obs[j] : tail[j - m.Dp];
-      else raw[e] = j < m.Dp ? proc_obs_elem(my_obs, j, m.obs_process) : tail[j - m.Dp];  // sin / cos columns: cold path
-      nm[e] = c_norm[j];
+  for (int i = 0; i < W0 / 2; ++i) d0[i] = 0.f;
+#pragma unroll
+  for (int i = 0; i < R1; ++i) d1[i] = 0.f;
+  const int wt = threadIdx.x & 127, lane = threadIdx.x & 31;
+  int stage = (int)(ring_pos & 0xFFFFu);
+  uint32_t phase = ring_pos >> 16;
+  int prev = -1;
+  const uint32_t b_lbo = (uint32_t)la.np * 16u;
+  const uint32_t b_kstep = 2u * b_lbo;  // bytes of one K step (16 rows) of the weight image
+  fence_operands(d0);
+  fence_operands(d1);
+  for (int k0 = 0; k0 < la.nk; k0 += la.kslice) {
+    mbar_wait(&bar_full[stage], phase);
+    wgmma_fence();
+    const uint32_t slot = la.ring_addr + (uint32_t)stage * la.slot_bytes;
+    const int k1 = min(la.nk, k0 + la.kslice);
+    for (int kk = k0; kk < k1; ++kk) {
+      const uint64_t da = wgmma_desc(la.a_addr + (uint32_t)kk * 2048u, 1024u, 128u);
+      const uint32_t b = slot + (uint32_t)(kk - k0) * b_kstep;
+      Wgmma<W0>::mma(d0, da, wgmma_desc(b, b_lbo, 128u), kk > 0 ? 1u : 0u);
+      if constexpr (W1 > 0) Wgmma<W1>::mma(d1, da, wgmma_desc(b + (uint32_t)(W0 / 8) * 128u, b_lbo, 128u), kk > 0 ? 1u : 0u);
     }
-    uint32_t pk[4];
+    wgmma_commit();
+    if (prev >= 0) {  // the previous slice's MMAs are complete: hand its slot back to the producer
+      wgmma_wait<1>();
+      if (lane == 0) mbar_arrive(&bar_empty[prev]);
+    }
+    prev = stage;
+    if (++stage == la.nstages) { stage = 0; phase ^= 1u; }
+  }
+  wgmma_wait<0>();
+  fence_operands(d0);
+  fence_operands(d1);
+  if (lane == 0) mbar_arrive(&bar_empty[prev]);
+  wg_bar((threadIdx.x >> 7) & 1);  // every MMA of the warpgroup has read its operand buffer: it may be overwritten
+
+  const int r0 = 16 * (wt >> 5) + (lane >> 2);  // fragment rows r0 and r0 + 8
+  const int cq = 2 * (lane & 3);
+  if (la.mode == 0) {
+    auto store = [&](float x0, float x1, float x2, float x3, int col) {
+      float v[4] = {act_tc<ACT>(x0, la.leaky), act_tc<ACT>(x1, la.leaky), act_tc<ACT>(x2, la.leaky), act_tc<ACT>(x3, la.leaky)};
+      if (col == la.n_true || col == la.n_true + 1) v[0] = v[2] = 1.f;
+      if (col + 1 == la.n_true || col + 1 == la.n_true + 1) v[1] = v[3] = 1.f;
+      *reinterpret_cast<uint32_t*>(la.a_ptr + a_off(r0, col)) = pack_bf16(v[0], v[1]);
+      *reinterpret_cast<uint32_t*>(la.a_ptr + a_off(r0 + 8, col)) = pack_bf16(v[2], v[3]);
+    };
 #pragma unroll
-    for (int e = 0; e < 4; ++e)
-      pk[e] = pack_bf16((raw[2 * e] - nm[2 * e].x) * nm[2 * e].y, (raw[2 * e + 1] - nm[2 * e + 1].x) * nm[2 * e + 1].y);
-    tmem_st4(a_out + (uint32_t)(4 * gi), pk);
+    for (int j = 0; j < W0 / 8; ++j) store(d0[4 * j], d0[4 * j + 1], d0[4 * j + 2], d0[4 * j + 3], 8 * j + cq);
+    if constexpr (W1 > 0) {
+#pragma unroll
+      for (int j = 0; j < W1 / 8; ++j) store(d1[4 * j], d1[4 * j + 1], d1[4 * j + 2], d1[4 * j + 3], W0 + 8 * j + cq);
+    }
+    // operand columns past the accumulator (np .. kp_next): bias ones / zero pad
+    const int npad = la.kp_next - la.np;
+    for (int idx = wt; idx < 64 * (npad >> 1); idx += 128) {
+      const int r = idx & 63, col = la.np + 2 * (idx >> 6);
+      const float v0 = (col == la.n_true || col == la.n_true + 1) ? 1.f : 0.f;
+      const float v1 = (col + 1 == la.n_true || col + 1 == la.n_true + 1) ? 1.f : 0.f;
+      *reinterpret_cast<uint32_t*>(la.a_ptr + a_off(r, col)) = pack_bf16(v0, v1);
+    }
+    fence_proxy_async_smem();
+  } else {
+    float* stg = reinterpret_cast<float*>(la.a_ptr);
+#pragma unroll
+    for (int j = 0; j < W0 / 8; ++j) {
+      *reinterpret_cast<float2*>(stg + r0 * la.stg_ld + 8 * j + cq) = make_float2(d0[4 * j], d0[4 * j + 1]);
+      *reinterpret_cast<float2*>(stg + (r0 + 8) * la.stg_ld + 8 * j + cq) = make_float2(d0[4 * j + 2], d0[4 * j + 3]);
+    }
+    if constexpr (W1 > 0) {
+#pragma unroll
+      for (int j = 0; j < W1 / 8; ++j) {
+        *reinterpret_cast<float2*>(stg + r0 * la.stg_ld + W0 + 8 * j + cq) = make_float2(d1[4 * j], d1[4 * j + 1]);
+        *reinterpret_cast<float2*>(stg + (r0 + 8) * la.stg_ld + W0 + 8 * j + cq) = make_float2(d1[4 * j + 2], d1[4 * j + 3]);
+      }
+    }
   }
-  tmem_st_wait();
-  tc_fence_before();
-  __syncwarp();
-  if ((threadIdx.x & 31) == 0) {  // one arrival per warp: the barriers count warps
-    mbar_arrive(&bar_ar[0]);
-    mbar_arrive(&bar_ar[1]);
+  return (uint32_t)stage | (phase << 16);
+}
+
+// layer width -> register chunks: up to 128 columns in one, wider layers as 128 + the rest (np <= 256, multiple of 16)
+template <int ACT>
+__device__ __forceinline__ uint32_t run_layer(const LayerArgs& la, uint32_t ring_pos, uint64_t* bar_full, uint64_t* bar_empty) {
+  switch (la.np) {
+#define TC_W(N0, N1) \
+  case N0 + N1: return wg_layer<ACT, N0, N1>(la, ring_pos, bar_full, bar_empty);
+    TC_W(16, 0) TC_W(32, 0) TC_W(48, 0) TC_W(64, 0) TC_W(80, 0) TC_W(96, 0) TC_W(112, 0) TC_W(128, 0)
+    TC_W(128, 16) TC_W(128, 32) TC_W(128, 48) TC_W(128, 64) TC_W(128, 80) TC_W(128, 96) TC_W(128, 112) TC_W(128, 128)
+#undef TC_W
+    default: __trap();  // tc_make_plan admits multiples of 16 up to 256 only
   }
+  return ring_pos;
 }
 
 // Actions of (sequence n, step t) drawn from the CEM sampling distribution with exactly the Philox keying of
@@ -263,83 +337,47 @@ static __device__ __noinline__ void cem_tail_refit(const TailArgs* ap, int dims,
   }
 }
 
-// CS = column splits of the epilogue: 4 * CS epilogue warps; warp (q, cs) owns TMEM lane quadrant q (rows
-// 32q..32q+31) and every CS-th 16-column chunk.  Thread (row i, cs == 0) also owns the row's scalar state.
-//
-// Data flow of one layer (v3): the A operand (activations, bf16 pairs) lives in TMEM, written by the epilogue with
-// tcgen05.st and consumed by tcgen05.mma in its A-from-TMEM form; weights stream through the shared-memory ring.
-// Hidden layers are split in two N halves so that the epilogue of half 0 runs under the MMAs of half 1, and the next
-// layer's first K steps (which only read half 0's activations) run under the epilogue of half 1:
-//
-//   (width 208 = 13 chunks of 16 columns; half 0 = 8 chunks = 128 columns, half 1 = 5 chunks incl. the short tail chunk)
-//   MMA   : [l.h0 K0-7][l.h0 K8-12] [l.h1 K0-12]        [l+1.h0 K0-7] ..wait.. [l+1.h0 K8-12][l+1.h1 ...
-//   EPI   :                         [epi l.h0 -> A' cols 0-127]  [epi l.h1 -> A' cols 128-207]  [epi l+1.h0 ...
-// An MMA costs max(65, N / 2) cycles per K step (profiles/r2_umma_issue_rate_ts.txt): 128 + 80 columns is the cheapest
-// two-way split, and finer splits / per-round issue schedules measured slower (DESIGN.md section 4, wip/0003).
-//
-// TMEM columns: [0, 256) accumulators (hidden: halves at 0 and h0n; output layer at 0), [256, 384) and [384, 512)
-// the two activation buffers (layer g reads buffer g & 1 and its epilogue writes buffer (g + 1) & 1).
-template <int ACT, int CS, bool CEMF, bool TL, bool EXP = false>  // EXP: propagation "expectation" (member passes); its own
-                                                // instantiation -- compiled into the production kernel it cost 64 B of spills
+template <int ACT, bool CEMF, bool EXP = false>  // EXP: propagation "expectation" (member passes)
                                                 // CEMF: fused-CEM features compiled in (in-kernel sampling, last-CTA refit)
-                                                // TL: clock64 stamps (b200pets_debug_timeline); compiled out of production kernels --
-                                                // even predicated-off stamps cost issue slots in the issue-bound end-of-step phase
-__global__ void __launch_bounds__(64 + 128 * CS, 1)
+__global__ void __launch_bounds__(kThreads, 1)
 rollout_tc_kernel(const __grid_constant__ ModelDev m, const __grid_constant__ RolloutArgs a, const __grid_constant__ TcPlan p,
                   const long long num_tiles) {
-  constexpr int kEpiThreads = 128 * CS;
-  long long* const tl = TL ? a.timeline : nullptr;
-  constexpr int kThreadsAll = 64 + kEpiThreads;
   extern __shared__ __align__(128) uint8_t smem[];
   uint8_t* ring = smem + p.off_ring;
   float* obs_s = reinterpret_cast<float*>(smem + p.off_obs);
   float* act_s = reinterpret_cast<float*>(smem + p.off_act);
   float2* c_norm = reinterpret_cast<float2*>(smem + p.off_const);  // [Kp0] {mean, 1/std}; (0, 1) past the real inputs
-  float* tail_s = reinterpret_cast<float*>(smem + p.off_tail);      // [128][tail_ld]: operand columns Dp .. Kp0-1 per row
-  // per-output constants of the output-layer epilogue, one 16-byte load per output (padded to a multiple of 4 outputs):
+  // per-output constants of the output-layer maths, one 16-byte load per output (padded to a multiple of 4 outputs):
   //   x = max_logvar * log2(e), y = exp(max_logvar - min_logvar), z = exp(min_logvar / 2), w = 1 if the prediction is a
   //   delta to add to the old observation (0: keep the raw prediction -- no_delta columns, the learned-reward column, pad)
   const int outq = (m.out + 3) & ~3;
   float4* c_out = reinterpret_cast<float4*>(smem + p.off_cout);
   uint64_t* bar_full = reinterpret_cast<uint64_t*>(smem + p.off_bar);
   uint64_t* bar_empty = bar_full + kMaxStages;
-  uint64_t* bar_ar = bar_empty + kMaxStages;  // [2] activations of half h written (count: epilogue warps)
-  uint64_t* bar_acc = bar_ar + 2;             // [2] accumulator of half h complete (tcgen05.commit)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar_acc + 2);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int S = p.nstages;
   // Programmatic dependent launch (common.cuh): let the next kernel of the chain become resident now; everything up
-  // to the pdl_wait() below (barriers, TMEM, constant tables, the producer's first weight copies) reads only the
-  // staged model, which no kernel of a plan writes.
+  // to the pdl_wait() below (barriers, constant tables, the producer's first weight copies) reads only the staged
+  // model, which no kernel of a plan writes.
   pdl_trigger();
   if (CEMF) pdl_wait();  // the fused-CEM variants stage the sampling distribution in their prologue
-  if (tl && threadIdx.x == 64 && (blockIdx.x == 0 || blockIdx.x == 40)) {
-    long long gt;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt));
-    tl[256 + (blockIdx.x ? 8 : 0) + 0] = clock64();  // kernel entry (cycles), wall clock (ns)
-    tl[256 + (blockIdx.x ? 8 : 0) + 1] = gt;
-  }
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < S; ++s) {
       mbar_init(&bar_full[s], 1);
-      mbar_init(&bar_empty[s], 1);
+      mbar_init(&bar_empty[s], 8);  // one arrival per consumer warp
     }
-    mbar_init(&bar_ar[0], kEpiThreads / 32);  // one arrival per epilogue warp
-    mbar_init(&bar_ar[1], kEpiThreads / 32);
-    mbar_init(&bar_acc[0], 1);
-    mbar_init(&bar_acc[1], 1);
     mbar_fence_init();
   }
-  for (int j = threadIdx.x; j < m.Kp[0]; j += kThreadsAll)
+  for (int j = threadIdx.x; j < m.Kp[0]; j += kThreads)
     c_norm[j] = (j < m.in && m.norm_mode) ? make_float2(m.norm_mean_f[j], m.norm_istd_f[j]) : make_float2(0.f, 1.f);
-  // logvar clamp folded into two per-output constants (see the output-layer epilogue):
+  // logvar clamp folded into two per-output constants (see the output-layer maths):
   //   var = exp(min + softplus(max - softplus(max - lv) - min)) = exp(min) * (1 + exp(max - min) / (1 + exp(max - lv)))
   // [2][kCemTabDims]: sampling mean, sqrt(constrained variance): behind the weight ring, allocated for fused-CEM launches only
   float* cem_tab = reinterpret_cast<float*>(smem + p.smem_bytes);
   __shared__ int sh_tail[2];
-  for (int j = threadIdx.x; j < outq; j += kThreadsAll) {
+  for (int j = threadIdx.x; j < outq; j += kThreads) {
     const bool real = j < m.out;
     const float mn = (m.deterministic || !real) ? 0.f : m.min_lv[j], mx = (m.deterministic || !real) ? 0.f : m.max_lv[j];
     const bool delta = real && j < m.D && m.target_is_delta && !m.no_delta[j];
@@ -347,7 +385,7 @@ rollout_tc_kernel(const __grid_constant__ ModelDev m, const __grid_constant__ Ro
   }
   const int cem_dims = a.H * m.A;
   if (CEMF && a.cem_mu) {
-    for (int d = threadIdx.x; d < cem_dims; d += kThreadsAll) {
+    for (int d = threadIdx.x; d < cem_dims; d += kThreads) {
       const float mu = a.cem_mu[d], dp = a.cem_disp[d];
       float sd = dp;
       if (!a.cem_clipped) {  // trajectory_opt.py:122-125
@@ -358,11 +396,7 @@ rollout_tc_kernel(const __grid_constant__ ModelDev m, const __grid_constant__ Ro
       cem_tab[kCemTabDims + d] = sd;
     }
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   // propagation "expectation" (gaussian_mlp.py:213-215): every row through every member, mean and clamped logvar averaged
   // over the members: `passes` = M forward passes per horizon step over the same layer-0 operand, member = pass
@@ -373,14 +407,9 @@ rollout_tc_kernel(const __grid_constant__ ModelDev m, const __grid_constant__ Ro
   const long long Bm = shuffle ? 0 : (expect ? a.B : a.B / m.M);
   const int tpm = shuffle ? 1 : (int)((Bm + kTileM - 1) / kTileM);
   const int nlayers = p.nlayers;
-  const int L = nlayers - 1;         // index of the output layer
-  const int NpH = m.Np[0];           // padded hidden width
-  const int h0n = p.h0n;             // columns of N half 0 (multiple of 16)
-  const int c0 = h0n >> 4;           // 16-column chunks (= K steps of the next layer) in half 0
-  const int NpF = m.Np[L];
-  const bool final_early = NpF <= h0n;  // output accumulator fits in half 0's columns: may start under epilogue h1
+  const int L = nlayers - 1;  // index of the output layer
 
-  if (warp == 0) {
+  if (warp == 8) {
     // =========================== weight producer ===========================
     if (lane == 0) {
       int stage = 0;
@@ -392,142 +421,70 @@ rollout_tc_kernel(const __grid_constant__ ModelDev m, const __grid_constant__ Ro
           const int mem = expect ? pass : (shuffle ? shuffle_member(a.seed, a.offset, a.slot_mode, shuffle_global_group(geom, tile), t, m.M) : member);
           const uint8_t* base = m.img + (size_t)(blockIdx.x % m.img_replicas) * m.img_replica_stride + (size_t)mem * m.img_member_stride;
           for (int l = 0; l < nlayers; ++l) {
-            // one ring slot holds the whole layer image (K core columns contiguous): one barrier, one wait per layer
+            // K steps are contiguous in the image (16 rows x Np columns each): a slice is one bulk copy
             const uint8_t* lsrc = base + m.img_layer_off[l];
-            const uint32_t bytes = (uint32_t)m.Kp[l] * m.Np[l] * 2u;
-            mbar_wait(&bar_empty[stage], phase ^ 1u);
-            mbar_arrive_expect_tx(&bar_full[stage], bytes);
-            uint8_t* dst = ring + (size_t)stage * p.stage_bytes;
-            const uint32_t piece = ((bytes / 4u) + 127u) & ~127u;  // four copies in flight
-            for (uint32_t off = 0; off < bytes; off += piece)
-              bulk_g2s(dst + off, lsrc + off, min(piece, bytes - off), &bar_full[stage]);
-            if (++stage == S) { stage = 0; phase ^= 1u; }
+            const int nk = m.Kp[l] >> 4;
+            const uint32_t kstep = (uint32_t)m.Np[l] * 32u;
+            for (int k0 = 0; k0 < nk; k0 += p.kslice) {
+              const uint32_t bytes = (uint32_t)(min(nk, k0 + p.kslice) - k0) * kstep;
+              mbar_wait(&bar_empty[stage], phase ^ 1u);
+              mbar_arrive_expect_tx(&bar_full[stage], bytes);
+              bulk_g2s(ring + (size_t)stage * p.slot_bytes, lsrc + (size_t)k0 * kstep, bytes, &bar_full[stage]);
+              if (++stage == S) { stage = 0; phase ^= 1u; }
+            }
           }
         }
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    // =========================== MMA issuer ===========================
-    // The whole warp runs the control flow converged (waits are uniform); the MMAs and commits are issued by the one
-    // elected lane, always the same one, so that every tcgen05.commit tracks all MMAs issued before it.
-    {
-      int stage = 0;
-      uint32_t phase = 0, ar_par = 0;
-      uint32_t g = 0;  // global layer counter: selects the activation buffer
-      const uint32_t ring_addr = smem_u32(ring);
-      for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        for (int tp = (a.t1 - a.t0) * passes; tp > 0; --tp) {
-          const int t = a.t1 - (tp + passes - 1) / passes;  // (only the timeline stamps look at it)
-          for (int l = 0; l < nlayers; ++l, ++g) {
-            const bool stamp = tl && lane == 0 && blockIdx.x == 0 && t == a.t0 + 5 && tile == blockIdx.x;
-            const int nk = m.Kp[l] >> 4;
-            const bool hidden = l < L;
-            const uint32_t np = (uint32_t)m.Np[l];
-            const uint32_t b_lbo = np * 16u;
-            const uint32_t a_col = tmem_base + 256u + ((g & 1u) << 7);
-            const uint32_t slot_addr = ring_addr + (uint32_t)stage * p.stage_bytes;
-            const uint32_t slot_phase = phase;
-            uint64_t* slot_empty = &bar_empty[stage];
-            uint64_t* slot_full = &bar_full[stage];
-            if (++stage == S) { stage = 0; phase ^= 1u; }
-            const int n0 = hidden ? h0n : NpF;
-            const uint32_t idesc0 = umma_idesc_bf16_m128((uint32_t)n0);
-            const int ksplit = (l == 0) ? nk : min(nk, c0);  // K steps whose activations arrive with half 0
-            const uint64_t b_inc = (uint64_t)((2u * b_lbo) >> 4);  // descriptor start-address step per K step
-            if (stamp) tl[64 + l * 4 + 0] = clock64();
-            mbar_wait(slot_full, slot_phase);
-            mbar_wait(&bar_ar[0], ar_par);
-            if (!hidden && !final_early) mbar_wait(&bar_ar[1], ar_par);
-            tc_fence_after();
-            if (stamp) tl[64 + l * 4 + 1] = clock64();
-            uint64_t bdesc = umma_smem_desc(slot_addr, b_lbo, 128u);
-            if (elect_one()) {
-              uint64_t bd = bdesc;
-              uint32_t acol = a_col;
-              for (int kk = 0; kk < ksplit; ++kk) {
-                umma_bf16_ts(tmem_base, acol, bd, idesc0, kk != 0 ? 1u : 0u);
-                bd += b_inc;
-                acol += 8u;
-              }
-            }
-            __syncwarp();
-            if (hidden || final_early) {
-              mbar_wait(&bar_ar[1], ar_par);
-              tc_fence_after();
-            }
-            if (stamp) tl[64 + l * 4 + 2] = clock64();
-            if (elect_one()) {
-              uint64_t bd = bdesc + (uint64_t)ksplit * b_inc;
-              uint32_t acol = a_col + 8u * (uint32_t)ksplit;
-              for (int kk = ksplit; kk < nk; ++kk) {
-                umma_bf16_ts(tmem_base, acol, bd, idesc0, 1u);
-                bd += b_inc;
-                acol += 8u;
-              }
-              umma_commit(&bar_acc[0]);
-              if (hidden) {
-                const uint32_t idesc1 = umma_idesc_bf16_m128((uint32_t)(NpH - h0n));
-                bd = umma_smem_desc(slot_addr + (uint32_t)(h0n >> 3) * 128u, b_lbo, 128u);  // weight rows h0n..
-                acol = a_col;
-                const uint32_t d1 = tmem_base + (uint32_t)h0n;
-                for (int kk = 0; kk < nk; ++kk) {
-                  umma_bf16_ts(d1, acol, bd, idesc1, kk != 0 ? 1u : 0u);
-                  bd += b_inc;
-                  acol += 8u;
-                }
-                umma_commit(&bar_acc[1]);
-              }
-              umma_commit(slot_empty);
-            }
-            __syncwarp();
-            ar_par ^= 1u;
-            if (stamp) tl[64 + l * 4 + 3] = clock64();
-          }
-        }
-      }
-    }
   } else {
-    // =========================== epilogue ===========================
-    const int q = warp & 3;            // TMEM lane quadrant this warp may access (hardware: warp id % 4)
-    const int cs = (warp - 2) >> 2;    // column split
-    const int i = q * 32 + lane;       // tile row
-    const bool owner = cs == 0;                     // loads the row's observation / actions
-    const bool scorer = cs == (CS >= 3 ? 2 : 0);    // owns return / dead flag: scores reward + termination (a thread
-                                                    // with an idle gap after layer 1, not the action-loading one)
-    const uint32_t t_lane = tmem_base + ((uint32_t)(q * 32) << 16);
-    float* my_obs = obs_s + i * p.obs_ld;
-    // three action buffers indexed by step % 3: step t+1's actions are written while step t-1's are still being scored
-    auto act_buf = [&](int tt) { return act_s + (tt % 3) * (kTileM * p.act_ld) + i * p.act_ld; };
+    // =========================== consumer warpgroups ===========================
+    const int wg = warp >> 2;
+    const int wt = threadIdx.x & 127;
+    const int r = wt & 63, h = wt >> 6;  // row of the warpgroup, half of the row's work
+    const int i = wg * 64 + r;           // tile row
+    const bool owner = h == 0;           // the row's scalar state: observation / actions load, score, store
     const bool cem = CEMF && a.cem_mu != nullptr;
-    const bool sampler = cem && cs == (CS > 1 ? 1 : 0);  // the thread of this row that draws its sequence's actions
-    uint32_t acc0_par = 0, acc1_par = 0;
-    uint32_t g = 0;
+    const bool sampler = cem && h == 1;  // the thread of this row that draws its sequence's actions
+    uint8_t* abuf = smem + p.off_A + (size_t)wg * p.wg_bytes;
+    const float* stg = reinterpret_cast<const float*>(abuf) + r * p.stg_ld;  // this row's output accumulators
+    float* my_obs = obs_s + i * p.obs_ld;
+    float* my_act = act_s + i * p.act_ld;
     const int ngroups = (m.out + 3) >> 2;
     const bool draw = !m.deterministic && a.sample;
-    // scoring of step t may be deferred into the gap after hidden layer 2 of step t + 1 only if another hidden layer
-    // follows that gap: the output-layer epilogue (which overwrites obs / learned reward) then needs this thread first
-    const bool defer_score = L >= 4 && !expect;
-    auto epi_bar = [&]() { asm volatile("bar.sync 1, %0;" ::"n"(kEpiThreads) : "memory"); };
+    const int Kp0 = m.Kp[0];
+    LayerArgs la;
+    la.a_addr = smem_u32(abuf);
+    la.a_ptr = abuf;
+    la.ring_addr = smem_u32(ring);
+    la.slot_bytes = p.slot_bytes;
+    la.nstages = S;
+    la.kslice = p.kslice;
+    la.stg_ld = p.stg_ld;
+    la.leaky = m.leaky;
+    uint32_t ring_pos = 0;
 
-    const InDims in_dims{m.Kp[0], m.D, m.Dp, m.A, m.in, m.obs_process};
-    float* my_tail = tail_s + i * p.tail_ld;  // [act (A) | 1 | 1 | 0 ..]: written with the actions of the step to be built
-    auto build_input = [&](int) {
-      build_input_tmem(in_dims, my_obs, my_tail, c_norm, t_lane + 256u + ((g & 1u) << 7), cs,
-                       CS, bar_ar);
+    // layer-0 operand of one step: normalise(cat(proc(obs), act)), two constant-one bias columns, zero pad; the two
+    // threads of a row take alternate column pairs
+    auto build_input = [&]() {
+      for (int jp = h; jp < (Kp0 >> 1); jp += 2) {
+        float x[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int j = 2 * jp + e;
+          float raw;
+          if (j < m.Dp) raw = m.obs_process == B200PETS_PROC_NONE ? my_obs[j] : proc_obs_elem(my_obs, j, m.obs_process);
+          else if (j < m.Dp + m.A) raw = my_act[j - m.Dp];
+          else raw = j < m.Dp + m.A + 2 ? 1.f : 0.f;
+          const float2 nm = c_norm[j];
+          x[e] = (raw - nm.x) * nm.y;
+        }
+        *reinterpret_cast<uint32_t*>(abuf + a_off(r, 2 * jp)) = pack_bf16(x[0], x[1]);
+      }
+      fence_proxy_async_smem();
+      wg_bar(wg);
     };
 
-    // tail chunk of a hidden layer's activations: columns [16 c_tail, Kp) = (hid % 16) real ones, the two bias ones, zero pad
-    const int c_tail = (NpH >> 4) - 1;
-    const int hid_true = m.N[0];
-    const bool fast_tail = L >= 1 && CS == 4 && hid_true - 16 * c_tail == 8 && hid_true >= m.Kp[0];  // (layer-0 operand words stay below)
-    if (fast_tail && cs == 0) {  // tail_const_init: words [hid / 2, Np / 2) of both activation buffers = {1 1}, 0, 0, 0
-      const uint32_t kc[4] = {0x3F803F80u, 0u, 0u, 0u};
-      tmem_st4(t_lane + 256u + (uint32_t)(hid_true >> 1), kc);
-      tmem_st4(t_lane + 384u + (uint32_t)(hid_true >> 1), kc);
-      tmem_st_wait();
-      tc_fence_before();
-    }
     pdl_wait();  // actions / observation / row state are the previous kernels' outputs; ours are written after this
     for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       bool valid;
@@ -545,379 +502,150 @@ rollout_tc_kernel(const __grid_constant__ ModelDev m, const __grid_constant__ Ro
       }
       float tot = 0.f;
       int dead = 0;
-      // reward_fn(act_t, obs_{t+1}), termination, dead mask, accumulate (model_env.py:124-129, 186-188): row owner only
-      auto score = [&](int ts) {
-        const float* arow = act_buf(ts);
-        // model_env.py:124-128: pred_rewards only when reward_fn is None, an explicit reward_fn always wins
-        float rew = m.reward_fn == B200PETS_REWARD_LEARNED ? my_obs[m.D] : reward_eval(m.reward_fn, arow, m.A, 1, my_obs, m.D, 1);
-        const bool done = term_eval(m.term_fn, my_obs, m.D, 1);
-        if (valid) {
-          if (a.reward_out) a.reward_out[rid] = rew;
-          if (a.done_out) a.done_out[rid] = done ? 1 : 0;
-        }
-        if (dead) rew = 0.f;
-        dead |= done ? 1 : 0;
-        tot += rew;
-      };
       const float* act_row = cem ? nullptr : a.act + (rid / a.act_div) * a.act_row_stride;
       const int seq_n = (int)(rid / a.P);
       float* pop_row = (cem && a.pop_out && valid && rid % a.P == 0) ? a.pop_out + (size_t)seq_n * cem_dims : nullptr;  // in-kernel draw only
-      const bool act_regs = m.A <= 8 && !cem;  // next-step actions prefetched into registers (hidden behind the layers)
-      float an[8];
-      epi_bar();  // previous tile fully consumed before its row state is overwritten
-      if (scorer && a.load_state && valid) {
-        tot = a.total_state[rid];
-        dead = a.dead_state[rid];
-      }
+      // this step's actions into the row's action words: from the action tensor, or drawn in-kernel (fused CEM)
+      auto load_actions = [&](int t) {
+        if (owner && !cem) {
+          const float* ap = act_row + (long long)t * a.act_t_stride;
+#pragma unroll 1
+          for (int j = 0; j < m.A; ++j) my_act[j] = valid ? ap[j] : 0.f;
+        }
+        if (CEMF && sampler)
+          cem_sample_actions(a.seed, a.cem_offset, a.cem_clipped, a.cem_lb, a.cem_ub, cem_tab, cem_tab + kCemTabDims, a.seq0 + seq_n,
+                             t, m.A, my_act, pop_row);
+      };
+      wg_bar(wg);  // previous tile fully consumed before its row state is overwritten
       if (owner) {
+        if (a.load_state && valid) {
+          tot = a.total_state[rid];
+          dead = a.dead_state[rid];
+        }
 #pragma unroll 1
         for (int d = 0; d < m.D; ++d) {
           float v = 0.f;
           if (valid) v = a.init_from_obs0 ? a.obs0[d] : a.obs_in[rid * m.D + d];
           my_obs[d] = v;
         }
-        if (!cem) {
-          const float* ap = act_row + (long long)a.t0 * a.act_t_stride;
-          float* arow = act_buf(a.t0);
-#pragma unroll 1
-          for (int j = 0; j < m.A; ++j) {
-            const float v = valid ? ap[j] : 0.f;
-            arow[j] = v;
-            my_tail[j] = v;
-          }
-        }
-#pragma unroll 1
-        for (int j = m.A; j < in_dims.Kp0 - m.Dp; ++j) my_tail[j] = j < m.A + 2 ? 1.f : 0.f;  // bias ones, zero pad
       }
-      if (CEMF && sampler) cem_sample_actions(a.seed, a.cem_offset, a.cem_clipped, a.cem_lb, a.cem_ub, cem_tab, cem_tab + kCemTabDims, a.seq0 + seq_n, a.t0, m.A,
-                                      act_buf(a.t0), pop_row);
-      if (CEMF && sampler)
-        for (int j = 0; j < m.A; ++j) my_tail[j] = act_buf(a.t0)[j];
-      epi_bar();
-      build_input(a.t0);
+      load_actions(a.t0);
+      wg_bar(wg);
 
       for (int t = a.t0; t < a.t1; ++t) {
-        const bool stamp = tl && blockIdx.x == 0 && warp == 2 && lane == 0 && t == a.t0 + 5 && tile == blockIdx.x;
-        int sp = 0;
-        if (stamp) tl[sp++] = clock64();  // 0: step start (layer-0 operand already handed over)
-        if (tl && warp == 2 && lane == 0 && tile == blockIdx.x && (blockIdx.x == 0 || blockIdx.x == 40) && t - a.t0 < 60)
-          tl[128 + (blockIdx.x ? 64 : 0) + (t - a.t0)] = clock64();  // coarse: every step start of two CTAs
-        const bool more = t + 1 < a.t1;
-        if (owner && act_regs && more) {  // global loads complete under the layers (not in fused-CEM mode)
-          const float* ap = act_row + (long long)(t + 1) * a.act_t_stride;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) an[j] = (valid && j < m.A) ? ap[j] : 0.f;
-        }
-        float zpre0[4] = {0.f, 0.f, 0.f, 0.f}, zpre1[4] = {0.f, 0.f, 0.f, 0.f};  // statically indexed: registers
-
-        // propagation "expectation": one forward pass per member over the same layer-0 operand; everything that belongs to
-        // the step and not to a member (noise draw, action hand-over, state update, scoring) happens in the first / last pass
         for (int pass = 0; pass < passes; ++pass) {
-        const bool last_pass = pass == passes - 1;
-        // ---- hidden layers: accumulator half -> activation -> bf16 pairs -> next layer's A operand in TMEM ----
-        for (int l = 0; l < L; ++l, ++g) {
-          const int n_true = m.N[l];
-          const int kp_next = m.Kp[l + 1];
-          const uint32_t a_out = t_lane + 256u + (((g + 1u) & 1u) << 7);
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            if (h == 0) {
-              if (TL && tl && lane == 0 && blockIdx.x == 0 && t == a.t0 + 5 && tile == blockIdx.x) tl[400 + (warp - 2) * 16 + l * 4 + 1] = clock64();
-              mbar_wait(&bar_acc[0], acc0_par);
-              acc0_par ^= 1u;
-              if (TL && tl && lane == 0 && blockIdx.x == 0 && t == a.t0 + 5 && tile == blockIdx.x) tl[400 + (warp - 2) * 16 + l * 4 + 2] = clock64();
-            } else {
-              mbar_wait(&bar_acc[1], acc1_par);
-              acc1_par ^= 1u;
-            }
-            tc_fence_after();
-            if (stamp) tl[sp++] = clock64();  // accumulator half ready
-            const int cbeg = h == 0 ? 0 : c0;
-            const int cend = h == 0 ? c0 : (kp_next >> 4);
-            const int cend_whole = (fast_tail && h == 1) ? c_tail : cend;  // the tail chunk has its own fast form below
-            for (int c = cbeg + cs; c < cend_whole; c += CS) {
-              float v[16];
-              if (16 * c < NpH) {
-                uint32_t r[16];
-                tmem_ld16(t_lane + (uint32_t)(16 * c), r);
-                tmem_ld_wait();
-#pragma unroll
-                for (int e = 0; e < 16; ++e) v[e] = act_tc<ACT>(__uint_as_float(r[e]), m.leaky);
-              } else {
-#pragma unroll
-                for (int e = 0; e < 16; ++e) v[e] = 0.f;
-              }
-              if (16 * c + 15 >= n_true && 16 * c <= n_true + 1) {
-#pragma unroll
-                for (int e = 0; e < 16; ++e) {
-                  const int col = 16 * c + e;
-                  if (col == n_true || col == n_true + 1) v[e] = 1.f;
-                }
-              }
-              uint32_t pk[8];
-#pragma unroll
-              for (int e = 0; e < 8; ++e) pk[e] = pack_bf16(v[2 * e], v[2 * e + 1]);
-              tmem_st8(a_out + (uint32_t)(8 * c), pk);
-            }
-            if (fast_tail && h == 1) {
-              // Tail chunk, fast form: only its 8 real columns are activated and stored.  The two bias-one columns and the zero
-              // pad behind them sit in activation words that no layer ever changes: written once per CTA (tail_const_init).
-              // The generic form (the `col == n_true` selects above) costs ~800 cycles more per layer: 32 compare + select
-              // pairs chained through three predicate registers on the one warp whose arrival the next layer's MMAs wait
-              // for (profiles/r2_timeline_per_warp.txt).
-              if (p.tail_split) {  // two columns per column-split warp: tcgen05.ld.x2, 2 MUFU, one packed word
-                uint32_t r2[2];
-                tmem_ld2(t_lane + (uint32_t)(16 * c_tail + 2 * cs), r2);
-                tmem_ld_wait();
-                tmem_st1(a_out + (uint32_t)(8 * c_tail + cs),
-                         pack_bf16(act_tc<ACT>(__uint_as_float(r2[0]), m.leaky), act_tc<ACT>(__uint_as_float(r2[1]), m.leaky)));
-              } else if (cs == (c_tail - cbeg) % CS) {  // the warp whose turn it is: tcgen05.ld.x8, 8 MUFU, tcgen05.st.x4
-                uint32_t r8[8];
-                tmem_ld8(t_lane + (uint32_t)(16 * c_tail), r8);
-                tmem_ld_wait();
-                uint32_t pk4[4];
-#pragma unroll
-                for (int e = 0; e < 4; ++e)
-                  pk4[e] = pack_bf16(act_tc<ACT>(__uint_as_float(r8[2 * e]), m.leaky), act_tc<ACT>(__uint_as_float(r8[2 * e + 1]), m.leaky));
-                tmem_st4(a_out + (uint32_t)(8 * c_tail), pk4);
-              }
-            }
-            tmem_st_wait();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&bar_ar[h]);
-            if (TL && tl && lane == 0 && blockIdx.x == 0 && t == a.t0 + 5 && tile == blockIdx.x) tl[400 + (warp - 2) * 16 + l * 4 + (h == 0 ? 3 : 0)] = clock64();
-            if (stamp) tl[sp++] = clock64();  // activations of this half written
+          const bool last_pass = pass == passes - 1;
+          build_input();
+          for (int l = 0; l < nlayers; ++l) {
+            la.nk = m.Kp[l] >> 4;
+            la.np = m.Np[l];
+            la.mode = l < L ? 0 : 1;
+            la.n_true = m.N[l];
+            la.kp_next = l < L ? m.Kp[l + 1] : 0;
+            ring_pos = run_layer<ACT>(la, ring_pos, bar_full, bar_empty);
+            wg_bar(wg);  // hidden: next layer's operand complete; output: staged accumulators complete
           }
-          // ---- side work in the gap while the next layer's first accumulator half completes ----
-          if (l < 2) {  // this step's model noise: Philox + Box-Muller for output group g0 + l * CS
-            // (measured: spreading the four warps' draws over more gaps, two per gap, made the step 2 % slower -- the second
-            //  gap then holds two draws plus nothing to hide them under; profiles/README.md)
-            const int gq = (CS - 1 - cs) + l * CS;
-            if (pass == 0 && draw && !a.eps && gq < ngroups) {
-              float z4[4];
-              philox_normal4((uint32_t)rid_glob, (uint32_t)t, RNG_STREAM_EPS | (uint32_t)gq, (uint32_t)a.offset, a.seed, z4);
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                if (l == 0) zpre0[e] = z4[e];
-                else zpre1[e] = z4[e];
-              }
-            }
-            // previous step's reward / termination, off the critical path (the scorer thread has no noise group here)
-            if (l == 1 && scorer && t > a.t0 && defer_score) score(t - 1);
-            // fused CEM: next step's actions are drawn here by the row's sampler thread (third action buffer)
-            if (CEMF && l == (L > 1 ? 1 : 0) && sampler && more && last_pass)
-              cem_sample_actions(a.seed, a.cem_offset, a.cem_clipped, a.cem_lb, a.cem_ub, cem_tab, cem_tab + kCemTabDims, a.seq0 + seq_n, t + 1,
-                                 m.A, act_buf(t + 1), pop_row);
-            if (CEMF && l == (L > 1 ? 1 : 0) && sampler && more && last_pass)
-              for (int j = 0; j < m.A; ++j) my_tail[j] = act_buf(t + 1)[j];
-          } else if (l == 2 && owner && !cem && last_pass) {  // (earlier passes still need this step's actions in the tail)
-            if (!more) continue;
-            // next step's actions -> the other action buffer (the one score(t - 1) just finished reading)
-            float* arow = act_buf(t + 1);
-            if (act_regs) {
-#pragma unroll
-              for (int j = 0; j < 8; ++j)
-                if (j < m.A) {
-                  arow[j] = an[j];
-                  my_tail[j] = an[j];
-                }
-            } else {
-              const float* ap = act_row + (long long)(t + 1) * a.act_t_stride;
-      #pragma unroll 1
-        for (int j = 0; j < m.A; ++j) {
-                const float v = valid ? ap[j] : 0.f;
-                arow[j] = v;
-                my_tail[j] = v;
-              }
-            }
-          }
-        }
-        if (L < 3 && owner && more && !cem && last_pass) {  // shallow models: the action hand-over did not fit in a gap above
-          float* arow = act_buf(t + 1);
-          const float* ap = act_row + (long long)(t + 1) * a.act_t_stride;
-#pragma unroll 1
-          for (int j = 0; j < m.A; ++j) arow[j] = valid ? ap[j] : 0.f;
-          // (shallow models never take the fused path: the generic builder runs after the end-of-step barrier, and the
-          //  tail still holds this step's actions until then -- it is refreshed right before that builder call)
-        }
-
-        // ---- output layer: groups of 4 outputs; Gaussian sample, delta add-back (branch-free inner maths) ----
-        mbar_wait(&bar_acc[0], acc0_par);
-        acc0_par ^= 1u;
-        ++g;
-        tc_fence_after();
-        if (stamp) tl[sp++] = clock64();  // output accumulator ready
-        // the column split with the most output groups (cs = CS - 1: groups 0, CS, ..) bounds the end-of-step barrier
-        const bool stamp3 = tl && blockIdx.x == 0 && warp == 2 + 4 * (CS - 1) && lane == 0 && t == a.t0 + 5 && tile == blockIdx.x;
-        if (stamp3) tl[56] = clock64();
-        // Slot gq = outputs [4 gq, 4 gq + 4) AND (fused mode) the next step's layer-0 operand columns [4 gq, 4 gq + 4).
-        // Without an observation pre-processor input column j < D IS output j, so the thread that samples an output
-        // also normalises it and writes it straight into the next step's A operand in TMEM (tcgen05.st.x2): no
-        // barrier and no separate input-build pass between two steps (they were ~1.3 k cycles of every step); slots past
-        // the outputs carry the action / bias-one / pad columns.  Pre-processed observations keep the generic builder.
-        // (L >= 4: the next step's actions, written in the gap after hidden layer 2, must be ordered before this point
-        //  by one more accumulator barrier -- the same condition that lets the score be deferred.)
-        const bool fuse_in = more && m.obs_process == B200PETS_PROC_NONE && defer_score;  // (never with "expectation")
-        const int nslots = fuse_in ? max(ngroups, in_dims.Kp0 >> 2) : ngroups;
-        const uint32_t a_next = t_lane + 256u + ((g & 1u) << 7);  // A buffer of the next step's layer 0 (g already advanced)
-        for (int gq = CS - 1 - cs; gq < nslots; gq += CS) {  // reversed: the row owner (cs 0) gets the fewest groups
-          const int u = (gq - (CS - 1 - cs)) / CS;
-          float nw[4] = {0.f, 0.f, 0.f, 0.f};
-          if (gq < ngroups) {
-          uint32_t rm[4], rl[4] = {0u, 0u, 0u, 0u};
-          tmem_ld4(t_lane + (uint32_t)(4 * gq), rm);
-          if (!m.deterministic) tmem_ld4(t_lane + (uint32_t)(m.outp + 4 * gq), rl);
-          tmem_ld_wait();
-          if (stamp) tl[40 + 4 * u] = clock64();
-          // "expectation": member sums of the mean and of log2(1 + e2) (the clamped logvar is min + ln(1 + e2), see below)
-          // in the row's scratch words; the last pass turns them into the averaged mean and sqrt(exp(averaged logvar))
-          float sdv[4] = {0.f, 0.f, 0.f, 0.f};
-          if (expect) {
-            float* exm = reinterpret_cast<float*>(smem + p.off_exp) + i * p.exp_ld + 4 * gq;
-            float* exl = exm + outq;
-            const float inv_m = 1.0f / (float)passes;
+          // ---- output layer: groups of 4 outputs, the two threads of a row take alternate groups; Gaussian sample,
+          //      delta add-back (branch-free inner maths) ----
+          for (int gq = h; gq < ngroups; gq += 2) {
+            float rm[4], rl[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
-              const float4 ce = c_out[4 * gq + e];
-              float l2 = 0.f;
-              if (draw) {
-                const float e1 = ex2_approx(fmaf(__uint_as_float(rl[e]), -1.4426950408889634f, ce.x));
-                l2 = lg2_approx(1.f + ce.y * rcp_approx(1.f + e1));
-              }
-              const float am = (pass ? exm[e] : 0.f) + __uint_as_float(rm[e]);
-              const float al = (pass ? exl[e] : 0.f) + l2;
-              exm[e] = am;
-              exl[e] = al;
-              rm[e] = __float_as_uint(am * inv_m);
-              sdv[e] = ce.z * ex2_approx(0.5f * al * inv_m);  // sqrt(exp(min + ln2 * mean_m log2(1 + e2)))
+              rm[e] = stg[4 * gq + e];
+              if (!m.deterministic) rl[e] = stg[m.outp + 4 * gq + e];
             }
-            if (!last_pass) continue;
-          }
-          // Branch-free per output: one 16-byte constant load, 3 MUFU (ex2, rcp, sqrt), one LDS + FADD/FSEL + STS of the state.
-          //   var = exp(min + softplus(max - softplus(max - lv) - min)) = e^min * (1 + e^(max-min) / (1 + e^(max-lv)))
-          //   (gaussian_mlp.py:150-153 folded into two per-output constants), pred = mean + sqrt(var) * z
-          //   (model.py:467-471), next = pred + keep * old (one_dim_tr_model.py:281-286).  Padded outputs (o >= out)
-          //   land in the row's padding words; the learned-reward column is word D of the row.
-          float z[4] = {0.f, 0.f, 0.f, 0.f};
-          if (draw) {
-            if (a.eps) {
+            // "expectation": member sums of the mean and of log2(1 + e2) (the clamped logvar is min + ln(1 + e2), see below)
+            // in the row's scratch words; the last pass turns them into the averaged mean and sqrt(exp(averaged logvar))
+            float sdv[4] = {0.f, 0.f, 0.f, 0.f};
+            if (expect) {
+              float* exm = reinterpret_cast<float*>(smem + p.off_exp) + i * p.exp_ld + 4 * gq;
+              float* exl = exm + outq;
+              const float inv_m = 1.0f / (float)passes;
 #pragma unroll
               for (int e = 0; e < 4; ++e) {
-                const int oc = min(4 * gq + e, m.out - 1);
-                z[e] = valid ? a.eps[((size_t)(t - a.t0) * a.B + rid) * m.out + oc] : 0.f;
+                const float4 ce = c_out[4 * gq + e];
+                float l2 = 0.f;
+                if (draw) {
+                  const float e1 = ex2_approx(fmaf(rl[e], -1.4426950408889634f, ce.x));
+                  l2 = lg2_approx(1.f + ce.y * rcp_approx(1.f + e1));
+                }
+                const float am = (pass ? exm[e] : 0.f) + rm[e];
+                const float al = (pass ? exl[e] : 0.f) + l2;
+                exm[e] = am;
+                exl[e] = al;
+                rm[e] = am * inv_m;
+                sdv[e] = ce.z * ex2_approx(0.5f * al * inv_m);  // sqrt(exp(min + ln2 * mean_m log2(1 + e2)))
               }
-            } else if (u < 2 && u < L) {
-#pragma unroll
-              for (int e = 0; e < 4; ++e) z[e] = u == 0 ? zpre0[e] : zpre1[e];
-            } else {
-              philox_normal4((uint32_t)rid_glob, (uint32_t)t, RNG_STREAM_EPS | (uint32_t)gq, (uint32_t)a.offset, a.seed, z);
+              if (!last_pass) continue;
             }
-          }
-          if (stamp) tl[41 + 4 * u] = clock64();
-          const float4* cg = c_out + 4 * gq;
-          float* og = my_obs + 4 * gq;
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {  // two outputs at a time: loads up front so that the two chains overlap
-            if (h == 1 && 4 * gq + 2 >= m.out) continue;  // pure padding pair (17 outputs: group 4 holds one real output)
-            const float4 c0 = cg[2 * h], c1 = cg[2 * h + 1];
-            const float o0 = og[2 * h], o1 = og[2 * h + 1];
-            float p0 = __uint_as_float(rm[2 * h]), p1 = __uint_as_float(rm[2 * h + 1]);
+            // Per output: one 16-byte constant load, 3 MUFU (ex2, rcp, sqrt), one LDS + FADD/FSEL + STS of the state.
+            //   var = exp(min + softplus(max - softplus(max - lv) - min)) = e^min * (1 + e^(max-min) / (1 + e^(max-lv)))
+            //   (gaussian_mlp.py:150-153 folded into two per-output constants), pred = mean + sqrt(var) * z
+            //   (model.py:467-471), next = pred + keep * old (one_dim_tr_model.py:281-286).  Padded outputs (o >= out)
+            //   land in the row's padding words; the learned-reward column is word D of the row.
+            float z[4] = {0.f, 0.f, 0.f, 0.f};
             if (draw) {
-              // exp(max - lv) (inf is fine); exp(max - min) / (1 + e1); sqrt(exp(clamped logvar))
-              const float e10 = ex2_approx(fmaf(__uint_as_float(rl[2 * h]), -1.4426950408889634f, c0.x));
-              const float e11 = ex2_approx(fmaf(__uint_as_float(rl[2 * h + 1]), -1.4426950408889634f, c1.x));
-              const float e20 = c0.y * rcp_approx(1.f + e10), e21 = c1.y * rcp_approx(1.f + e11);
-              const float sd0 = expect ? sdv[2 * h] : c0.z * sqrt_approx(1.f + e20), sd1 = expect ? sdv[2 * h + 1] : c1.z * sqrt_approx(1.f + e21);
-              p0 = fmaf(sd0, z[2 * h], p0);
-              p1 = fmaf(sd1, z[2 * h + 1], p1);
+              if (a.eps) {
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                  const int oc = min(4 * gq + e, m.out - 1);
+                  z[e] = valid ? a.eps[((size_t)(t - a.t0) * a.B + rid) * m.out + oc] : 0.f;
+                }
+              } else {
+                philox_normal4((uint32_t)rid_glob, (uint32_t)t, RNG_STREAM_EPS | (uint32_t)gq, (uint32_t)a.offset, a.seed, z);
+              }
             }
-            // a select, not old * 0: a stale Inf / NaN word must not leak
-            nw[2 * h] = c0.w != 0.f ? p0 + o0 : p0;
-            nw[2 * h + 1] = c1.w != 0.f ? p1 + o1 : p1;
-            og[2 * h] = nw[2 * h];
-            og[2 * h + 1] = nw[2 * h + 1];
-          }
-          if (stamp) tl[42 + 4 * u] = clock64();
-          }
-          if (fuse_in && 4 * gq < in_dims.Kp0) {  // next step's operand columns 4 gq .. 4 gq + 3
-            if (stamp) tl[43 + 4 * u] = clock64();
-            float x[4];
+            const float4* cg = c_out + 4 * gq;
+            float* og = my_obs + 4 * gq;
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
-              const int j = 4 * gq + e;
-              const float tv = my_tail[max(j - m.D, 0)];  // next step's actions / bias ones / pad (unused for j < D)
-              const float2 nm = c_norm[j];
-              x[e] = ((j < m.D ? nw[e] : tv) - nm.x) * nm.y;
+              const float4 ce = cg[e];
+              float pv = rm[e];
+              if (draw) {
+                // exp(max - lv) (inf is fine); exp(max - min) / (1 + e1); sqrt(exp(clamped logvar))
+                const float e1 = ex2_approx(fmaf(rl[e], -1.4426950408889634f, ce.x));
+                const float e2 = ce.y * rcp_approx(1.f + e1);
+                const float sd = expect ? sdv[e] : ce.z * sqrt_approx(1.f + e2);
+                pv = fmaf(sd, z[e], pv);
+              }
+              // a select, not old * 0: a stale Inf / NaN word must not leak
+              og[e] = ce.w != 0.f ? pv + og[e] : pv;
             }
-            uint32_t pk[2] = {pack_bf16(x[0], x[1]), pack_bf16(x[2], x[3])};
-            tmem_st2(a_next + (uint32_t)(2 * gq), pk);
-            if (stamp) tl[48 + u] = clock64();
           }
+          wg_bar(wg);  // the row's words are complete; the staging area may be overwritten by the next operand
         }
-        if (!last_pass) {  // next member: same observation, same actions, through the generic builder (it arrives on both barriers)
-          tc_fence_before();
-          build_input(t);
-          continue;
-        }
-        if (fuse_in) {  // hand the operand to the MMA warp: both halves' barriers, as build_input_tmem does
-          if (stamp) tl[52] = clock64();
-          tmem_st_wait();
-          if (stamp) tl[53] = clock64();
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) {
-            mbar_arrive(&bar_ar[0]);
-            mbar_arrive(&bar_ar[1]);
+        // ---- reward, termination, accumulate (model_env.py:124-129, 186-188) ----
+        if (owner) {
+          // model_env.py:124-128: pred_rewards only when reward_fn is None, an explicit reward_fn always wins
+          float rew = m.reward_fn == B200PETS_REWARD_LEARNED ? my_obs[m.D] : reward_eval(m.reward_fn, my_act, m.A, 1, my_obs, m.D, 1);
+          const bool done = term_eval(m.term_fn, my_obs, m.D, 1);
+          if (valid) {
+            if (a.reward_out) a.reward_out[rid] = rew;
+            if (a.done_out) a.done_out[rid] = done ? 1 : 0;
           }
-          if (stamp) tl[54] = clock64();
-        } else {
-          tc_fence_before();
+          if (dead) rew = 0.f;
+          dead |= done ? 1 : 0;
+          tot += rew;
         }
-        if (stamp) tl[sp++] = clock64();  // outputs sampled (fused mode: next input handed over)
-        if (stamp3) tl[57] = clock64();
-        const bool score_now = scorer && !(more && defer_score);
-        // the row's words are written by four warps: a barrier before anything reads the whole row (the generic input
-        // builder, an immediate score).  In fused mode with deferred scoring nothing does until the next step's gaps,
-        // which are ordered behind this point by the accumulator barriers.
-        if (!fuse_in || !(more && defer_score)) epi_bar();
-        if (stamp) tl[sp++] = clock64();  // barrier
-        if (more && !fuse_in) {  // generic path: next step's layer 0 starts while the owner scores this step
-          if (L < 3) {  // shallow models handed the actions over after the last gap: copy them behind the barrier
-            if (owner)
-              for (int j = 0; j < m.A; ++j) my_tail[j] = act_buf(t + 1)[j];
-            epi_bar();
-          }
-          build_input(t + 1);
+        if (t + 1 < a.t1) {
+          wg_bar(wg);  // the score has read this step's actions
+          load_actions(t + 1);
+          wg_bar(wg);  // both threads of a row build the next operand from the action words one of them wrote
         }
-        if (stamp) tl[sp++] = clock64();  // next input handed over
-        if (stamp3) tl[58] = clock64();
-        // ---- reward, termination, accumulate: deferred into a gap of the next step when the model is deep enough ----
-        if (score_now) score(t);
-        if (stamp) tl[sp++] = clock64();  // reward done
-        }  // passes
       }
       // ---- store row state ----
-      if (owner && a.store_state && valid && a.obs_out) {
+      if (owner && a.store_state && valid) {
+        if (a.obs_out) {
 #pragma unroll 1
-        for (int d = 0; d < m.D; ++d) a.obs_out[rid * m.D + d] = my_obs[d];
-      }
-      if (scorer && a.store_state && valid) {
+          for (int d = 0; d < m.D; ++d) a.obs_out[rid * m.D + d] = my_obs[d];
+        }
         if (a.total_state) a.total_state[rid] = tot;
         if (a.dead_state) a.dead_state[rid] = (uint8_t)dead;
       }
     }
   }
 
-  tc_fence_before();
   __syncthreads();
-  if (tl && threadIdx.x == 64 && (blockIdx.x == 0 || blockIdx.x == 40)) {
-    long long gt;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt));
-    tl[256 + (blockIdx.x ? 8 : 0) + 2] = clock64();  // all tiles of this CTA done
-    tl[256 + (blockIdx.x ? 8 : 0) + 3] = gt;
-  }
-  if (warp == 1) tmem_dealloc(tmem_base, 512);
   // ---- fused CEM iteration: the last CTA to get here refits the sampling distribution ----
   if (CEMF && a.tail_counter) {
     if (threadIdx.x == 0) {
@@ -942,329 +670,76 @@ rollout_tc_kernel(const __grid_constant__ ModelDev m, const __grid_constant__ Ro
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// self test: one 128 x n x k GEMM through the same operand layouts / descriptors
+// self test: one 128 x n x k GEMM through the rollout kernel's operand layouts, descriptors, weight ring and
+// accumulator fragments: one warpgroup, rows 0-63 then rows 64-127 through the same operand buffer.  a_pairs = 1 writes
+// A as bf16 pairs per thread and row, as the hidden-layer epilogue does; 0 as 16-byte core-matrix rows.
 // ---------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128, 1) umma_selftest_kernel(int k, int n, const float* __restrict__ A,
-                                                                const float* __restrict__ B, float* __restrict__ D) {
+__global__ void __launch_bounds__(128, 1) wgmma_selftest_kernel(int k, int n, int a_pairs, uint32_t wg_bytes, int stg_ld,
+                                                                const float* __restrict__ A, const float* __restrict__ B,
+                                                                float* __restrict__ D) {
   extern __shared__ __align__(128) uint8_t smem[];
-  uint8_t* A_s = smem;                       // 128 * k * 2
-  uint8_t* B_s = smem + 128 * k * 2;         // n * k * 2
-  uint64_t* bar = reinterpret_cast<uint64_t*>(B_s + n * k * 2);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar + 1);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  if (tid == 0) {
-    mbar_init(bar, 1);
-    mbar_fence_init();
-  }
-  // A: [128][k] row-major fp32 -> canonical bf16
-  for (int idx = tid; idx < 128 * (k / 8); idx += 128) {
-    int i = idx % 128, kc = idx / 128;
-    float x[8];
-    for (int e = 0; e < 8; ++e) x[e] = A[i * k + kc * 8 + e];
-    *reinterpret_cast<uint4*>(A_s + a_chunk_off(i, kc)) =
-        make_uint4(pack_bf16(x[0], x[1]), pack_bf16(x[2], x[3]), pack_bf16(x[4], x[5]), pack_bf16(x[6], x[7]));
-  }
-  // B: [n][k] row-major fp32 -> [kc][n / 8][n % 8][8]
-  for (int idx = tid; idx < n * (k / 8); idx += 128) {
-    int nn = idx % n, kc = idx / n;
-    float x[8];
-    for (int e = 0; e < 8; ++e) x[e] = B[nn * k + kc * 8 + e];
-    *reinterpret_cast<uint4*>(B_s + (size_t)(kc * (n / 8) + (nn >> 3)) * 128 + (nn & 7) * 16) =
-        make_uint4(pack_bf16(x[0], x[1]), pack_bf16(x[2], x[3]), pack_bf16(x[4], x[5]), pack_bf16(x[6], x[7]));
-  }
-  fence_proxy_async_smem();
-  if (warp == 0) tmem_alloc(tmem_slot, 256);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  if (tid == 0) {
-    const uint32_t idesc = umma_idesc_bf16_m128((uint32_t)n);
-    const uint32_t b_lbo = (uint32_t)n * 16u;
-    for (int kk = 0; kk < k / 16; ++kk) {
-      const uint64_t adesc = umma_smem_desc(smem_u32(A_s) + (uint32_t)(2 * kk) * 2048u, 2048u, 128u);
-      const uint64_t bdesc = umma_smem_desc(smem_u32(B_s) + (uint32_t)(2 * kk) * b_lbo, b_lbo, 128u);
-      umma_bf16_ss(tmem_base, adesc, bdesc, idesc, kk != 0 ? 1u : 0u);
-    }
-    umma_commit(bar);
-  }
-  __syncwarp();
-  mbar_wait(bar, 0);
-  tc_fence_after();
-  const int i = warp * 32 + lane;
-  for (int c = 0; c < n / 16; ++c) {
-    uint32_t r[16];
-    tmem_ld16(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(16 * c), r);
-    tmem_ld_wait();
-    for (int e = 0; e < 16; ++e) D[i * n + 16 * c + e] = __uint_as_float(r[e]);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_base, 256);
-}
-
-
-// self test of the A-from-TMEM form: the four warps write their rows of A (bf16 pairs) with tcgen05.st
-__global__ void __launch_bounds__(128, 1) umma_selftest_ts_kernel(int k, int n, const float* __restrict__ A,
-                                                                   const float* __restrict__ B, float* __restrict__ D) {
-  extern __shared__ __align__(128) uint8_t smem[];
-  uint8_t* B_s = smem;
-  uint64_t* bar = reinterpret_cast<uint64_t*>(B_s + n * k * 2);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar + 1);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  if (tid == 0) {
-    mbar_init(bar, 1);
-    mbar_fence_init();
-  }
-  for (int idx = tid; idx < n * (k / 8); idx += 128) {
-    int nn = idx % n, kc = idx / n;
-    float x[8];
-    for (int e = 0; e < 8; ++e) x[e] = B[nn * k + kc * 8 + e];
-    *reinterpret_cast<uint4*>(B_s + (size_t)(kc * (n / 8) + (nn >> 3)) * 128 + (nn & 7) * 16) =
-        make_uint4(pack_bf16(x[0], x[1]), pack_bf16(x[2], x[3]), pack_bf16(x[4], x[5]), pack_bf16(x[6], x[7]));
-  }
-  fence_proxy_async_smem();
-  if (warp == 0) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t a_col = 256;
-  const int i = warp * 32 + lane;
-  const uint32_t t_lane = tmem_base + ((uint32_t)(warp * 32) << 16);
-  for (int kk = 0; kk < k / 16; ++kk) {
-    uint32_t r[8];
-    for (int e = 0; e < 8; ++e) r[e] = pack_bf16(A[i * k + kk * 16 + 2 * e], A[i * k + kk * 16 + 2 * e + 1]);
-    tmem_st8(t_lane + a_col + (uint32_t)(8 * kk), r);
-  }
-  tmem_st_wait();
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (tid == 0) {
-    const uint32_t idesc = umma_idesc_bf16_m128((uint32_t)n);
-    const uint32_t b_lbo = (uint32_t)n * 16u;
-    for (int kk = 0; kk < k / 16; ++kk) {
-      const uint64_t bdesc = umma_smem_desc(smem_u32(B_s) + (uint32_t)(2 * kk) * b_lbo, b_lbo, 128u);
-      umma_bf16_ts(tmem_base, tmem_base + a_col + (uint32_t)(8 * kk), bdesc, idesc, kk != 0 ? 1u : 0u);
-    }
-    umma_commit(bar);
-  }
-  __syncwarp();
-  mbar_wait(bar, 0);
-  tc_fence_after();
-  for (int c = 0; c < n / 16; ++c) {
-    uint32_t r[16];
-    tmem_ld16(t_lane + (uint32_t)(16 * c), r);
-    tmem_ld_wait();
-    for (int e = 0; e < 16; ++e) D[i * n + 16 * c + e] = __uint_as_float(r[e]);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_base, 512);
-}
-
-// ---------------------------------------------------------------------------------------------------------
-// micro-benchmark: issue rate of back-to-back tcgen05.mma for different shared-memory operand layouts
-//   mode 0: no swizzle, K core columns strided (LBO = rows*16, SBO = 128)      <- layout of the rollout kernel
-//   mode 1: SWIZZLE_128B K-major (SBO = 1024, 32 B start-address advance per K step inside a 64-element block)
-//   mode 2: no swizzle, the two K halves of a row group adjacent (LBO = 128, SBO = (K/8)*128)
-// Data is whatever is in shared memory: timing only.
-// ---------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint64_t umma_smem_desc_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFFu);
-  d |= (uint64_t)1 << 16;                      // LBO (unused for swizzled K-major)
-  d |= (uint64_t)((1024u >> 4) & 0x3FFFu) << 32;  // SBO: 8 rows x 128 B
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;                      // SWIZZLE_128B
-  return d;
-}
-
-__global__ void __launch_bounds__(128, 1) umma_bench_kernel(int mode, int k, int n, int reps, long long* out) {
-  extern __shared__ __align__(128) uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* A_s = smem;
-  uint8_t* B_s = smem + 128 * 256 * 2;
-  __shared__ uint64_t bar;
-  __shared__ uint32_t tmem_slot;
-  const int tid = threadIdx.x, warp = tid >> 5;
-  for (int i = tid; i < (128 + 256) * 256 * 2 / 16; i += 128) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
+  uint8_t* B_s = smem + wg_bytes;  // laid out as the weight ring would hold it: slice s of kSliceK16 K steps in slot s
+  const int nsl = (k / 16 + kSliceK16 - 1) / kSliceK16;
+  uint64_t* bar_full = reinterpret_cast<uint64_t*>(B_s + (size_t)n * k * 2);  // [2][nsl]: one set per row half
+  uint64_t* bar_empty = bar_full + 2 * nsl;
+  const int tid = threadIdx.x;
   if (tid == 0) {
-    mbar_init(&bar, 1);
+    for (int s = 0; s < 2 * nsl; ++s) mbar_init(&bar_full[s], 1);
+    for (int s = 0; s < nsl; ++s) mbar_init(&bar_empty[s], 8);  // (nobody waits for the slots to be released)
     mbar_fence_init();
   }
-  fence_proxy_async_smem();
-  if (warp == 0) tmem_alloc(&tmem_slot, 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_slot;
-  if (tid == 0) {
-    const uint32_t idesc = umma_idesc_bf16_m128((uint32_t)n);
-    const uint32_t a0 = smem_u32(A_s), b0 = smem_u32(B_s);
-    long long t0 = clock64();
-    for (int r = 0; r < reps; ++r) {
-      for (int kk = 0; kk < (mode >= 3 ? 0 : k / 16); ++kk) {
-        uint64_t ad, bd;
-        if (mode == 0) {
-          ad = umma_smem_desc(a0 + (uint32_t)(2 * kk) * 2048u, 2048u, 128u);
-          bd = umma_smem_desc(b0 + (uint32_t)(2 * kk) * (uint32_t)n * 16u, (uint32_t)n * 16u, 128u);
-        } else if (mode == 1) {
-          ad = umma_smem_desc_sw128(a0 + (uint32_t)(kk >> 2) * 128u * 128u + (uint32_t)(kk & 3) * 32u);
-          bd = umma_smem_desc_sw128(b0 + (uint32_t)(kk >> 2) * (uint32_t)n * 128u + (uint32_t)(kk & 3) * 32u);
-        } else {
-          ad = umma_smem_desc(a0 + (uint32_t)kk * 256u, 128u, (uint32_t)(k / 8) * 128u);
-          bd = umma_smem_desc(b0 + (uint32_t)kk * 256u, 128u, (uint32_t)(k / 8) * 128u);
-        }
-        if (mode < 3) umma_bf16_ss(tmem_base, ad, bd, idesc, 1u);
+  // B: [n][k] row-major fp32 -> [k / 8][n / 8][n % 8][8]
+  for (int idx = tid; idx < n * (k / 8); idx += 128) {
+    int nn = idx % n, kc = idx / n;
+    float x[8];
+    for (int e = 0; e < 8; ++e) x[e] = B[nn * k + kc * 8 + e];
+    *reinterpret_cast<uint4*>(B_s + (size_t)(kc * (n / 8) + (nn >> 3)) * 128 + (nn & 7) * 16) =
+        make_uint4(pack_bf16(x[0], x[1]), pack_bf16(x[2], x[3]), pack_bf16(x[4], x[5]), pack_bf16(x[6], x[7]));
+  }
+  for (int half = 0; half < 2; ++half) {
+    // A: rows 64 half .. 64 half + 63 of [128][k] row-major fp32
+    if (a_pairs) {
+      for (int idx = tid; idx < 64 * (k / 2); idx += 128) {
+        const int r = idx & 63, c = 2 * (idx >> 6);
+        const float* src = A + (64 * half + r) * k + c;
+        *reinterpret_cast<uint32_t*>(A_s + a_off(r, c)) = pack_bf16(src[0], src[1]);
       }
-      if (mode == 4) {  // A-from-TMEM form (the rollout kernel's), tight issue loop
-        uint64_t bd = umma_smem_desc(b0, (uint32_t)n * 16u, 128u);
-        const uint64_t b_inc = (2u * (uint32_t)n * 16u) >> 4;
-        uint32_t acol = tmem_base + 256u;
-        const int nk = k / 16;
-        for (int kk = 0; kk < nk; ++kk) {
-          umma_bf16_ts(tmem_base, acol, bd, idesc, 1u);
-          acol += 8u;
-          bd += b_inc;
-        }
-      }
-      if (mode == 3) {  // tight issue: precomputed descriptors, start-address field advanced by a constant
-        uint64_t ad = umma_smem_desc(a0, 2048u, 128u), bd = umma_smem_desc(b0, (uint32_t)n * 16u, 128u);
-        const uint64_t a_inc = (2u * 2048u) >> 4, b_inc = (2u * (uint32_t)n * 16u) >> 4;
-        const int nk = k / 16;
-#pragma unroll 4
-        for (int kk = 0; kk < nk; ++kk) {
-          umma_bf16_ss(tmem_base, ad, bd, idesc, 1u);
-          ad += a_inc;
-          bd += b_inc;
-        }
+    } else {
+      for (int idx = tid; idx < 64 * (k / 8); idx += 128) {
+        const int r = idx & 63, kc = idx >> 6;
+        const float* src = A + (64 * half + r) * k + kc * 8;
+        *reinterpret_cast<uint4*>(A_s + a_off(r, 8 * kc)) =
+            make_uint4(pack_bf16(src[0], src[1]), pack_bf16(src[2], src[3]), pack_bf16(src[4], src[5]), pack_bf16(src[6], src[7]));
       }
     }
-    long long t1 = clock64();
-    umma_commit(&bar);
-    mbar_wait(&bar, 0);
-    long long t2 = clock64();
-    out[0] = t1 - t0;
-    out[1] = t2 - t0;
-  }
-  __syncthreads();
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_base, 512);
-}
-
-// ---------------------------------------------------------------------------------------------------------
-// micro-benchmark: the hidden-layer epilogue (tcgen05.ld x16 -> 16 x tanh.approx + FFMA -> bf16 pack -> tcgen05.st x8,
-// 13 chunks dealt to 4 column-split warps per lane quadrant, 16 warps) with / without MMAs running next to it.
-//   flags bit 0: MUFU + FFMA work, bit 1: TMEM loads / stores, bit 2: concurrent A-from-TMEM MMAs (M128 x n x 16,
-//   `nmma` of them, accumulating into columns [208, 208 + n): not the columns the epilogue reads), bit 3: the MMAs
-//   accumulate into the columns the epilogue reads (data is garbage either way: timing only), bit 4: the next chunk's
-//   tcgen05.ld is issued before this chunk's maths (software prefetch), bit 5 / 6 / 7: bf16 pack by integer round-half-up /
-//   integer round-to-nearest-even / no conversion instead of cvt.rn.bf16x2.f32 (F2FP).
-// out[0] = cycles of `reps` epilogue passes (warp 2), out[1] = cycles issue -> completion of the MMAs, out[2] = MMA issue only.
-// ---------------------------------------------------------------------------------------------------------
-template <int flags>
-__global__ void __launch_bounds__(64 + 512, 1) epi_bench_kernel(int nmma, int n, int reps, long long* out) {
-  extern __shared__ __align__(128) uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  __shared__ uint64_t bar;
-  __shared__ uint32_t tmem_slot;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  for (int i = tid; i < 256 * 256 * 2 / 16; i += blockDim.x) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
-  if (tid == 0) {
-    mbar_init(&bar, 1);
-    mbar_fence_init();
-  }
-  fence_proxy_async_smem();
-  if (warp == 1) tmem_alloc(&tmem_slot, 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_slot;
-  if (warp == 1) {
-    if ((flags & 4) && elect_one()) {
-      const uint32_t idesc = umma_idesc_bf16_m128((uint32_t)n);
-      const uint64_t bd0 = umma_smem_desc(smem_u32(smem), (uint32_t)n * 16u, 128u);
-      const uint64_t b_inc = (2u * (uint32_t)n * 16u) >> 4;
-      const uint32_t d = tmem_base + ((flags & 8) ? 0u : 208u);
-      long long t0 = clock64();
-      for (int i = 0; i < nmma; i += 12) {
-        uint64_t bd = bd0;
-        uint32_t acol = tmem_base + 416u;
-        for (int kk = 0; kk < 12 && i + kk < nmma; ++kk) {  // 96 activation columns = 12 K steps
-          umma_bf16_ts(d, acol, bd, idesc, 1u);
-          acol += 8u;
-          bd += b_inc;
-        }
-      }
-      long long t1 = clock64();
-      umma_commit(&bar);
-      mbar_wait(&bar, 0);
-      long long t2 = clock64();
-      out[1] = t2 - t0;
-      out[2] = t1 - t0;
+    fence_proxy_async_smem();
+    __syncthreads();
+    if (tid == 0)  // the slots are already filled: complete this half's phase of them without a copy
+      for (int s = 0; s < nsl; ++s) mbar_arrive(&bar_full[half * nsl + s]);
+    LayerArgs la;
+    la.a_addr = smem_u32(A_s);
+    la.a_ptr = A_s;
+    la.ring_addr = smem_u32(B_s);
+    la.slot_bytes = (uint32_t)kSliceK16 * n * 32u;
+    la.nstages = nsl;
+    la.kslice = kSliceK16;
+    la.nk = k / 16;
+    la.np = n;
+    la.mode = 1;
+    la.n_true = n;
+    la.kp_next = 0;
+    la.stg_ld = stg_ld;
+    la.leaky = 0.f;
+    run_layer<B200PETS_ACT_RELU>(la, 0u, bar_full + half * nsl, bar_empty);
+    wg_bar(0);
+    const float* stg = reinterpret_cast<const float*>(A_s);
+    for (int idx = tid; idx < 64 * n; idx += 128) {
+      const int r = idx / n, c = idx % n;
+      D[(64 * half + r) * n + c] = stg[r * stg_ld + c];
     }
-    __syncwarp();
-  } else if (warp >= 2) {
-    const int q = warp & 3, cs = (warp - 2) >> 2;
-    const uint32_t t_lane = tmem_base + ((uint32_t)(q * 32) << 16);
-    asm volatile("bar.sync 1, 512;" ::: "memory");
-    long long t0 = clock64();
-    float keep = 0.f;
-    for (int r = 0; r < reps; ++r) {
-      uint32_t nxt[16];
-      if ((flags & 2) && (flags & 16)) tmem_ld16(t_lane + (uint32_t)(16 * cs), nxt);
-      for (int c = cs; c < 13; c += 4) {
-        uint32_t r16[16];
-        if (flags & 2) {
-          if (flags & 16) {
-            tmem_ld_wait();
-#pragma unroll
-            for (int e = 0; e < 16; ++e) r16[e] = nxt[e];
-            if (c + 4 < 13) tmem_ld16(t_lane + (uint32_t)(16 * (c + 4)), nxt);
-          } else {
-            tmem_ld16(t_lane + (uint32_t)(16 * c), r16);
-            tmem_ld_wait();
-          }
-        } else {
-#pragma unroll
-          for (int e = 0; e < 16; ++e) r16[e] = __float_as_uint(keep + (float)e);
-        }
-        float v[16];
-#pragma unroll
-        for (int e = 0; e < 16; ++e) {
-          const float x = __uint_as_float(r16[e]);
-          v[e] = (flags & 1) ? fmaf(x, tanh_approx(x), x) : x;
-        }
-        uint32_t pk[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          if (flags & 32) {  // round-half-up on the integer pipe + byte permute
-            pk[e] = __byte_perm(__float_as_uint(v[2 * e]) + 0x8000u, __float_as_uint(v[2 * e + 1]) + 0x8000u, 0x7632);
-          } else if (flags & 64) {  // round-to-nearest-even on the integer pipe
-            const uint32_t a0 = __float_as_uint(v[2 * e]), a1 = __float_as_uint(v[2 * e + 1]);
-            pk[e] = __byte_perm(a0 + 0x7FFFu + ((a0 >> 16) & 1u), a1 + 0x7FFFu + ((a1 >> 16) & 1u), 0x7632);
-          } else if (flags & 128) {  // no conversion at all
-            pk[e] = __float_as_uint(v[2 * e] + v[2 * e + 1]);
-          } else {
-            pk[e] = pack_bf16(v[2 * e], v[2 * e + 1]);
-          }
-        }
-        if ((flags & 2) && c < 12) tmem_st8(t_lane + 416u + (uint32_t)(8 * c), pk);
-        else keep += __uint_as_float(pk[0]);
-      }
-      if (flags & 2) tmem_st_wait();
-      asm volatile("bar.sync 1, 512;" ::: "memory");
-    }
-    long long t1 = clock64();
-    if (warp == 2 && lane == 0) out[0] = t1 - t0;
-    if (keep == 123.456f) out[3] = 1;
+    __syncthreads();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, 512);
 }
 
 }  // namespace
@@ -1285,45 +760,26 @@ static int tc_device_limits() {  // cached per device (a process may drive sever
 }
 
 // smem plan for a model; returns false when the tensor-core path does not cover the dimensions
-bool tc_make_plan(const ModelDev& m, int max_smem, TcPlan* out, bool expectation = false) {
+bool tc_make_plan(const ModelDev& m, int max_smem, TcPlan* out, bool expectation = false, bool cem = false) {
   TcPlan p{};
   p.nlayers = m.L + 1;
   if (m.in + 2 > 256 || m.hid + 2 > 256 || m.nout > 256 || m.D > 256) return false;
-  int kp_max = 0, tm = 32;
-  uint32_t stage = 0;
+  int kp_max = 0;
   for (int l = 0; l < p.nlayers; ++l) {
     if (m.Np[l] > 256 || m.Kp[l] > 256) return false;
-    p.nblk[l] = (m.Kp[l] + 63) / 64;
     kp_max = max(kp_max, m.Kp[l]);
-    stage = max(stage, (uint32_t)m.Kp[l] * m.Np[l] * 2u);
-    while (tm < m.Np[l]) tm *= 2;
   }
-  p.stage_bytes = (stage + 127u) & ~127u;
-  p.tmem_cols = 512;
-  (void)tm;
-  // N split of the hidden layers (16-column chunks): half 0 takes ~8/13 of them (width 208: 128 + 80 columns).  An MMA costs
-  // max(65, N / 2) cycles per K step (profiles/r2_umma_issue_rate_ts.txt), so 128 + 80 is 130 cycles per K step where
-  // 144 + 64 was 137; every column-split warp gets exactly two chunks of half 0, one of half 1 and a slice of the tail chunk.
-  {
-    const int C = m.Np[0] / 16;
-    int c0 = (C * 8 + 6) / 13;
-    static const int c0_env = [] { const char* e = getenv("B200PETS_TC_H0CHUNKS"); return e ? atoi(e) : 0; }();  // A/B switch
-    if (c0_env > 0) c0 = c0_env;
-    c0 = max(1, min(C - 1, c0));
-    p.h0n = c0 * 16;
-  }
-  if (m.Np[0] - p.h0n < 16) return false;
-  static const int ts_env = [] { const char* e = getenv("B200PETS_TC_TAILSPLIT"); return e ? atoi(e) : 0; }();  // A/B switch
-  p.tail_split = ts_env;
+  p.kp_max = kp_max;
+  const int npl = m.Np[p.nlayers - 1];
+  p.stg_ld = npl + 4;
+  p.wg_bytes = ((uint32_t)max(64 * kp_max * 2, 64 * p.stg_ld * 4) + 127u) & ~127u;
   const int outq = (m.out + 3) & ~3;
   p.obs_ld = max(m.D, outq) | 1;  // a row holds the D observation words, the learned-reward word and the output padding
   p.act_ld = m.A | 1;
   uint32_t off = 0;
-  p.off_A = 0;
+  p.off_A = off; off += 2u * p.wg_bytes;
   p.off_obs = off; off += (uint32_t)kTileM * p.obs_ld * 4;
-  p.off_act = off; off += 3u * (uint32_t)kTileM * p.act_ld * 4;
-  p.tail_ld = (m.Kp[0] - m.Dp) | 1;
-  p.off_tail = off; off += (uint32_t)kTileM * p.tail_ld * 4;
+  p.off_act = off; off += (uint32_t)kTileM * p.act_ld * 4;
   off = (off + 15u) & ~15u;
   p.off_const = off; off += (uint32_t)(2 * m.Kp[0]) * 4;
   off = (off + 15u) & ~15u;
@@ -1333,13 +789,23 @@ bool tc_make_plan(const ModelDev& m, int max_smem, TcPlan* out, bool expectation
   p.exp_ld = (2 * outq) | 1;
   if (expectation) off += (uint32_t)kTileM * p.exp_ld * 4;
   off = (off + 15u) & ~15u;
-  p.off_bar = off; off += (2 * kMaxStages + 4) * 8 + 16;
+  p.off_bar = off; off += 2 * kMaxStages * 8;
   off = (off + 127u) & ~127u;
   p.off_ring = off;
-  int S = ((int)max_smem - (int)off) / (int)p.stage_bytes;
-  if (S < 1) return false;  // S >= 2: one layer in use, the next one in flight; S == 1 (wide layers): no prefetch
+  const int cem_tab = cem ? 2 * kCemTabDims * (int)sizeof(float) : 0;
+  // longest slices that still leave three slots (one in use, two in flight); wide models get shorter slices
+  int S = 0;
+  for (p.kslice = kSliceK16;; --p.kslice) {
+    uint32_t slot = 0;
+    for (int l = 0; l < p.nlayers; ++l) slot = max(slot, (uint32_t)min(m.Kp[l] >> 4, p.kslice) * m.Np[l] * 32u);
+    p.slot_bytes = (slot + 127u) & ~127u;
+    S = ((int)max_smem - cem_tab - (int)off) / (int)p.slot_bytes;
+    if (S >= 3 || p.kslice == 1) break;
+  }
+  if (S < 2) return false;
   p.nstages = min(S, kMaxStages);
-  p.smem_bytes = off + (uint32_t)p.nstages * p.stage_bytes;
+  p.smem_bytes = off + max((uint32_t)p.nstages * p.slot_bytes, cem ? kTailScratch : 0u);
+  if ((int)p.smem_bytes + cem_tab > max_smem) return false;
   *out = p;
   return true;
 }
@@ -1354,8 +820,10 @@ int launch_rollout_tc(const ModelDev& m, const RolloutArgs& a, cudaStream_t stre
   int rc = tc_device_limits();
   if (rc) return rc;
   const bool expect = a.propagation == B200PETS_PROP_EXPECTATION;
+  const bool cemf = a.cem_mu != nullptr || a.tail_counter != nullptr;
+  if (expect && cemf) return b200pets_set_error(B200PETS_EUNSUPPORTED, "fused CEM iteration does not cover propagation='expectation'");
   TcPlan p;
-  if (!tc_make_plan(m, g_max_smem, &p, expect))
+  if (!tc_make_plan(m, g_max_smem, &p, expect, cemf))
     return b200pets_set_error(B200PETS_EUNSUPPORTED, "model dimensions outside the tensor-core path (in %d hid %d out %d)",
                               m.in, m.hid, m.out);
   long long tiles;
@@ -1368,77 +836,40 @@ int launch_rollout_tc(const ModelDev& m, const RolloutArgs& a, cudaStream_t stre
     tiles = (long long)m.M * ((Bm + kTileM - 1) / kTileM);
   }
   const unsigned grid = (unsigned)min((long long)g_sm_count, tiles);
-  const bool cemf = a.cem_mu != nullptr || a.tail_counter != nullptr;
   void (*kern)(const ModelDev, const RolloutArgs, const TcPlan, const long long) = nullptr;
-  if (expect && cemf) return b200pets_set_error(B200PETS_EUNSUPPORTED, "fused CEM iteration does not cover propagation='expectation'");
   if (expect) {
-    kern = m.act == B200PETS_ACT_SILU   ? rollout_tc_kernel<B200PETS_ACT_SILU, kEpiSplit, false, false, true>
-           : m.act == B200PETS_ACT_RELU ? rollout_tc_kernel<B200PETS_ACT_RELU, kEpiSplit, false, false, true>
-                                        : rollout_tc_kernel<B200PETS_ACT_LEAKY_RELU, kEpiSplit, false, false, true>;
-  } else
-  switch (m.act) {
-    case B200PETS_ACT_SILU:
-      if (a.timeline && !cemf) kern = rollout_tc_kernel<B200PETS_ACT_SILU, kEpiSplit, false, true>;  // the one instrumented variant
-      else kern = cemf ? rollout_tc_kernel<B200PETS_ACT_SILU, kEpiSplit, true, false> : rollout_tc_kernel<B200PETS_ACT_SILU, kEpiSplit, false, false>;
-      break;
-    case B200PETS_ACT_RELU:
-      kern = cemf ? rollout_tc_kernel<B200PETS_ACT_RELU, kEpiSplit, true, false> : rollout_tc_kernel<B200PETS_ACT_RELU, kEpiSplit, false, false>;
-      break;
-    default:
-      kern = cemf ? rollout_tc_kernel<B200PETS_ACT_LEAKY_RELU, kEpiSplit, true, false>
-                  : rollout_tc_kernel<B200PETS_ACT_LEAKY_RELU, kEpiSplit, false, false>;
-      break;
+    kern = m.act == B200PETS_ACT_SILU   ? rollout_tc_kernel<B200PETS_ACT_SILU, false, true>
+           : m.act == B200PETS_ACT_RELU ? rollout_tc_kernel<B200PETS_ACT_RELU, false, true>
+                                        : rollout_tc_kernel<B200PETS_ACT_LEAKY_RELU, false, true>;
+  } else {
+    switch (m.act) {
+      case B200PETS_ACT_SILU:
+        kern = cemf ? rollout_tc_kernel<B200PETS_ACT_SILU, true> : rollout_tc_kernel<B200PETS_ACT_SILU, false>;
+        break;
+      case B200PETS_ACT_RELU:
+        kern = cemf ? rollout_tc_kernel<B200PETS_ACT_RELU, true> : rollout_tc_kernel<B200PETS_ACT_RELU, false>;
+        break;
+      default:
+        kern = cemf ? rollout_tc_kernel<B200PETS_ACT_LEAKY_RELU, true> : rollout_tc_kernel<B200PETS_ACT_LEAKY_RELU, false>;
+        break;
+    }
   }
   const size_t smem_launch = (size_t)p.smem_bytes + (cemf ? (size_t)2 * kCemTabDims * sizeof(float) : 0);
-  if (smem_launch > (size_t)g_max_smem)
-    return b200pets_set_error(B200PETS_EUNSUPPORTED, "fused CEM iteration: no shared memory left for the sampling table");
   CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_launch));
-  CUDA_TRY(launch_pdl(kern, dim3(grid), dim3(64 + 128 * kEpiSplit), smem_launch, stream, m, a, p, tiles));
+  CUDA_TRY(launch_pdl(kern, dim3(grid), dim3(kThreads), smem_launch, stream, m, a, p, tiles));
   return B200PETS_OK;
 }
 
-int launch_umma_selftest(int k, int n, const float* a, const float* b, float* d, cudaStream_t stream) {
-  const bool ts = k < 0;  // negative k selects the A-from-TMEM form
-  if (ts) k = -k;
+int launch_wgmma_selftest(int k, int n, const float* a, const float* b, float* d, cudaStream_t stream) {
+  const bool pairs = k < 0;  // negative k: A written as bf16 pairs per thread (the hidden-layer epilogue's stores)
+  if (pairs) k = -k;
   if (k % 16 || n % 16 || n > 256 || k > 256 || k < 16 || n < 16)
     return b200pets_set_error(B200PETS_EINVAL, "selftest needs k, n multiples of 16, <= 256");
-  if (ts) {
-    size_t smem_ts = (size_t)n * k * 2 + 64;
-    CUDA_TRY(cudaFuncSetAttribute(umma_selftest_ts_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_ts));
-    umma_selftest_ts_kernel<<<1, 128, smem_ts, stream>>>(k, n, a, b, d);
-    CUDA_TRY(cudaGetLastError());
-    return B200PETS_OK;
-  }
-  size_t smem = (size_t)128 * k * 2 + (size_t)n * k * 2 + 64;
-  CUDA_TRY(cudaFuncSetAttribute(umma_selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  umma_selftest_kernel<<<1, 128, smem, stream>>>(k, n, a, b, d);
-  CUDA_TRY(cudaGetLastError());
-  return B200PETS_OK;
-}
-
-int launch_umma_bench(int mode, int k, int n, int reps, long long* out, cudaStream_t stream) {
-  if (mode >= 100) {  // epilogue micro-benchmark: flags = mode - 100, k = number of concurrent MMAs, n = their N
-    if (n % 16 || n > 208 || n < 16) return b200pets_set_error(B200PETS_EINVAL, "epi_bench: bad n");
-    size_t smem_e = (size_t)256 * 256 * 2 + 1024;
-    void (*kern)(int, int, int, long long*) = nullptr;
-    switch (mode - 100) {  // compile-time flag sets: a run-time test per element would dominate what is being measured
-#define EPI_CASE(F) case F: kern = epi_bench_kernel<F>; break;
-      EPI_CASE(0) EPI_CASE(1) EPI_CASE(2) EPI_CASE(3) EPI_CASE(4) EPI_CASE(7) EPI_CASE(19) EPI_CASE(23)
-      EPI_CASE(32) EPI_CASE(33) EPI_CASE(34) EPI_CASE(35) EPI_CASE(39) EPI_CASE(51) EPI_CASE(55)
-      EPI_CASE(64) EPI_CASE(65) EPI_CASE(66) EPI_CASE(67) EPI_CASE(71)
-      EPI_CASE(128) EPI_CASE(129) EPI_CASE(130) EPI_CASE(131) EPI_CASE(135)
-#undef EPI_CASE
-      default: return b200pets_set_error(B200PETS_EINVAL, "epi_bench: flag set %d not instantiated", mode - 100);
-    }
-    CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_e));
-    kern<<<1, 64 + 512, smem_e, stream>>>(k, n, reps, out);
-    CUDA_TRY(cudaGetLastError());
-    return B200PETS_OK;
-  }
-  if (k % 16 || n % 16 || n > 256 || k > 256) return b200pets_set_error(B200PETS_EINVAL, "umma_bench: bad shape");
-  size_t smem = (size_t)(128 + 256) * 256 * 2 + 1024;
-  CUDA_TRY(cudaFuncSetAttribute(umma_bench_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  umma_bench_kernel<<<1, 128, smem, stream>>>(mode, k, n, reps, out);
+  const int stg_ld = n + 4;
+  const uint32_t wg_bytes = ((uint32_t)max(64 * k * 2, 64 * stg_ld * 4) + 127u) & ~127u;
+  const size_t smem = (size_t)wg_bytes + (size_t)n * k * 2 + 3 * 4 * 8;
+  CUDA_TRY(cudaFuncSetAttribute(wgmma_selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  wgmma_selftest_kernel<<<1, 128, smem, stream>>>(k, n, pairs ? 1 : 0, wg_bytes, stg_ld, a, b, d);
   CUDA_TRY(cudaGetLastError());
   return B200PETS_OK;
 }

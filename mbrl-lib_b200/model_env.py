@@ -125,7 +125,7 @@ class ModelEnv:
             self.staged.ensure_fresh()
 
     def push_weights(self):
-        """Re-stage the packed device copy NOW (fp32 gather of the elite members + bf16 UMMA images, a few small kernels on
+        """Re-stage the packed device copy NOW (fp32 gather of the elite members + bf16 tensor-core images, a few small kernels on
         the model's stream): what the end of ``ModelTrainer.train`` / ``set_elite`` / ``update_normalizer`` should call."""
         self.staged.ensure_fresh()
 

@@ -339,7 +339,7 @@ def _cfg_to_dict(cfg) -> dict:
 
 def _instantiate(cfg, **overrides):
     """Minimal stand-in for hydra.utils.instantiate: ``_target_`` names ending in a class we provide map to
-    ours (so ``mbrl.planning.CEMOptimizer`` in the shipped YAMLs selects the B200 implementation)."""
+    ours (so ``mbrl.planning.CEMOptimizer`` in the shipped YAMLs selects this implementation)."""
     d = _cfg_to_dict(cfg)
     d.update(overrides)
     target = d.pop("_target_")

@@ -1,7 +1,7 @@
-"""Generate golden vectors from the *imported reference* (mbrl-lib at /root/reference) -- run in the build
+"""Generate golden vectors from the *imported reference* (mbrl-lib copied into oracle/_ref by oracle/install_ref.py) -- run in the build
 container only:
 
-    PYTHONPATH=oracle/ref_shims:/root/reference python oracle/gen_golden.py
+    PYTHONPATH=oracle/ref_shims:oracle/_ref python oracle/gen_golden.py
 
 The reference's RNG calls (torch.randperm, torch.normal, truncated_normal_) are monkey-fed the same
 injected draws that `mbrl_lib_b200.synthetic` regenerates from numpy seeds anywhere, so the committed

@@ -1,4 +1,4 @@
-"""Multi-GPU (NCCL) check of the population-sharded CEM: needs >= 2 GPUs on the box (gpurun --gpus 2); skipped otherwise.
+"""Multi-GPU (NCCL) check of the population-sharded CEM: needs >= 2 GPUs; skipped otherwise.
 The single-GPU equivalent of the same property (two shards in one process) is tests/test_gpu_shuffle.py::
 test_sharded_cem_equals_unsharded_plan."""
 import json
@@ -20,7 +20,7 @@ def _free_port():
         return s.getsockname()[1]
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two GPUs (gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two GPUs")
 def test_sharded_cem_over_nccl_equals_single_gpu_plan():
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2", "--master-addr", "127.0.0.1",
            "--master-port", str(_free_port()), os.path.join(ROOT, "tests", "multi_worker.py")]

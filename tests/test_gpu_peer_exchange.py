@@ -4,7 +4,7 @@ on ONE GPU, so that the single-GPU suite covers them (tests/test_gpu_multi.py ne
 * world = 1: values push + global select + elite push + refit + next population must equal, bit for bit,
   b200pets_cem_update (the single-GPU refit) followed by b200pets_cem_sample_shard on the refitted distribution;
 * world = 2 emulated in one process: two "ranks" with their own buffers, kernels on two streams (they wait for each other's
-  flags, so they must be co-resident: two single-CTA selects + sampling CTAs fit a B200 many times over); both must end
+  flags, so they must be co-resident: two single-CTA selects + sampling CTAs fit an H100 many times over); both must end
   with the refit of the UNION population and draw their own shard of the next one.
 NaNs, ties at the selection threshold and a -inf are in the values on purpose.
 """

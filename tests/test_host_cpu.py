@@ -122,13 +122,13 @@ def test_staging_signature_tracks_training_side_changes():
     assert len({s0, s1, s2, s3}) == 4
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/mbrl"), reason="reference tree only exists in the build container")
+@pytest.mark.skipif(not os.path.isdir(os.path.join(ROOT, "oracle", "_ref", "mbrl")), reason="no oracle/_ref (oracle/install_ref.py)")
 def test_staging_reads_the_real_reference_objects():
     """Drop-in check against mbrl-lib's own classes (imported with the API shims): the staging code must find every
     attribute it needs on OneDTransitionRewardModel(GaussianMLP) and resolve mbrl's own reward / termination fns."""
     import sys
 
-    sys.path[:0] = [os.path.join(ROOT, "oracle", "ref_shims"), "/root/reference"]
+    sys.path[:0] = [os.path.join(ROOT, "oracle", "ref_shims"), os.path.join(ROOT, "oracle", "_ref")]
     try:
         import mbrl.env.reward_fns as R
         import mbrl.env.termination_fns as T

@@ -1,13 +1,12 @@
 """The drop-in boundary against REAL mbrl-lib objects (SURVEY.md 8b; VERDICT r1 "boundary is a mirror, never a plug-in").
 
-The unmodified reference is imported from ``baseline/_ref`` (the pip --target install that travels to the GPU box) or
-``/root/reference`` (build container), with the four absent pure-Python deps shimmed (``oracle/ref_shims``).
+The unmodified reference is imported from ``oracle/_ref`` (made by ``oracle/install_ref.py``; the tests skip without it), with the four absent pure-Python deps shimmed (``oracle/ref_shims``).
 
 * CPU (here): ``staging.StagedModel(stage=False)`` reads a real ``mbrl.models.OneDTransitionRewardModel(GaussianMLP)``
   after ``set_elite`` / ``update_normalizer`` exactly as the kernels need it, its signature notices what
   ``ModelTrainer`` / ``Normalizer.update_stats`` change between ``act()`` calls, the reference's own reward /
   termination callables resolve to device functions, and the shipped ``conf/action_optimizer/{cem,icem,mppi}.yaml``
-  instantiate through ``_instantiate`` into the B200 classes.
+  instantiate through ``_instantiate`` into this project's classes.
 * GPU: the real reference model object lives on cuda:0; OUR ``ModelEnv`` wraps it and must reproduce what the
   REFERENCE's ``ModelEnv.evaluate_action_sequences`` computes on the very same object with the same injected draws.
 """
@@ -121,7 +120,7 @@ def test_reference_callables_resolve_to_device_functions():
 def _shipped_yaml(rel):
     import yaml
 
-    for base in (os.path.join(ROOT, "baseline", "_ref"), "/root/reference"):
+    for base in (os.path.join(ROOT, "oracle", "_ref"),):
         path = os.path.join(base, "mbrl", "examples", "conf", "action_optimizer", rel)
         if os.path.exists(path):
             with open(path) as f:
