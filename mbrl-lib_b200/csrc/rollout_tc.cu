@@ -109,8 +109,30 @@ struct LayerArgs {
   float leaky;
 };
 
+// One K slice: N K steps (kk0 .. kk0 + N - 1 of the layer) issued back to back as one wgmma group.  N is a compile-time
+// constant so that the group is straight-line code: a loop with a runtime trip count is unrolled with a remainder whose
+// branches sit between the MMAs, and ptxas then waits for each MMA to complete before it issues the next one
+// (C7519 / C7520).  Only the layer's first K step overwrites the accumulators.
+template <int N, int W0, int W1, int R0, int R1>
+__device__ __forceinline__ void wg_slice(float (&d0)[R0], float (&d1)[R1], uint32_t a_addr, uint32_t slot, uint32_t b_lbo,
+                                         int kk0) {
+  const uint32_t b_kstep = 2u * b_lbo;  // bytes of one K step (16 rows) of the weight image
+  wgmma_fence();
+#pragma unroll
+  for (int j = 0; j < N; ++j) {
+    const uint64_t da = wgmma_desc(a_addr + (uint32_t)(kk0 + j) * 2048u, 1024u, 128u);
+    const uint32_t b = slot + (uint32_t)j * b_kstep;
+    const uint32_t acc = (j > 0 || kk0 > 0) ? 1u : 0u;
+    Wgmma<W0>::mma(d0, da, wgmma_desc(b, b_lbo, 128u), acc);
+    if constexpr (W1 > 0) Wgmma<W1>::mma(d1, da, wgmma_desc(b + (uint32_t)(W0 / 8) * 128u, b_lbo, 128u), acc);
+  }
+  wgmma_commit();
+}
+
+// Inlined into the kernel: ptxas also serialises wgmma chains in a function that is called (C7510).
 template <int ACT, int W0, int W1>
-static __device__ __noinline__ uint32_t wg_layer(const LayerArgs la, uint32_t ring_pos, uint64_t* bar_full, uint64_t* bar_empty) {
+__device__ __forceinline__ uint32_t wg_layer(const LayerArgs& la, uint32_t ring_pos, uint64_t* bar_full, uint64_t* bar_empty) {
+  static_assert(kSliceK16 == 4, "wg_layer dispatches slices of 1 .. 4 K steps");
   constexpr int R1 = W1 > 0 ? W1 / 2 : 1;
   float d0[W0 / 2], d1[R1];
 #pragma unroll
@@ -122,21 +144,17 @@ static __device__ __noinline__ uint32_t wg_layer(const LayerArgs la, uint32_t ri
   uint32_t phase = ring_pos >> 16;
   int prev = -1;
   const uint32_t b_lbo = (uint32_t)la.np * 16u;
-  const uint32_t b_kstep = 2u * b_lbo;  // bytes of one K step (16 rows) of the weight image
   fence_operands(d0);
   fence_operands(d1);
   for (int k0 = 0; k0 < la.nk; k0 += la.kslice) {
     mbar_wait(&bar_full[stage], phase);
-    wgmma_fence();
     const uint32_t slot = la.ring_addr + (uint32_t)stage * la.slot_bytes;
-    const int k1 = min(la.nk, k0 + la.kslice);
-    for (int kk = k0; kk < k1; ++kk) {
-      const uint64_t da = wgmma_desc(la.a_addr + (uint32_t)kk * 2048u, 1024u, 128u);
-      const uint32_t b = slot + (uint32_t)(kk - k0) * b_kstep;
-      Wgmma<W0>::mma(d0, da, wgmma_desc(b, b_lbo, 128u), kk > 0 ? 1u : 0u);
-      if constexpr (W1 > 0) Wgmma<W1>::mma(d1, da, wgmma_desc(b + (uint32_t)(W0 / 8) * 128u, b_lbo, 128u), kk > 0 ? 1u : 0u);
+    switch (min(la.nk - k0, la.kslice)) {
+      case 1: wg_slice<1, W0, W1>(d0, d1, la.a_addr, slot, b_lbo, k0); break;
+      case 2: wg_slice<2, W0, W1>(d0, d1, la.a_addr, slot, b_lbo, k0); break;
+      case 3: wg_slice<3, W0, W1>(d0, d1, la.a_addr, slot, b_lbo, k0); break;
+      default: wg_slice<4, W0, W1>(d0, d1, la.a_addr, slot, b_lbo, k0); break;
     }
-    wgmma_commit();
     if (prev >= 0) {  // the previous slice's MMAs are complete: hand its slot back to the producer
       wgmma_wait<1>();
       if (lane == 0) mbar_arrive(&bar_empty[prev]);
