@@ -123,6 +123,13 @@ int b200pets_model_refresh(b200pets_model_t model, const float* const* weights, 
 void b200pets_model_destroy(b200pets_model_t model);
 /* 1 if the tensor-core path covers this model's dimensions, else 0 (callers then use B200PETS_PREC_F32). */
 int b200pets_model_supports_tc(b200pets_model_t model);
+/* Launch plans the rollout kernels choose for this model on the current device when running `propagation`
+ * (B200PETS_PROP_*), computed by the same code as the launchers:
+ *   info[0] tensor-core kernel: K steps (16 weight rows each) per ring slot, 1..4; 0 = no tensor-core plan
+ *   info[1] tensor-core kernel: weight ring slots (0 when info[0] == 0)
+ *   info[2] tensor-core kernel: dynamic shared memory in bytes (0 when info[0] == 0)
+ *   info[3] fp32 kernel: rows per CTA tile, 64, 32 or 16; 0 = the model does not fit */
+int b200pets_model_plan_info(b200pets_model_t model, int32_t propagation, int32_t info[4]);
 
 typedef struct {
   int32_t population;  /* N */

@@ -53,6 +53,7 @@ _SIGNATURES = {
                                          C.POINTER(C.c_double), C.POINTER(C.c_float), C.POINTER(C.c_float), _P]),
     "b200pets_model_destroy": (None, [_P]),
     "b200pets_model_supports_tc": (C.c_int, [_P]),
+    "b200pets_model_plan_info": (C.c_int, [_P, C.c_int32, C.POINTER(C.c_int32)]),
     "b200pets_eval_workspace_bytes": (C.c_size_t, [_P, C.POINTER(RolloutCfg)]),
     "b200pets_eval_sequences": (C.c_int, [_P, C.POINTER(RolloutCfg), _P, _P, _P, _P, _P, _P, _P, C.c_size_t, _P]),
     "b200pets_step": (C.c_int, [_P, C.c_int32, C.c_int32, C.c_int64, _P, _P, _P, _P, C.c_uint64, C.c_uint64, C.c_int32,

@@ -285,6 +285,25 @@ void b200pets_model_destroy(b200pets_model_t model) {
 
 int b200pets_model_supports_tc(b200pets_model_t model) { return model && model->tc_ok ? 1 : 0; }
 
+int b200pets_model_plan_info(b200pets_model_t model, int32_t propagation, int32_t info[4]) {
+  if (!model || !info) return b200pets_set_error(B200PETS_EINVAL, "model_plan_info: null argument");
+  if (propagation < B200PETS_PROP_RANDOM_MODEL || propagation > B200PETS_PROP_EXPECTATION)
+    return b200pets_set_error(B200PETS_EINVAL, "model_plan_info: unknown propagation %d", propagation);
+  int kslice = 0, nstages = 0, smem = 0;
+  if (model->tc_ok) {
+    int rc = tc_plan_info(model->dev, propagation == B200PETS_PROP_EXPECTATION, &kslice, &nstages, &smem);
+    if (rc) return rc;
+  }
+  F32Plan fp;
+  int rc = f32_tile_plan(model->dev, &fp);
+  if (rc) return rc;
+  info[0] = kslice;
+  info[1] = nstages;
+  info[2] = smem;
+  info[3] = fp.rows;
+  return B200PETS_OK;
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // rollouts
 // ---------------------------------------------------------------------------------------------------------

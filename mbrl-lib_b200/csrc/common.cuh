@@ -83,6 +83,18 @@ struct RolloutArgs {
   float tail_alpha;
 };
 
+// Launch plans, chosen on the host from the model's shape and the device's opt-in shared memory (the launchers and
+// b200pets_model_plan_info call the same functions).
+struct F32Plan {
+  int rows;     // rows per CTA tile of rollout_f32_kernel: 64, 32 or 16 (0: no tile fits)
+  int LD;       // row stride (floats) of the activation buffers
+  int wmax;     // widest layer (input or output columns)
+  size_t smem;  // dynamic shared memory of one CTA
+};
+int f32_tile_plan(const ModelDev& m, F32Plan* p);
+// tensor-core kernel: K steps per ring slot (0: no plan for this propagation), ring slots, dynamic shared memory
+int tc_plan_info(const ModelDev& m, bool expectation, int* kslice, int* nstages, int* smem_bytes);
+
 // ------------------------------------------------------------------------------------------------------
 // Philox4x32-10 counter RNG (Salmon et al. 2011).  key = seed, counter = (a, b, c, d).
 // ------------------------------------------------------------------------------------------------------

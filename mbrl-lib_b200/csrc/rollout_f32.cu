@@ -305,30 +305,46 @@ static long long f32_num_tiles(const ModelDev& m, const RolloutArgs& a, int TR) 
   return (long long)m.M * ((Bm + TR - 1) / TR);
 }
 
-int launch_rollout_f32(const ModelDev& m, const RolloutArgs& a, cudaStream_t stream) {
+// Tile of rollout_f32_kernel for a model on the current device: the most rows per CTA (64, 32 or 16) whose buffers fit
+// in the opt-in shared memory.  p->rows = 0 when not even 16 rows fit.  Also what b200pets_model_plan_info reports.
+int f32_tile_plan(const ModelDev& m, F32Plan* p) {
   int wmax = m.in;
   for (int l = 0; l <= m.L; ++l) wmax = max(wmax, m.N[l]);
-  const int LD = ((wmax + 3) & ~3) + 4;
-  auto smem_for = [&](int TR) {
-    return (size_t)TR * (2 * LD + m.D + m.A + m.nout + 2) * sizeof(float) + (size_t)TR * (2 * sizeof(long long) + sizeof(int));
-  };
+  p->wmax = wmax;
+  p->LD = ((wmax + 3) & ~3) + 4;
   int dev = 0, max_smem = 0;
   CUDA_TRY(cudaGetDevice(&dev));
   CUDA_TRY(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-  if (smem_for(64) <= (size_t)max_smem) {
-    size_t sm = smem_for(64);
+  p->rows = 0;
+  p->smem = 0;
+  for (int TR = 64; TR >= 16; TR /= 2) {
+    const size_t sm = (size_t)TR * (2 * p->LD + m.D + m.A + m.nout + 2) * sizeof(float) +
+                      (size_t)TR * (2 * sizeof(long long) + sizeof(int));
+    if (sm <= (size_t)max_smem) {
+      p->rows = TR;
+      p->smem = sm;
+      break;
+    }
+  }
+  return B200PETS_OK;
+}
+
+int launch_rollout_f32(const ModelDev& m, const RolloutArgs& a, cudaStream_t stream) {
+  F32Plan p;
+  int rc = f32_tile_plan(m, &p);
+  if (rc) return rc;
+  const size_t sm = p.smem;
+  if (p.rows == 64) {
     CUDA_TRY(cudaFuncSetAttribute(rollout_f32_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-    rollout_f32_kernel<64><<<(unsigned)f32_num_tiles(m, a, 64), kThreads, sm, stream>>>(m, a, LD);
-  } else if (smem_for(32) <= (size_t)max_smem) {
-    size_t sm = smem_for(32);
+    rollout_f32_kernel<64><<<(unsigned)f32_num_tiles(m, a, 64), kThreads, sm, stream>>>(m, a, p.LD);
+  } else if (p.rows == 32) {
     CUDA_TRY(cudaFuncSetAttribute(rollout_f32_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-    rollout_f32_kernel<32><<<(unsigned)f32_num_tiles(m, a, 32), kThreads, sm, stream>>>(m, a, LD);
-  } else if (smem_for(16) <= (size_t)max_smem) {
-    size_t sm = smem_for(16);
+    rollout_f32_kernel<32><<<(unsigned)f32_num_tiles(m, a, 32), kThreads, sm, stream>>>(m, a, p.LD);
+  } else if (p.rows == 16) {
     CUDA_TRY(cudaFuncSetAttribute(rollout_f32_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-    rollout_f32_kernel<16><<<(unsigned)f32_num_tiles(m, a, 16), kThreads, sm, stream>>>(m, a, LD);
+    rollout_f32_kernel<16><<<(unsigned)f32_num_tiles(m, a, 16), kThreads, sm, stream>>>(m, a, p.LD);
   } else {
-    return b200pets_set_error(B200PETS_EUNSUPPORTED, "layer width %d needs more shared memory than a CTA has", wmax);
+    return b200pets_set_error(B200PETS_EUNSUPPORTED, "layer width %d needs more shared memory than a CTA has", p.wmax);
   }
   CUDA_TRY(cudaGetLastError());
   return B200PETS_OK;

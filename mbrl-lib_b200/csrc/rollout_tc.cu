@@ -834,6 +834,18 @@ bool tc_supported(const ModelDev& m) {
   return tc_make_plan(m, g_max_smem, &p);
 }
 
+// the plan launch_rollout_tc uses for an evaluation / step (no fused CEM iteration) with or without "expectation"
+int tc_plan_info(const ModelDev& m, bool expectation, int* kslice, int* nstages, int* smem_bytes) {
+  int rc = tc_device_limits();
+  if (rc) return rc;
+  TcPlan p;
+  const bool ok = tc_make_plan(m, g_max_smem, &p, expectation, false);
+  *kslice = ok ? p.kslice : 0;
+  *nstages = ok ? p.nstages : 0;
+  *smem_bytes = ok ? (int)p.smem_bytes : 0;
+  return B200PETS_OK;
+}
+
 int launch_rollout_tc(const ModelDev& m, const RolloutArgs& a, cudaStream_t stream) {
   int rc = tc_device_limits();
   if (rc) return rc;

@@ -221,7 +221,7 @@ class ShardedCEMOptimizer:
             H = shape[0]
             # the same (seed, offset) on every rank: draws are keyed by GLOBAL sequence / row / group indices
             call = env._next_offset()
-            rcfg = _lib.RolloutCfg(n_loc, H, fused.num_particles, _lib.PREC[env.precision], _lib.PROP[prop],
+            rcfg = _lib.RolloutCfg(n_loc, H, fused.num_particles, _lib.PREC[env.precision_for(prop)], _lib.PROP[prop],
                                    _lib.TS1_TILE_SHUFFLE, env._seed, 0, self.local_offset, self.population_size)
             obs0 = env._obs_to_device(fused.obs)
             eval_ws = env._workspace(self.lib.b200pets_eval_workspace_bytes(env.staged.handle, C.byref(rcfg)))

@@ -32,6 +32,7 @@ class ModelEnv:
         self.ts1 = ts1
         self.lib = _lib.load()
         self.staged = StagedModel(model, reward_fn, termination_fn)
+        self._auto = precision == "auto"
         if precision == "auto":
             precision = "bf16_tc" if self.staged.supports_tc() else "f32"
         self.precision = precision
@@ -52,6 +53,15 @@ class ModelEnv:
         if pm not in _lib.PROP:
             raise ValueError(f"Invalid propagation method {pm}.")  # gaussian_mlp.py:216
         return pm
+
+    def precision_for(self, propagation: str) -> str:
+        """The kernel a call with ``propagation`` runs on.  ``precision="auto"`` picks the tensor-core kernel only where
+        it has a launch plan for that propagation: "expectation" keeps per-row member sums in shared memory, so a model
+        the tensor-core kernel covers for TS1 / TSinf can still need the fp32 kernel there.  An explicit precision is
+        used as given (and fails loudly where its kernel does not cover the call)."""
+        if self._auto and self.precision == "bf16_tc" and not self.staged.supports_tc(propagation):
+            return "f32"
+        return self.precision
 
     def _next_offset(self) -> int:
         """Philox stream counter of this environment: one value per API call.  ``b200pets_cem_plan`` derives the
@@ -97,7 +107,7 @@ class ModelEnv:
         kernels use in tile-shuffle mode for Philox ``offset`` (``b200pets_shuffle_member_map``).  Diagnostics /
         parity tests: the oracle consumes it as the reference's per-step assignment (gaussian_mlp.py:202-212)."""
         prop = self._propagation()
-        cfg = _lib.RolloutCfg(population, horizon, num_particles, _lib.PREC[self.precision], _lib.PROP[prop],
+        cfg = _lib.RolloutCfg(population, horizon, num_particles, _lib.PREC[self.precision_for(prop)], _lib.PROP[prop],
                               _lib.TS1_TILE_SHUFFLE, self._seed, offset, first_sequence, global_population)
         groups = int(self.lib.b200pets_shuffle_num_groups(C.byref(cfg)))
         M = len(self.staged.members())
@@ -219,7 +229,7 @@ class ModelEnv:
                 done = torch.empty(B, dtype=torch.uint8, device=self.device)
             with torch.cuda.device(self.device):
                 _lib.check(self.lib.b200pets_step(
-                    self.staged.handle, _lib.PREC[self.precision], _lib.PROP[prop], B, _lib.ptr(obs), _lib.ptr(actions),
+                    self.staged.handle, _lib.PREC[self.precision_for(prop)], _lib.PROP[prop], B, _lib.ptr(obs), _lib.ptr(actions),
                     _lib.ptr(perm), _lib.ptr(_eps), self._seed, self._call_offset() if _offset is None else _offset,
                     int(bool(sample)), _lib.ptr(next_obs),
                     _lib.ptr(reward), _lib.ptr(done), _lib.stream_ptr()), "step")
@@ -270,7 +280,7 @@ class ModelEnv:
                         perms = torch.randperm(B, device=self.device).view(1, B)
                 elif prop == "random_model" and (self.ts1 == "perms" or self._few_groups(population_size, num_particles)):
                     perms = torch.stack([torch.randperm(B, device=self.device) for _ in range(horizon)])
-            cfg = _lib.RolloutCfg(population_size, horizon, num_particles, _lib.PREC[self.precision], _lib.PROP[prop],
+            cfg = _lib.RolloutCfg(population_size, horizon, num_particles, _lib.PREC[self.precision_for(prop)], _lib.PROP[prop],
                                   _lib.TS1_PERMS if perms is not None else _lib.TS1_TILE_SHUFFLE, self._seed,
                                   self._call_offset() if _offset is None else _offset, int(_shard[0]), int(_shard[1]))
             obs0 = self._obs_to_device(initial_state)

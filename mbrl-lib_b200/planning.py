@@ -158,7 +158,7 @@ class CEMOptimizer(Optimizer):
             n = H if prop == "random_model" else 1
             perms = torch.stack([torch.stack([torch.randperm(B, device=self.device) for _ in range(n)])
                                  for _ in range(self.num_iterations)])
-        rcfg = _lib.RolloutCfg(self.population_size, H, obj.num_particles, _lib.PREC[env.precision], _lib.PROP[prop],
+        rcfg = _lib.RolloutCfg(self.population_size, H, obj.num_particles, _lib.PREC[env.precision_for(prop)], _lib.PROP[prop],
                                _lib.TS1_PERMS if perms is not None else _lib.TS1_TILE_SHUFFLE, env._seed,
                                env._next_offset())
         ccfg = _lib.CemCfg(self.num_iterations, self.elite_num, float(self.alpha), int(self.return_mean_elites),

@@ -149,8 +149,19 @@ class StagedModel:
         self.desc = desc
         self._sig = sig
 
-    def supports_tc(self) -> bool:
-        return bool(self.lib.b200pets_model_supports_tc(self.handle))
+    def supports_tc(self, propagation: Optional[str] = None) -> bool:
+        """Whether the tensor-core kernel covers this model; with ``propagation``, whether it has a launch plan for
+        that propagation method ("expectation" needs more shared memory than the other two)."""
+        if propagation is None:
+            return bool(self.lib.b200pets_model_supports_tc(self.handle))
+        return self.plan_info(propagation)["kslice"] > 0
+
+    def plan_info(self, propagation: str) -> dict:
+        """Launch plans of the rollout kernels for this model on the current device (``b200pets_model_plan_info``)."""
+        info = (C.c_int32 * 4)()
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.b200pets_model_plan_info(self.handle, _lib.PROP[propagation], info), "model_plan_info")
+        return {"kslice": info[0], "nstages": info[1], "tc_smem": info[2], "f32_rows": info[3]}
 
     def close(self):
         if self.handle is not None:

@@ -13,6 +13,7 @@ from __future__ import annotations
 
 import dataclasses
 import hashlib
+import itertools
 from typing import Dict, List, Optional, Sequence
 
 import numpy as np
@@ -44,6 +45,9 @@ class CaseSpec:
     action_ub: float = 1.0
     obs0_first: Optional[float] = None  # e.g. 1.4 for humanoid height
     seed: int = 0
+    # added to the output bias of every other logvar column (columns 0, 2, 4, ... take the offsets in turn), after
+    # all draws: pushes raw logvars far outside [min_logvar, max_logvar]
+    logvar_offsets: Sequence[float] = ()
 
     @property
     def proc_obs_dim(self) -> int:
@@ -149,6 +153,45 @@ _register(CaseSpec("ant_learned_fn", obs_dim=27, act_dim=8, hid_size=64, num_lay
                    population=24, horizon=7, particles=5, obs0_first=0.6))
 
 
+
+# Launch-plan cases: shapes that put the kernels on the launch plans the cases above never reach (the plan each one
+# lands on is read back from b200pets_model_plan_info by tests/test_gpu_parity.py::test_launch_plans_are_covered).
+# Tensor-core kernel: K steps per weight-ring slot 1 / 2 / 3, a two-slot ring, hidden widths of 16, 128, 144 and 256
+# accumulator columns (hid % 16 of 14, 15 and 0: where the two bias-one columns sit against the accumulator's end),
+# 256-column input and output layers, seven hidden layers, expectation at a shortened slice.  fp32 kernel: 32- and
+# 16-row tiles.  Plus a model whose raw logvars sit far outside [min_logvar, max_logvar].
+_register(CaseSpec("plan_hid14_deep", obs_dim=5, act_dim=2, hid_size=14, num_layers=7, ensemble_size=3, elites=None,
+                   activation="relu", normalize="float32", population=37, horizon=5, particles=3))
+_register(CaseSpec("plan_hid143", obs_dim=17, act_dim=6, hid_size=143, num_layers=3, ensemble_size=4, elites=(1, 3),
+                   population=45, horizon=6, particles=4))
+_register(CaseSpec("plan_hid128_det", obs_dim=20, act_dim=7, hid_size=128, num_layers=2, ensemble_size=2, elites=None,
+                   normalize="float32", deterministic=True, reward_fn="pusher", population=30, horizon=5, particles=2,
+                   action_lb=-2.0, action_ub=2.0))
+_register(CaseSpec("plan_k3", obs_dim=90, act_dim=6, population=21, horizon=4, particles=5))
+_register(CaseSpec("plan_k2_hid254", obs_dim=90, act_dim=17, hid_size=254, num_layers=3, ensemble_size=2, elites=None,
+                   activation="relu", propagation="fixed_model", population=26, horizon=4, particles=4))
+_register(CaseSpec("plan_k1_out256", obs_dim=127, act_dim=8, hid_size=254, num_layers=2, ensemble_size=2, elites=None,
+                   activation="leaky_relu", learned_rewards=True, reward_fn=None, population=19, horizon=3, particles=4))
+_register(CaseSpec("plan_in254", obs_dim=11, act_dim=243, num_layers=2, ensemble_size=2, elites=None,
+                   population=17, horizon=3, particles=4))
+_register(CaseSpec("plan_ring2", obs_dim=120, act_dim=17, num_layers=2, ensemble_size=2, elites=None,
+                   learned_rewards=True, reward_fn=None, population=23, horizon=3, particles=4))
+_register(CaseSpec("plan_k4_hid254", obs_dim=60, act_dim=20, hid_size=254, num_layers=2, ensemble_size=2, elites=None,
+                   learned_rewards=True, reward_fn=None, population=22, horizon=3, particles=4))
+_register(CaseSpec("plan_exp_k2", obs_dim=57, act_dim=8, hid_size=254, num_layers=2, ensemble_size=3, elites=None,
+                   propagation="expectation", population=13, horizon=3, particles=3))
+_register(CaseSpec("plan_f32_hid512", obs_dim=17, act_dim=6, hid_size=512, num_layers=2, ensemble_size=2, elites=None,
+                   population=100, horizon=4, particles=4))
+_register(CaseSpec("plan_f32_hid512_exp", obs_dim=17, act_dim=6, hid_size=512, num_layers=2, ensemble_size=2,
+                   elites=None, propagation="expectation", population=25, horizon=4, particles=4))
+_register(CaseSpec("plan_f32_humanoid_exp", obs_dim=376, act_dim=17, learned_rewards=True, reward_fn=None,
+                   term_fn="humanoid", propagation="expectation", population=10, horizon=3, particles=4,
+                   action_lb=-0.4, action_ub=0.4, obs0_first=1.4))
+_register(CaseSpec("plan_logvar_extreme", obs_dim=17, act_dim=6, hid_size=64, num_layers=2, ensemble_size=3,
+                   elites=None, population=30, horizon=5, particles=4, logvar_offsets=(10.0, -30.0, -100.0)))
+PLAN_CASES = [n for n in CASES if n.startswith("plan_")]
+
+
 def _rng(spec: CaseSpec, stream: int) -> np.random.Generator:
     return np.random.default_rng([spec.seed, stream, int(hashlib.sha1(spec.name.encode()).hexdigest()[:8], 16)])
 
@@ -173,6 +216,9 @@ def make_model_arrays(spec: CaseSpec) -> Dict[str, object]:
         if li == len(dims) - 1 and not spec.deterministic:
             # moderately confident model: raw logvar around -5 (sigma ~ 0.08)
             b[:, :, spec.out_size:] += -5.0
+        if li == len(dims) - 1 and not spec.deterministic and spec.logvar_offsets:
+            for j, off in zip(range(0, spec.out_size, 2), itertools.cycle(spec.logvar_offsets)):
+                b[:, :, spec.out_size + j] += off
         weights.append(w.astype(np.float32))
         biases.append(b.astype(np.float32))
     out = {

@@ -1,9 +1,10 @@
 """Generate golden vectors from the *imported reference* (mbrl-lib copied into oracle/_ref by oracle/install_ref.py) -- run in the build
 container only:
 
-    PYTHONPATH=oracle/ref_shims:oracle/_ref python oracle/gen_golden.py
+    PYTHONPATH=oracle/ref_shims:oracle/_ref python oracle/gen_golden.py [NAME ...]
 
-The reference's RNG calls (torch.randperm, torch.normal, truncated_normal_) are monkey-fed the same
+With NAMEs, only the rollout goldens of those synthetic cases are (re)written, e.g. `... gen_golden.py plan_k3`; every
+other file under tests/golden stays as it is.  The reference's RNG calls (torch.randperm, torch.normal, truncated_normal_) are monkey-fed the same
 injected draws that `mbrl_lib_b200.synthetic` regenerates from numpy seeds anywhere, so the committed
 `tests/golden/*.npz` hold only outputs + input checksums.  TEST INFRASTRUCTURE; nothing shipped uses it.
 """
@@ -304,8 +305,13 @@ def gen_counter_world():
 if __name__ == "__main__":
     torch.manual_seed(0)
     os.makedirs(GOLD, exist_ok=True)
+    if len(sys.argv) > 1:
+        for nm in sys.argv[1:]:
+            gen_rollout(nm)
+        sys.exit(0)
     for nm in ["cartpole", "halfcheetah", "halfcheetah_small", "pets_halfcheetah_small", "humanoid_trunc",
-               "relu_expectation", "silu_expectation", "hopper_tsinf", "cartpole_pets", "pusher_det", "walker_ant", "humanoid_v4", "tc_hid64", "tc_wide", "tc_shallow", "ant_learned_fn"]:
+               "relu_expectation", "silu_expectation", "hopper_tsinf", "cartpole_pets", "pusher_det", "walker_ant", "humanoid_v4",
+               "tc_hid64", "tc_wide", "tc_shallow", "ant_learned_fn"] + syn.PLAN_CASES:
         gen_rollout(nm)
     gen_step("mbpo_halfcheetah_small", 1000)
     gen_step("cartpole", 500)

@@ -20,8 +20,12 @@ pytestmark = pytest.mark.gpu
 
 DEV = "cuda:0"
 CONTINUOUS = ["halfcheetah_small", "pets_halfcheetah_small", "humanoid_trunc", "cartpole_pets", "pusher_det", "halfcheetah",
-              "humanoid_v4", "tc_hid64", "tc_wide", "tc_shallow", "silu_expectation"]
+              "humanoid_v4", "tc_hid64", "tc_wide", "tc_shallow", "silu_expectation"] + syn.PLAN_CASES
 DISCRETE = ["cartpole", "relu_expectation", "hopper_tsinf", "walker_ant", "ant_learned_fn"]
+# the cases the tensor-core kernel is compared with the oracle on: every continuous-reward case it has a plan for
+TC_CONTINUOUS = ["halfcheetah_small", "pets_halfcheetah_small", "humanoid_trunc", "cartpole_pets", "pusher_det", "halfcheetah",
+                 "tc_hid64", "tc_wide", "tc_shallow", "silu_expectation"] + \
+                [n for n in syn.PLAN_CASES if not n.startswith("plan_f32_")]
 
 
 class _Env:
@@ -70,6 +74,7 @@ def gpu_returns(env, spec, inp):
 def assert_close_continuous(got, ref, tol):
     scale = max(1.0, float(np.abs(ref).max()))
     err = np.abs(got - ref).max()
+    print(f"max |diff| {err:.3e} = {err / scale:.2e} of scale {scale:.3g} (bar {tol:.0e})")
     assert np.isfinite(got).all()
     assert err <= tol * scale, f"max |diff| {err:.3e} > {tol:.1e} * {scale:.3g}"
 
@@ -134,8 +139,7 @@ def test_rollout_f32_discrete_rewards(golden_dir, name):
     assert_close_discrete(got, gold["returns"], spec.particles)
 
 
-@pytest.mark.parametrize("name", ["halfcheetah_small", "pets_halfcheetah_small", "humanoid_trunc", "cartpole_pets",
-                                  "pusher_det", "halfcheetah", "tc_hid64", "tc_wide", "tc_shallow", "silu_expectation"])
+@pytest.mark.parametrize("name", TC_CONTINUOUS)
 def test_rollout_tc_matches_oracle(golden_dir, name):
     spec, arrays, env = make_env(name, "bf16_tc")
     inp = syn.make_rollout_inputs(spec)
@@ -389,6 +393,99 @@ def test_humanoid_v4_dims_use_fp32_path():
     assert env.precision == "f32" and not env.staged.supports_tc()
     _, _, env_tc = make_env("humanoid_v4", "bf16_tc")
     inp = syn.make_rollout_inputs(spec)
+    with pytest.raises(NotImplementedError):
+        gpu_returns(env_tc, spec, inp)
+
+
+def test_launch_plans_are_covered():
+    """The kernels pick their launch plan from the model's shape at run time (b200pets_model_plan_info reports it, from
+    the same code as the launchers).  The cases the oracle comparisons run must together reach every plan class:
+    tensor-core ring slices of 1-4 K steps, rings of two, three and more slots, accumulator widths around the 128-column
+    split, the bias-one columns at either side of the accumulator's end, 256-column layers, the deepest model, and the
+    fp32 kernel's 64 / 32 / 16-row tiles in each of its row mappings."""
+    from test_gpu_shuffle import SHUFFLE_CASES
+
+    f32_modes = {"perms": set(), "tile_shuffle": set(), "expectation": set()}
+    tc = {"kslice": set(), "slots": set(), "hid_np": set(), "out_np": set(), "hid_mod16": set(), "kp0": set(), "hid_kp": set(),
+          "hidden_layers": set(), "deterministic": set(), "exp_kslice": set()}
+    tc_cases = set(TC_CONTINUOUS) | {c[0] for c in SHUFFLE_CASES if c[1] == "bf16_tc"}
+    f32_shuffle = {c[0] for c in SHUFFLE_CASES if c[1] == "f32"}
+    print()
+    for name, spec in syn.CASES.items():
+        _, _, env = make_env(name, "f32")
+        plan = env.staged.plan_info(spec.propagation)
+        print(f"{name:24s} {spec.propagation:13s} {plan}")
+        rows = plan["f32_rows"]
+        assert rows in (16, 32, 64), (name, plan)
+        if name in CONTINUOUS:
+            f32_modes["expectation" if spec.propagation == "expectation" else "perms"].add(rows)
+        if name in f32_shuffle:
+            f32_modes["tile_shuffle"].add(rows)
+        if name not in tc_cases:
+            continue
+        assert plan["kslice"] > 0 and plan["nstages"] >= 2 and plan["tc_smem"] > 0, (name, plan)
+        hid_np = -(-spec.hid_size // 16) * 16
+        out_np = -(-spec.out_size // 16) * 16 * (1 if spec.deterministic else 2)
+        tc["kslice"].add(plan["kslice"])
+        tc["slots"].add(min(plan["nstages"], 4))
+        tc["hid_np"].add(hid_np)
+        tc["out_np"].add(out_np)
+        tc["hid_mod16"].add(spec.hid_size % 16)
+        tc["kp0"].add(-(-(spec.in_size + 2) // 16) * 16)  # input + two bias-one columns, padded to a K step
+        tc["hid_kp"].add(-(-(spec.hid_size + 2) // 16) * 16)
+        tc["hidden_layers"].add(spec.num_layers)
+        tc["deterministic"].add(spec.deterministic)
+        if spec.propagation == "expectation":
+            tc["exp_kslice"].add(plan["kslice"])
+    assert tc["kslice"] >= {1, 2, 3, 4}, tc["kslice"]
+    assert tc["slots"] >= {2, 3, 4}, tc["slots"]  # 4 stands for four or more
+    assert tc["hid_np"] >= {16, 128, 144, 256}, tc["hid_np"]
+    assert 256 in tc["out_np"] and True in tc["deterministic"]
+    assert tc["hid_mod16"] >= {0, 14, 15}, tc["hid_mod16"]
+    assert 256 in tc["kp0"] and 256 in tc["hid_kp"]
+    assert 7 in tc["hidden_layers"]  # B200PETS_MAX_LAYERS - 1
+    assert min(tc["exp_kslice"]) < 4, tc["exp_kslice"]
+    for mode, seen in f32_modes.items():
+        assert seen >= {16, 32, 64}, (mode, seen)
+
+
+def test_auto_precision_follows_the_propagation_plan():
+    """A model the tensor-core kernel covers for TS1 but not for "expectation" (whose per-row member sums take shared
+    memory the weight ring needs): precision="auto" must run expectation calls on the fp32 kernel, at its bar, and an
+    explicit "bf16_tc" must still refuse them loudly."""
+    import dataclasses
+
+    import mbrl_lib_b200 as bp
+    from mbrl_lib_b200 import functions
+    from oracle import pets_oracle as po
+
+    spec = syn.CaseSpec("auto_expectation_fallback", obs_dim=100, act_dim=8, propagation="expectation",
+                        population=20, horizon=4, particles=5)
+    arrays = syn.make_model_arrays(spec)
+    model = bp.model_from_arrays(spec, arrays, DEV)
+    env = bp.ModelEnv(_Env(spec), model, functions.no_termination, functions.REWARD_FNS[spec.reward_fn],
+                      generator=torch.Generator(device=DEV), precision="auto")
+    assert env.staged.plan_info("random_model")["kslice"] > 0
+    assert env.staged.plan_info("expectation")["kslice"] == 0
+    inp = syn.make_rollout_inputs(spec)
+    got = gpu_returns(env, spec, inp)
+    assert_close_continuous(got, oracle_returns(spec, arrays, inp), 2e-4)
+    st = syn.make_step_inputs(spec, 100)
+    state = env.reset(st["obs"], return_as_np=True)
+    nobs, rew, _, _ = env.step(st["act"], state, sample=True, _eps=torch.from_numpy(st["eps"]).to(DEV))
+    on, orw, _ = po.OracleModel(spec, arrays).step(torch.from_numpy(st["obs"]), torch.from_numpy(st["act"]), None,
+                                                   torch.from_numpy(st["eps"]))
+    scale = max(1.0, float(on.abs().max()))
+    assert np.abs(nobs - on.numpy()).max() <= 2e-4 * scale
+    assert np.abs(rew - orw.numpy()).max() <= 2e-4 * scale
+    assert env.precision == "bf16_tc" and env.precision_for("expectation") == "f32"
+    # the same model under TS1 keeps the tensor-core kernel
+    ts1 = dataclasses.replace(spec, propagation="random_model")
+    env_ts1 = bp.ModelEnv(_Env(ts1), bp.model_from_arrays(ts1, arrays, DEV), functions.no_termination,
+                          functions.REWARD_FNS[spec.reward_fn], precision="auto")
+    assert env_ts1.precision_for("random_model") == "bf16_tc"
+    env_tc = bp.ModelEnv(_Env(spec), model, functions.no_termination, functions.REWARD_FNS[spec.reward_fn],
+                         precision="bf16_tc")
     with pytest.raises(NotImplementedError):
         gpu_returns(env_tc, spec, inp)
 

@@ -10,45 +10,90 @@ from test_gpu_parity import DEV, make_env
 pytestmark = pytest.mark.gpu
 
 
+def _refit_values(N, k, seed):
+    """Returns with every hazard of the selection: NaN (-> -1e-10), +inf among the elites, -inf, and the k-th value in
+    the middle of a run of k exact zeros of both signs, so the selection ends inside a tie."""
+    g = np.random.default_rng(seed)
+    v = g.standard_normal(N).astype(np.float32)
+    order = g.permutation(N)
+    hi, zeros, rest = order[:k // 2], order[k // 2:k // 2 + k], order[k // 2 + k:]
+    v[hi] = np.abs(v[hi]) + 1.0
+    v[hi[:2]] = np.inf
+    v[zeros] = np.where(g.random(zeros.size) < 0.5, np.float32(0.0), np.float32(-0.0))
+    v[rest] = -np.abs(v[rest]) - 1e-3
+    v[rest[:max(3, N // 977)]] = np.nan
+    v[rest[-3:]] = -np.inf
+    return v
+
+
+# (population, dims, k, unbiased, use_std, elites_out): run_select's three kernels --
+#   n <= 2048 with k * dims * 4 <= 150 KB: the single-CTA refit with the elite rows in shared memory;
+#   n <= 2048 with larger elite sets: cem_select_kernel's counting rank (config 3's iCEM refit: pop 1000, k 100, 40 x 17),
+#     and with dims > 1241 its partial sums in the global workspace;
+#   n > 2048: cem_select_kernel's radix select (config 5's scale), again also with global partial sums.
+REFIT_SHAPES = {
+    "single_cta": (500, 180, 50, 1, 0, True),
+    "counting_config3": (1000, 680, 100, 1, 1, True),
+    "counting_global_partials": (1500, 1300, 40, 0, 0, False),
+    "radix_config5": (64000, 36, 6400, 1, 0, False),
+    "radix_global_partials": (5000, 1300, 60, 0, 1, True),
+}
+
+
 def test_large_population_refit_matches_torch():
-    """config 5 scale: N = 64 000, k = 6 400 goes through the radix-select path; torch.topk / mean / var on the device
-    is the checker (library code used as a test oracle only)."""
-    import mbrl_lib_b200 as bp
+    """config 5 scale: N = 64 000, k = 6 400 goes through the radix-select path (checker: _check_refit)."""
+    _check_refit("radix_config5")
+
+
+@pytest.mark.parametrize("branch", [b for b in REFIT_SHAPES if b != "radix_config5"])
+def test_refit_branches_match_float64(branch):
+    """The other kernels run_select dispatches to (see REFIT_SHAPES), with the same checker."""
+    _check_refit(branch)
+
+
+def _check_refit(branch):
+    """b200pets_cem_update against a float64 restatement of trajectory_opt.py:170-186: elites = the first k of the
+    stable order by (-value, index) (the header's "ties broken by lowest index", -0.0 equal to +0.0), momentum-blended
+    mean / (unbiased) variance or std, best value / row, elite rows by descending value."""
     from mbrl_lib_b200 import _lib
 
     lib = _lib.load()
-    N, dims, k, alpha = 64000, 36, 6400, 0.1
-    g = torch.Generator(device=DEV).manual_seed(3)
-    pop = torch.randn(N, dims, device=DEV, generator=g)
-    vals = torch.randn(N, device=DEV, generator=g)
-    vals[::977] = float("nan")
-    vals[5::1000] = 0.25  # ties
-    mu = torch.zeros(dims, device=DEV)
-    disp = torch.ones(dims, device=DEV)
+    N, dims, k, unbiased, use_std, with_elites = REFIT_SHAPES[branch]
+    alpha = 0.1
+    vals = _refit_values(N, k, seed=N + dims)
+    g = np.random.default_rng(dims)
+    pop = g.standard_normal((N, dims)).astype(np.float32)
+    mu0 = g.standard_normal(dims).astype(np.float32)
+    disp0 = (0.5 + g.random(dims)).astype(np.float32)
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(DEV)  # noqa: E731
+    pop_d, v_d, mu, disp = t(pop), t(vals), t(mu0), t(disp0)
     best_v = torch.full((1,), float("-inf"), device=DEV)
     best_s = torch.zeros(dims, device=DEV)
     idx = torch.empty(k, dtype=torch.int32, device=DEV)
+    elites = torch.full((k, dims), float("nan"), device=DEV) if with_elites else None
     nbytes = lib.b200pets_cem_update_workspace_bytes(N, dims, k)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=DEV)
-    v_in = vals.clone()
-    _lib.check(lib.b200pets_cem_update(N, dims, k, alpha, 1, 0, _lib.ptr(pop), _lib.ptr(v_in), _lib.ptr(mu), _lib.ptr(disp),
-                                       _lib.ptr(best_v), _lib.ptr(best_s), _lib.ptr(idx), None, _lib.ptr(ws), nbytes,
-                                       _lib.stream_ptr()))
+    _lib.check(lib.b200pets_cem_update(N, dims, k, alpha, unbiased, use_std, _lib.ptr(pop_d), _lib.ptr(v_d), _lib.ptr(mu),
+                                       _lib.ptr(disp), _lib.ptr(best_v), _lib.ptr(best_s), _lib.ptr(idx), _lib.ptr(elites),
+                                       _lib.ptr(ws), nbytes, _lib.stream_ptr()))
     torch.cuda.synchronize()
-    ref_v = vals.clone()
-    ref_v[ref_v.isnan()] = -1e-10
-    assert torch.equal(v_in, ref_v)  # NaN rule applied in place
-    top_v, _ = ref_v.topk(k)
-    sel = idx.long()
-    assert sel.unique().numel() == k and bool((sel[1:] > sel[:-1]).all())  # k distinct indices, ascending
-    thr = top_v[-1]
-    assert bool((ref_v[sel] >= thr).all())
-    assert torch.allclose(ref_v[sel].sort(descending=True).values, top_v)  # same multiset of values as torch.topk
-    elite = pop[sel]
-    torch.testing.assert_close(mu, (1 - alpha) * elite.mean(0), rtol=1e-4, atol=1e-5)
-    torch.testing.assert_close(disp, alpha * torch.ones(dims, device=DEV) + (1 - alpha) * elite.var(0), rtol=1e-4, atol=1e-5)
-    assert float(best_v) == float(ref_v.max())
-    torch.testing.assert_close(best_s, pop[int(ref_v.argmax())])
+    ref = np.where(np.isnan(vals), np.float32(-1e-10), vals)
+    assert np.array_equal(v_d.cpu().numpy(), ref)  # NaN rule applied in place
+    key = ref + np.float32(0.0)  # -0.0 -> +0.0
+    order = np.lexsort((np.arange(N), -key))  # stable: by descending value, then ascending index
+    want = np.sort(order[:k])
+    got = idx.cpu().numpy()
+    assert np.array_equal(got, want), (f"{np.setdiff1d(got, want).size} selected indices differ; "
+                                       f"values of the extra ones {ref[np.setdiff1d(got, want)][:8]}")
+    elite = pop[order[:k]].astype(np.float64)
+    var = elite.var(0, ddof=1 if unbiased else 0)
+    nd = np.sqrt(var) if use_std else var
+    np.testing.assert_allclose(mu.cpu().numpy(), alpha * mu0 + (1 - alpha) * elite.mean(0), rtol=1e-4, atol=1e-5)
+    np.testing.assert_allclose(disp.cpu().numpy(), alpha * disp0 + (1 - alpha) * nd, rtol=1e-4, atol=1e-5)
+    assert float(best_v) == float(key[order[0]])  # +inf, lowest index of the two
+    assert np.array_equal(best_s.cpu().numpy(), pop[order[0]])
+    if with_elites:  # descending value, lower index first on ties: exactly the stable order's first k rows
+        assert np.array_equal(elites.cpu().numpy(), pop[order[:k]])
 
 
 @pytest.mark.parametrize("precision", ["bf16_tc", "f32"])

@@ -12,6 +12,7 @@ Also here: shard invariance (the property that makes multi-GPU results independe
 distribution-level equivalence of the tile-shuffle law and the reference's randperm law (two-sample KS over 200
 draws each), and ShardedCEMOptimizer == CEMOptimizer on the union population (two shards on one GPU).
 """
+import dataclasses
 import threading
 
 import numpy as np
@@ -42,11 +43,26 @@ def _eval_shuffle(env, spec, inp, offset, shard=(0, 0), rows=False, eps=None, ac
     return (rr if rows else out).cpu().numpy()
 
 
-@pytest.mark.parametrize("precision,tol", [("f32", 2e-4), ("bf16_tc", 5e-3)])
-@pytest.mark.parametrize("name", ["halfcheetah", "pets_halfcheetah_small", "humanoid_trunc", "tc_hid64", "cartpole_pets"])
-def test_tile_shuffle_matches_oracle(name, precision, tol):
+TOL = {"f32": 2e-4, "bf16_tc": 5e-3}
+# (case, precision, population or None for the case's own).  The fp32 kernel splits a 128-row shuffle group into 2, 4 or
+# 8 tiles (64, 32 or 16 rows); the populations of the wide fp32-only models are large enough to fill more than one tile of
+# their group.
+SHUFFLE_CASES = [(n, p, None) for n in ["halfcheetah", "pets_halfcheetah_small", "humanoid_trunc", "tc_hid64", "cartpole_pets"]
+                 for p in ("f32", "bf16_tc")] + \
+                [("plan_f32_hid512", "f32", None), ("humanoid_v4", "f32", 70), ("plan_hid143", "f32", None),
+                 ("plan_hid143", "bf16_tc", None), ("plan_k3", "bf16_tc", None), ("plan_ring2", "bf16_tc", None),
+                 ("plan_k1_out256", "bf16_tc", None), ("plan_hid14_deep", "bf16_tc", None),
+                 ("plan_logvar_extreme", "bf16_tc", None), ("plan_logvar_extreme", "f32", None)]
+
+
+@pytest.mark.parametrize("name,precision,population", SHUFFLE_CASES,
+                         ids=[f"{n}-{p}-{TOL[p]}" + (f"-pop{pop}" if pop else "") for n, p, pop in SHUFFLE_CASES])
+def test_tile_shuffle_matches_oracle(name, precision, population):
+    tol = TOL[precision]
     spec, arrays, env = make_env(name, precision, ts1="tile_shuffle")
     env._few_groups = lambda *a: False  # always the in-kernel draw, also for the small parity cases
+    if population is not None:
+        spec = dataclasses.replace(spec, population=population)
     inp = syn.make_rollout_inputs(spec)
     offset = 7 * 1024
     got = _eval_shuffle(env, spec, inp, offset)
@@ -109,16 +125,22 @@ def test_shard_invariance_bit_exact(precision):
     assert np.isfinite(full).all() and np.unique(full).size > N // 2
 
 
-@pytest.mark.parametrize("precision,tol", [("f32", 5e-4), ("bf16_tc", 5e-3)])
-def test_fused_cem_plan_tile_shuffle_matches_oracle(precision, tol):
+CEM_PLAN_SHAPES = [(p, tol, n, h) for n, h in [(500, 30), (2100, 8)] for p, tol in [("f32", 5e-4), ("bf16_tc", 5e-3)]]
+
+
+@pytest.mark.parametrize("precision,tol,population,horizon", CEM_PLAN_SHAPES,
+                         ids=[f"{p}-{tol}" + ("" if n == 500 else f"-pop{n}-h{h}") for p, tol, n, h in CEM_PLAN_SHAPES])
+def test_fused_cem_plan_tile_shuffle_matches_oracle(precision, tol, population, horizon):
     """b200pets_cem_plan (the call bench.py's `value` times) in its production mode -- tile shuffle -- at config 2's
     full size, population noise and model noise injected, against the oracle's CEM over the oracle rollout with the
-    exported per-iteration member maps."""
+    exported per-iteration member maps.  A population above 2048 takes the plan's other refit: particle mean, then the
+    radix select."""
     import mbrl_lib_b200 as bp
     from mbrl_lib_b200.planning import _FusedObjective
     from oracle import pets_oracle as po
 
     spec, arrays, env = make_env("halfcheetah", precision, ts1="tile_shuffle")
+    spec = dataclasses.replace(spec, population=population, horizon=horizon)
     inp = syn.make_rollout_inputs(spec, with_noise=False)
     iters = 2
     nz = syn.make_cem_noise(spec, iters)

@@ -10,7 +10,7 @@ from mbrl_lib_b200 import synthetic as syn
 from oracle import pets_oracle as po
 
 ROLLOUT_CASES = ["cartpole", "halfcheetah", "halfcheetah_small", "pets_halfcheetah_small", "humanoid_trunc",
-                 "relu_expectation", "silu_expectation", "hopper_tsinf", "cartpole_pets", "pusher_det", "walker_ant", "humanoid_v4", "tc_hid64", "tc_wide", "tc_shallow", "ant_learned_fn"]
+                 "relu_expectation", "silu_expectation", "hopper_tsinf", "cartpole_pets", "pusher_det", "walker_ant", "humanoid_v4", "tc_hid64", "tc_wide", "tc_shallow", "ant_learned_fn"] + syn.PLAN_CASES
 
 
 def _load(golden_dir, name):
