@@ -48,7 +48,7 @@ extern "C" {
 #define B200PETS_REWARD_INVERTED_PENDULUM 3
 #define B200PETS_REWARD_HALFCHEETAH 4
 #define B200PETS_REWARD_PUSHER 5
-#define B200PETS_REWARD_EXTERNAL 255 /* b200pets_step only: reward left to the caller's callable */
+#define B200PETS_REWARD_EXTERNAL 255 /* reward left to the caller's callable (b200pets_step, b200pets_eval_trajectory) */
 
 /* termination_fn: mbrl/env/termination_fns.py */
 #define B200PETS_TERM_NONE 0
@@ -58,7 +58,7 @@ extern "C" {
 #define B200PETS_TERM_WALKER2D 4
 #define B200PETS_TERM_ANT 5
 #define B200PETS_TERM_HUMANOID 6
-#define B200PETS_TERM_EXTERNAL 255 /* b200pets_step only */
+#define B200PETS_TERM_EXTERNAL 255 /* b200pets_step, b200pets_eval_trajectory */
 
 /* uncertainty propagation: mbrl/models/gaussian_mlp.py:179-216 */
 #define B200PETS_PROP_RANDOM_MODEL 0 /* TS1   */
@@ -160,6 +160,28 @@ size_t b200pets_eval_workspace_bytes(b200pets_model_t model, const b200pets_roll
 int b200pets_eval_sequences(b200pets_model_t model, const b200pets_rollout_cfg* cfg, const float* obs0,
                             const float* actions, const int64_t* perms, const float* eps, float* returns,
                             float* row_returns, void* workspace, size_t workspace_bytes, void* stream);
+
+/* evaluate_action_sequences with reward / termination callables the kernels do not know (B200PETS_REWARD_EXTERNAL /
+ * B200PETS_TERM_EXTERNAL; b200pets_eval_sequences refuses those).  The observation trajectory does not depend on reward
+ * or done (model_env.py:178-191), so the evaluation runs in windows of steps [t0, t1), in order, t0 = 0 first:
+ *   1. b200pets_eval_trajectory rolls the model over the window and writes, for local step s = t - t0 and row
+ *      r = n*P + p: next_obs [dev] float[t1-t0][B][D], reward [dev] float[t1-t0][B] (learned column or known function;
+ *      0 for an external one), done [dev] uint8[t1-t0][B] (known function; 0 for an external one).  Each may be NULL.
+ *   2. the caller overwrites reward / done with its callables' values on those rows;
+ *   3. b200pets_trajectory_returns applies the reference's masking (a reward after termination counts 0) and
+ *      accumulates per-row totals in the workspace; after the window with t1 == H it writes returns [dev] float[N]
+ *      (particle mean) and row_returns [dev] float[B] (or NULL).
+ * obs0 (read when t0 == 0), actions, perms, eps and cfg are those of b200pets_eval_sequences and are passed whole for
+ * every window: Philox keys, shuffle groups and shards are the same, so how H is split into windows changes nothing.
+ * One workspace of b200pets_trajectory_workspace_bytes carries the row state from window to window. */
+size_t b200pets_trajectory_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* cfg);
+int b200pets_eval_trajectory(b200pets_model_t model, const b200pets_rollout_cfg* cfg, int32_t t0, int32_t t1,
+                             const float* obs0, const float* actions, const int64_t* perms, const float* eps,
+                             float* next_obs, float* reward, uint8_t* done, void* workspace, size_t workspace_bytes,
+                             void* stream);
+int b200pets_trajectory_returns(const b200pets_rollout_cfg* cfg, int32_t t0, int32_t t1, const float* reward,
+                                const uint8_t* done, float* returns, float* row_returns, void* workspace,
+                                size_t workspace_bytes, void* stream);
 
 /* The member every shuffle group uses at every step when perms == NULL (exactly what the kernels draw; parity
  * tests feed it to the oracle as a per-row member assignment, gaussian_mlp.py:202-212 with the permutation replaced).

@@ -56,6 +56,11 @@ _SIGNATURES = {
     "b200pets_model_plan_info": (C.c_int, [_P, C.c_int32, C.POINTER(C.c_int32)]),
     "b200pets_eval_workspace_bytes": (C.c_size_t, [_P, C.POINTER(RolloutCfg)]),
     "b200pets_eval_sequences": (C.c_int, [_P, C.POINTER(RolloutCfg), _P, _P, _P, _P, _P, _P, _P, C.c_size_t, _P]),
+    "b200pets_trajectory_workspace_bytes": (C.c_size_t, [_P, C.POINTER(RolloutCfg)]),
+    "b200pets_eval_trajectory": (C.c_int, [_P, C.POINTER(RolloutCfg), C.c_int32, C.c_int32, _P, _P, _P, _P, _P, _P, _P, _P,
+                                           C.c_size_t, _P]),
+    "b200pets_trajectory_returns": (C.c_int, [C.POINTER(RolloutCfg), C.c_int32, C.c_int32, _P, _P, _P, _P, _P, C.c_size_t,
+                                              _P]),
     "b200pets_step": (C.c_int, [_P, C.c_int32, C.c_int32, C.c_int64, _P, _P, _P, _P, C.c_uint64, C.c_uint64, C.c_int32,
                                 _P, _P, _P, _P]),
     "b200pets_mbpo_mask": (C.c_int, [C.c_int64, _P, _P, _P, _P]),

@@ -327,34 +327,37 @@ static int dispatch(const b200pets_model_s* mdl, int precision, const RolloutArg
   return b200pets_set_error(B200PETS_EINVAL, "unknown precision %d", precision);
 }
 
+static size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
+
 size_t b200pets_eval_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* cfg) {
   if (!model || !cfg) return 0;
   const size_t B = (size_t)cfg->population * cfg->particles;
-  return ((B * model->desc.obs_dim * sizeof(float) + 255) & ~(size_t)255) + ((B * sizeof(float) + 255) & ~(size_t)255) + ((B + 255) & ~(size_t)255);
+  return al256(B * model->desc.obs_dim * sizeof(float)) + al256(B * sizeof(float)) + al256(B);
 }
 
-// the rollout of one evaluation: per-row totals [B] (row r = n * P + p) in *totals_out, no particle mean
-static int eval_rows(b200pets_model_t model, const b200pets_rollout_cfg* cfg, const float* obs0, const float* actions,
-                     const int64_t* perms, const float* eps, float* row_returns, void* workspace, size_t workspace_bytes,
-                     void* stream_, float** totals_out) {
-  if (!model || !cfg || !obs0 || !actions || !workspace) return b200pets_set_error(B200PETS_EINVAL, "eval_sequences: null argument");
-  cudaStream_t stream = (cudaStream_t)stream_;
+// checks shared by every evaluation entry point
+static int check_eval(b200pets_model_t model, const b200pets_rollout_cfg* cfg, const char* what) {
   const b200pets_model_desc& d = model->desc;
   const int N = cfg->population, H = cfg->horizon, P = cfg->particles;
-  if (N <= 0 || H <= 0 || P <= 0) return b200pets_set_error(B200PETS_EINVAL, "eval_sequences: population, horizon, particles must be positive");
+  if (N <= 0 || H <= 0 || P <= 0) return b200pets_set_error(B200PETS_EINVAL, "%s: population, horizon, particles must be positive", what);
   const long long B = (long long)N * P;
   if (B % d.num_members != 0)  // mbrl/models/gaussian_mlp.py:195-200
     return b200pets_set_error(B200PETS_EINVAL, "GaussianMLP ensemble requires batch size to be a multiple of the number of models. "
                                                "Current batch size is %lld for %d models.", B, d.num_members);
-  if (d.reward_fn == B200PETS_REWARD_EXTERNAL || d.term_fn == B200PETS_TERM_EXTERNAL)
-    return b200pets_set_error(B200PETS_EUNSUPPORTED, "eval_sequences: external reward/termination callables need the per-step API");
-  if (workspace_bytes < b200pets_eval_workspace_bytes(model, cfg)) return b200pets_set_error(B200PETS_EINVAL, "eval_sequences: workspace too small");
-  unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
-  float* obs_state = reinterpret_cast<float*>(ws);
-  size_t o1 = ((size_t)B * d.obs_dim * sizeof(float) + 255) & ~(size_t)255;
-  float* total = row_returns ? row_returns : reinterpret_cast<float*>(ws + o1);
-  uint8_t* dead = ws + o1 + (((size_t)B * sizeof(float) + 255) & ~(size_t)255);
+  return B200PETS_OK;
+}
 
+// Rollout launches for steps [t0, t1) of the evaluation `cfg` describes.  Between launches a row's observation is carried
+// in obs_state [B][D] (stored when keep_obs, or when the window is split into per-step launches); its reward total and
+// dead flag in total / dead when those are given (NULL: the kernel's own accumulation is not kept).  traj_* (or NULL)
+// receive every step's next observation, reward and done at [t - t0][row].
+static int rollout_steps(b200pets_model_t model, const b200pets_rollout_cfg* cfg, int t0, int t1, bool keep_obs,
+                         const float* obs0, const float* actions, const int64_t* perms, const float* eps, float* obs_state,
+                         float* total, uint8_t* dead, float* traj_obs, float* traj_reward, uint8_t* traj_done,
+                         cudaStream_t stream) {
+  const b200pets_model_desc& d = model->desc;
+  const int N = cfg->population, H = cfg->horizon, P = cfg->particles;
+  const long long B = (long long)N * P;
   RolloutArgs a{};
   a.N = N; a.H = H; a.P = P; a.B = B;
   a.propagation = cfg->propagation;
@@ -370,22 +373,26 @@ static int eval_rows(b200pets_model_t model, const b200pets_rollout_cfg* cfg, co
   if (ts1 && perms) {
     // reference TS1: a fresh permutation of all rows every step => rows change member (and tile) between steps;
     // one launch per step, state carried through the workspace
-    for (int t = 0; t < H; ++t) {
+    for (int t = t0; t < t1; ++t) {
       RolloutArgs s = a;
       s.slot_mode = 0;
       s.perm = reinterpret_cast<const long long*>(perms) + (size_t)t * B;
       s.eps = eps ? eps + (size_t)t * B * d.out_size : nullptr;
       s.t0 = t; s.t1 = t + 1;
-      s.init_from_obs0 = t == 0; s.load_state = t > 0; s.store_state = 1;
+      s.init_from_obs0 = t == 0; s.load_state = t > 0 && total; s.store_state = 1;
       s.obs_in = obs_state; s.obs_out = obs_state;
+      s.traj_obs = traj_obs ? traj_obs + (size_t)(t - t0) * B * d.obs_dim : nullptr;
+      s.traj_reward = traj_reward ? traj_reward + (size_t)(t - t0) * B : nullptr;
+      s.traj_done = traj_done ? traj_done + (size_t)(t - t0) * B : nullptr;
       int rc = dispatch(model, precision, s, stream);
       if (rc) return rc;
     }
   } else {
-    a.t0 = 0; a.t1 = H;
-    a.eps = eps;
-    a.init_from_obs0 = 1; a.load_state = 0; a.store_state = 1;
-    a.obs_in = nullptr; a.obs_out = nullptr;
+    a.t0 = t0; a.t1 = t1;
+    a.eps = eps ? eps + (size_t)t0 * B * d.out_size : nullptr;
+    a.init_from_obs0 = t0 == 0; a.load_state = t0 > 0 && total; a.store_state = 1;
+    a.obs_in = t0 == 0 ? nullptr : obs_state; a.obs_out = keep_obs ? obs_state : nullptr;
+    a.traj_obs = traj_obs; a.traj_reward = traj_reward; a.traj_done = traj_done;
     if (cfg->propagation == B200PETS_PROP_EXPECTATION) {
       a.slot_mode = 0; a.perm = nullptr;
     } else if (perms) {  // TSinf with the reset permutation
@@ -396,8 +403,100 @@ static int eval_rows(b200pets_model_t model, const b200pets_rollout_cfg* cfg, co
     int rc = dispatch(model, precision, a, stream);
     if (rc) return rc;
   }
+  return B200PETS_OK;
+}
+
+// the rollout of one evaluation: per-row totals [B] (row r = n * P + p) in *totals_out, no particle mean
+static int eval_rows(b200pets_model_t model, const b200pets_rollout_cfg* cfg, const float* obs0, const float* actions,
+                     const int64_t* perms, const float* eps, float* row_returns, void* workspace, size_t workspace_bytes,
+                     void* stream_, float** totals_out) {
+  if (!model || !cfg || !obs0 || !actions || !workspace) return b200pets_set_error(B200PETS_EINVAL, "eval_sequences: null argument");
+  const b200pets_model_desc& d = model->desc;
+  { int rc = check_eval(model, cfg, "eval_sequences"); if (rc) return rc; }
+  if (d.reward_fn == B200PETS_REWARD_EXTERNAL || d.term_fn == B200PETS_TERM_EXTERNAL)
+    return b200pets_set_error(B200PETS_EUNSUPPORTED, "eval_sequences: external reward/termination callables cannot run inside "
+                                                     "this call; use b200pets_eval_trajectory, the callable, then b200pets_trajectory_returns");
+  if (workspace_bytes < b200pets_eval_workspace_bytes(model, cfg)) return b200pets_set_error(B200PETS_EINVAL, "eval_sequences: workspace too small");
+  const size_t B = (size_t)cfg->population * cfg->particles;
+  unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
+  float* obs_state = reinterpret_cast<float*>(ws);
+  const size_t o1 = al256(B * d.obs_dim * sizeof(float));
+  float* total = row_returns ? row_returns : reinterpret_cast<float*>(ws + o1);
+  uint8_t* dead = ws + o1 + al256(B * sizeof(float));
+  int rc = rollout_steps(model, cfg, 0, cfg->horizon, false, obs0, actions, perms, eps, obs_state, total, dead, nullptr, nullptr,
+                         nullptr, (cudaStream_t)stream_);
+  if (rc) return rc;
   *totals_out = total;
   return B200PETS_OK;
+}
+
+namespace {
+// model_env.py:183-188 over the steps of one window: a reward after termination is replaced (a select: NaN / inf
+// cannot leak), then the row dies, then the reward is added.  Same order of operations as the rollout kernels.
+__global__ void trajectory_returns_kernel(long long B, int T, int first, const float* __restrict__ reward,
+                                          const uint8_t* __restrict__ done, float* total, uint8_t* dead,
+                                          float* __restrict__ row_out) {
+  const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= B) return;
+  float tot = first ? 0.f : total[r];
+  int dd = first ? 0 : (int)dead[r];
+  for (int t = 0; t < T; ++t) {
+    const float rew = reward[(size_t)t * B + r];
+    tot += dd ? 0.f : rew;
+    dd |= done[(size_t)t * B + r] != 0;
+  }
+  total[r] = tot;
+  dead[r] = (uint8_t)dd;
+  if (row_out) row_out[r] = tot;
+}
+}  // namespace
+
+// trajectory workspace: reward totals [B], dead flags [B], then the carried observations [B][D] (the returns call does
+// not know D, so the per-row scalars come first)
+size_t b200pets_trajectory_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* cfg) {
+  if (!model || !cfg) return 0;
+  const size_t B = (size_t)cfg->population * cfg->particles;
+  return al256(B * sizeof(float)) + al256(B) + al256(B * model->desc.obs_dim * sizeof(float));
+}
+
+int b200pets_eval_trajectory(b200pets_model_t model, const b200pets_rollout_cfg* cfg, int32_t t0, int32_t t1,
+                             const float* obs0, const float* actions, const int64_t* perms, const float* eps,
+                             float* next_obs, float* reward, uint8_t* done, void* workspace, size_t workspace_bytes,
+                             void* stream) {
+  if (!model || !cfg || !actions || !workspace || (t0 == 0 && !obs0))
+    return b200pets_set_error(B200PETS_EINVAL, "eval_trajectory: null argument");
+  { int rc = check_eval(model, cfg, "eval_trajectory"); if (rc) return rc; }
+  if (t0 < 0 || t1 <= t0 || t1 > cfg->horizon)
+    return b200pets_set_error(B200PETS_EINVAL, "eval_trajectory: steps [%d, %d) outside the horizon %d", t0, t1, cfg->horizon);
+  if (workspace_bytes < b200pets_trajectory_workspace_bytes(model, cfg))
+    return b200pets_set_error(B200PETS_EINVAL, "eval_trajectory: workspace too small");
+  const size_t B = (size_t)cfg->population * cfg->particles;
+  float* obs_state = reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(workspace) + al256(B * sizeof(float)) + al256(B));
+  return rollout_steps(model, cfg, t0, t1, t1 < cfg->horizon, obs0, actions, perms, eps, obs_state, nullptr, nullptr, next_obs,
+                       reward, done, (cudaStream_t)stream);
+}
+
+int b200pets_trajectory_returns(const b200pets_rollout_cfg* cfg, int32_t t0, int32_t t1, const float* reward,
+                                const uint8_t* done, float* returns, float* row_returns, void* workspace,
+                                size_t workspace_bytes, void* stream_) {
+  if (!cfg || !reward || !done || !workspace) return b200pets_set_error(B200PETS_EINVAL, "trajectory_returns: null argument");
+  const int N = cfg->population, H = cfg->horizon, P = cfg->particles;
+  if (N <= 0 || H <= 0 || P <= 0)
+    return b200pets_set_error(B200PETS_EINVAL, "trajectory_returns: population, horizon, particles must be positive");
+  if (t0 < 0 || t1 <= t0 || t1 > H)
+    return b200pets_set_error(B200PETS_EINVAL, "trajectory_returns: steps [%d, %d) outside the horizon %d", t0, t1, H);
+  const long long B = (long long)N * P;
+  if (workspace_bytes < al256((size_t)B * sizeof(float)) + al256((size_t)B))
+    return b200pets_set_error(B200PETS_EINVAL, "trajectory_returns: workspace too small");
+  if (t1 == H && !returns) return b200pets_set_error(B200PETS_EINVAL, "trajectory_returns: null returns on the last window");
+  cudaStream_t stream = (cudaStream_t)stream_;
+  float* total = reinterpret_cast<float*>(workspace);
+  uint8_t* dead = reinterpret_cast<unsigned char*>(workspace) + al256((size_t)B * sizeof(float));
+  trajectory_returns_kernel<<<(unsigned)((B + 255) / 256), 256, 0, stream>>>(B, t1 - t0, t0 == 0, reward, done, total, dead,
+                                                                             t1 == H ? row_returns : nullptr);
+  CUDA_TRY(cudaGetLastError());
+  if (t1 < H) return B200PETS_OK;
+  return launch_particle_mean(N, P, total, returns, stream);  // model_env.py:190-191
 }
 
 int b200pets_eval_sequences(b200pets_model_t model, const b200pets_rollout_cfg* cfg, const float* obs0,
@@ -459,8 +558,6 @@ __global__ void cem_init_kernel(int dims, const float* __restrict__ x0, const fl
   disp[d] = clipped ? 1.0f : (w * w) / 16.0f;  // trajectory_opt.py:100-108
 }
 }  // namespace
-
-static size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 size_t b200pets_cem_plan_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg) {
   if (!model || !rcfg || !ccfg) return 0;

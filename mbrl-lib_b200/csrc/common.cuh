@@ -65,6 +65,10 @@ struct RolloutArgs {
   // step outputs (b200pets_step): next_obs = obs_out, reward, done
   float* reward_out;       // [B] or NULL
   uint8_t* done_out;       // [B] or NULL
+  // trajectory outputs (b200pets_eval_trajectory): step t of the launch lands at [t - t0][rid]; NULL = not stored
+  float* traj_obs;         // [t1-t0][B][D] next observation
+  float* traj_reward;      // [t1-t0][B] the learned column or the known reward function, 0 for an external one
+  uint8_t* traj_done;      // [t1-t0][B] the known termination function, 0 for an external one
   // ---- fused CEM iteration (tensor-core kernel only): population sampled in-kernel, refit by the last CTA ----
   const float* cem_mu;     // [H*A] sampling mean; non-NULL switches the action source to in-kernel sampling
   const float* cem_disp;   // [H*A] variance (truncated normal) or std (clipped normal)

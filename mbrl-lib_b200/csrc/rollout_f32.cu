@@ -274,10 +274,18 @@ __global__ void __launch_bounds__(kThreads) rollout_f32_kernel(const ModelDev m,
       bool done = term_eval(m.term_fn, obs_s + i * m.D, m.D, 1);
       if (a.reward_out) a.reward_out[rid_s[i]] = rew;
       if (a.done_out) a.done_out[rid_s[i]] = done ? 1 : 0;
+      const size_t tr = (size_t)(t - a.t0) * a.B + rid_s[i];
+      if (a.traj_reward) a.traj_reward[tr] = rew;
+      if (a.traj_done) a.traj_done[tr] = done ? 1 : 0;
       if (dead_s[i]) rew = 0.f;
       dead_s[i] |= done ? 1 : 0;
       tot_s[i] += rew;
     }
+    if (a.traj_obs)
+      for (int idx = tid; idx < nv * m.D; idx += kThreads) {
+        const int i = idx / m.D, d = idx % m.D;
+        if (rid_s[i] >= 0) a.traj_obs[((size_t)(t - a.t0) * a.B + rid_s[i]) * m.D + d] = obs_s[idx];
+      }
     __syncthreads();
   }
   // ---- store state ------------------------------------------------------------------------------

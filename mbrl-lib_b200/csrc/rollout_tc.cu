@@ -355,8 +355,11 @@ static __device__ __noinline__ void cem_tail_refit(const TailArgs* ap, int dims,
   }
 }
 
-template <int ACT, bool CEMF, bool EXP = false>  // EXP: propagation "expectation" (member passes)
-                                                // CEMF: fused-CEM features compiled in (in-kernel sampling, last-CTA refit)
+template <int ACT, bool CEMF, bool EXP = false, bool TRAJ = false>
+// EXP: propagation "expectation" (member passes)
+// CEMF: fused-CEM features compiled in (in-kernel sampling, last-CTA refit)
+// TRAJ: per-step trajectory stores compiled in (b200pets_eval_trajectory); the other variants are compiled without them
+//       so that their schedule stays what it was
 __global__ void __launch_bounds__(kThreads, 1)
 rollout_tc_kernel(const __grid_constant__ ModelDev m, const __grid_constant__ RolloutArgs a, const __grid_constant__ TcPlan p,
                   const long long num_tiles) {
@@ -641,6 +644,15 @@ rollout_tc_kernel(const __grid_constant__ ModelDev m, const __grid_constant__ Ro
             if (a.reward_out) a.reward_out[rid] = rew;
             if (a.done_out) a.done_out[rid] = done ? 1 : 0;
           }
+          if (TRAJ && valid) {
+            const size_t tr = (size_t)(t - a.t0) * a.B + rid;
+            if (a.traj_reward) a.traj_reward[tr] = rew;
+            if (a.traj_done) a.traj_done[tr] = done ? 1 : 0;
+            if (a.traj_obs) {
+#pragma unroll 1
+              for (int d = 0; d < m.D; ++d) a.traj_obs[tr * m.D + d] = my_obs[d];
+            }
+          }
           if (dead) rew = 0.f;
           dead |= done ? 1 : 0;
           tot += rew;
@@ -846,6 +858,14 @@ int tc_plan_info(const ModelDev& m, bool expectation, int* kslice, int* nstages,
   return B200PETS_OK;
 }
 
+// the variant with per-step trajectory stores (b200pets_eval_trajectory) for an activation
+template <bool EXP>
+static void (*traj_kernel(int act))(const ModelDev, const RolloutArgs, const TcPlan, const long long) {
+  return act == B200PETS_ACT_SILU   ? rollout_tc_kernel<B200PETS_ACT_SILU, false, EXP, true>
+         : act == B200PETS_ACT_RELU ? rollout_tc_kernel<B200PETS_ACT_RELU, false, EXP, true>
+                                    : rollout_tc_kernel<B200PETS_ACT_LEAKY_RELU, false, EXP, true>;
+}
+
 int launch_rollout_tc(const ModelDev& m, const RolloutArgs& a, cudaStream_t stream) {
   int rc = tc_device_limits();
   if (rc) return rc;
@@ -883,6 +903,10 @@ int launch_rollout_tc(const ModelDev& m, const RolloutArgs& a, cudaStream_t stre
         kern = cemf ? rollout_tc_kernel<B200PETS_ACT_LEAKY_RELU, true> : rollout_tc_kernel<B200PETS_ACT_LEAKY_RELU, false>;
         break;
     }
+  }
+  if (a.traj_obs || a.traj_reward || a.traj_done) {
+    if (cemf) return b200pets_set_error(B200PETS_EUNSUPPORTED, "fused CEM iteration has no trajectory outputs");
+    kern = expect ? traj_kernel<true>(m.act) : traj_kernel<false>(m.act);
   }
   const size_t smem_launch = (size_t)p.smem_bytes + (cemf ? (size_t)2 * kCemTabDims * sizeof(float) : 0);
   CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_launch));

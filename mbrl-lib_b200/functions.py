@@ -4,8 +4,9 @@ The reference passes these as Python callables (``reward_fn(act, next_obs)``, ``
 next_obs)``, ``obs_process_fn(obs)``; mbrl/env/reward_fns.py, mbrl/env/termination_fns.py,
 mbrl/env/pets_halfcheetah.py:91-121, mbrl/env/pets_cartpole.py:78-101).  The kernels implement the shipped
 ones as device functions selected by id; :func:`resolve_reward` / :func:`resolve_term` map a callable (ours
-or mbrl-lib's own, matched by module + name) to that id.  Anything else is "external": the per-step kernel
-still advances the model and the caller's callable is applied to its device tensors.
+or mbrl-lib's own, matched by module + name) to that id.  Anything else is "external": the kernels still
+advance the model and the caller's callable is applied to their device tensors (per step in ``ModelEnv.step``, per
+window of steps in ``ModelEnv.evaluate_action_sequences``).
 
 The torch bodies below are the host-visible definitions of the same functions (used for external/hybrid
 evaluation and by users who want the callables); they run on whatever device their inputs live on.

@@ -252,10 +252,21 @@ class ModelEnv:
     def render(self, mode="human"):
         pass
 
+    def has_external_callables(self) -> bool:
+        """True when the reward or the termination function is a callable the kernels do not know: evaluations then run
+        the rollout in windows and apply the callable once per window (see :meth:`evaluate_action_sequences`)."""
+        d = self.staged.desc
+        return d.reward_fn == _lib.REWARD["external"] or d.term_fn == _lib.TERM["external"]
+
     def evaluate_action_sequences(self, action_sequences: torch.Tensor, initial_state: np.ndarray, num_particles: int, *,
                                   _perms: Optional[torch.Tensor] = None, _eps: Optional[torch.Tensor] = None,
                                   _row_returns: Optional[torch.Tensor] = None, _offset: Optional[int] = None,
-                                  _shard=(0, 0)) -> torch.Tensor:
+                                  _shard=(0, 0), _window: Optional[int] = None) -> torch.Tensor:
+        """model_env.py:145-191.  Known reward / termination functions run inside the rollout kernel.  A callable the
+        kernels do not know is applied to whole windows of steps: the kernel writes every step's next observation, then
+        ``reward_fn(act, next_obs)`` / ``termination_fn(act, next_obs)`` are called ONCE per window on all its T * B rows
+        (fp32 device tensors, rows in the reference's order: step-major, then ``n * P + p``).  Such callables must
+        therefore compute each row from that row alone, as all of mbrl-lib's reward and termination functions do."""
         with torch.no_grad():
             assert len(action_sequences.shape) == 3  # model_env.py:166
             population_size, horizon, action_dim = action_sequences.shape
@@ -263,9 +274,6 @@ class ModelEnv:
             if initial_state.ndim != 1:
                 raise NotImplementedError("pixel observations are outside the GaussianMLP hot path")
             self._fresh()
-            d = self.staged.desc
-            if d.reward_fn == _lib.REWARD["external"] or d.term_fn == _lib.TERM["external"]:
-                return self._evaluate_stepwise(action_sequences, initial_state, num_particles)
             actions = action_sequences.to(self.device, torch.float32).contiguous()
             prop = self._propagation()
             perms = _perms
@@ -285,10 +293,13 @@ class ModelEnv:
                                   self._call_offset() if _offset is None else _offset, int(_shard[0]), int(_shard[1]))
             obs0 = self._obs_to_device(initial_state)
             returns = torch.empty(population_size, dtype=torch.float32, device=self.device)
-            need = self.lib.b200pets_eval_workspace_bytes(self.staged.handle, C.byref(cfg))
-            ws = self._workspace(need)
             if perms is not None:
                 perms = perms.to(torch.int64).contiguous()
+            if self.has_external_callables():
+                self._evaluate_with_callables(cfg, actions, obs0, perms, _eps, returns, _row_returns, _window)
+                return returns
+            need = self.lib.b200pets_eval_workspace_bytes(self.staged.handle, C.byref(cfg))
+            ws = self._workspace(need)
             with torch.cuda.device(self.device):
                 _lib.check(self.lib.b200pets_eval_sequences(
                     self.staged.handle, C.byref(cfg), _lib.ptr(obs0), _lib.ptr(actions), _lib.ptr(perms), _lib.ptr(_eps),
@@ -296,23 +307,48 @@ class ModelEnv:
                     "eval_sequences")
             return returns
 
-    def _evaluate_stepwise(self, action_sequences, initial_state, num_particles):
-        """evaluate_action_sequences for user callables the kernels do not know: model step on the GPU kernel,
-        reward / termination through the caller's torch functions (model_env.py:170-191 verbatim semantics)."""
-        population_size, horizon, _ = action_sequences.shape
-        tiling = (num_particles * population_size,) + (1,) * initial_state.ndim
-        obs_batch = np.tile(initial_state, tiling).astype(np.float32)
-        keep = self._return_as_np
-        state = self.reset(obs_batch, return_as_np=False)
-        B = obs_batch.shape[0]
-        total = torch.zeros(B, 1, device=self.device)
-        terminated = torch.zeros(B, 1, dtype=torch.bool, device=self.device)
-        for t in range(horizon):
-            a = torch.repeat_interleave(action_sequences[:, t, :].to(self.device), num_particles, dim=0)
-            _, rewards, dones, state = self.step(a, state, sample=True)
-            rewards = rewards.clone()
-            rewards[terminated] = 0
-            terminated |= dones
-            total += rewards
-        self._return_as_np = keep
-        return total.reshape(-1, num_particles).mean(dim=1)
+    def _evaluate_with_callables(self, cfg, actions, obs0, perms, eps, returns, row_returns, window):
+        """The evaluation ``cfg`` describes with the caller's reward / termination callables: per window of T steps one
+        trajectory launch (next observations, kernel-side reward / done), the callables on the window's T * B rows, and
+        the masking / accumulation kernel (model_env.py:178-191).  The row state stays in one workspace throughout."""
+        N, H, A = actions.shape
+        P = cfg.particles
+        B, D = N * P, self.staged.desc.obs_dim
+        T = trajectory_window(B, D, A, H) if window is None else max(1, min(int(window), H))
+        ws = self._workspace(self.lib.b200pets_trajectory_workspace_bytes(self.staged.handle, C.byref(cfg)))
+        next_obs = torch.empty(T, B, D, dtype=torch.float32, device=self.device)
+        reward = torch.empty(T, B, dtype=torch.float32, device=self.device)
+        done = torch.empty(T, B, dtype=torch.uint8, device=self.device)
+        ext_reward = self.staged.desc.reward_fn == _lib.REWARD["external"]
+        ext_term = self.staged.desc.term_fn == _lib.TERM["external"]
+        with torch.cuda.device(self.device):
+            for t0 in range(0, H, T):
+                t1 = min(t0 + T, H)
+                rows = (t1 - t0) * B
+                _lib.check(self.lib.b200pets_eval_trajectory(
+                    self.staged.handle, C.byref(cfg), t0, t1, _lib.ptr(obs0), _lib.ptr(actions), _lib.ptr(perms),
+                    _lib.ptr(eps), _lib.ptr(next_obs), _lib.ptr(reward), _lib.ptr(done), _lib.ptr(ws), ws.numel(),
+                    _lib.stream_ptr()), "eval_trajectory")
+                # the reference's action batch of each step, torch.repeat_interleave over particles (model_env.py:181)
+                act = actions[:, t0:t1].transpose(0, 1).repeat_interleave(P, dim=1).reshape(rows, A)
+                nobs = next_obs[:t1 - t0].view(rows, D)
+                if ext_reward:
+                    reward[:t1 - t0].view(rows).copy_(self.reward_fn(act, nobs).reshape(rows))
+                if ext_term:
+                    done[:t1 - t0].view(rows).copy_(self.termination_fn(act, nobs).reshape(rows))
+                _lib.check(self.lib.b200pets_trajectory_returns(
+                    C.byref(cfg), t0, t1, _lib.ptr(reward), _lib.ptr(done), _lib.ptr(returns), _lib.ptr(row_returns),
+                    _lib.ptr(ws), ws.numel(), _lib.stream_ptr()), "trajectory_returns")
+
+
+# Device memory one window of an evaluation with external callables may take for its next observations, actions, rewards
+# and done flags: long horizons over large populations are split so that these stay bounded.
+TRAJECTORY_WINDOW_BYTES = 256 << 20
+
+
+def trajectory_window(batch: int, obs_dim: int, act_dim: int, horizon: int,
+                      budget: int = TRAJECTORY_WINDOW_BYTES) -> int:
+    """Steps per window: as many as fit ``budget`` bytes of fp32 next observations and actions, fp32 rewards and uint8
+    done flags for ``batch`` rows each, at least 1 and at most ``horizon``."""
+    per_step = batch * (4 * obs_dim + 4 * act_dim + 4 + 1)
+    return max(1, min(horizon, budget // max(per_step, 1)))

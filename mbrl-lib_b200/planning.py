@@ -8,6 +8,8 @@
 * When ``obj_fun`` is the ``evaluate_action_sequences`` closure built by
   :func:`create_trajectory_optim_agent_for_model`, ``CEMOptimizer`` runs the whole optimisation as one
   C call (``b200pets_cem_plan``): every iteration's sample -> rollout -> refit is enqueued back to back.
+  With a reward or termination callable the kernels do not know it runs the per-iteration loop instead, the
+  objective applying the callable to windows of the rollout (``ModelEnv.evaluate_action_sequences``).
 * ``TrajectoryOptimizer`` / ``TrajectoryOptimizerAgent`` / ``create_trajectory_optim_agent_for_model``:
   reference semantics (warm-start shift, action cache, RuntimeError when the eval fn is unset).
 """
@@ -112,7 +114,9 @@ class CEMOptimizer(Optimizer):
                  callback: Optional[Callable[[torch.Tensor, torch.Tensor, int], None]] = None, *,
                  _noise: Optional[torch.Tensor] = None, _model_noise=None, **kwargs) -> torch.Tensor:
         x0 = x0.to(self.device, torch.float32).contiguous()
-        if isinstance(obj_fun, _FusedObjective) and callback is None:
+        # the fused plan runs every iteration inside one C call, which cannot call back into Python: with a reward or
+        # termination callable the kernels do not know, the loop below evaluates through the objective instead
+        if isinstance(obj_fun, _FusedObjective) and callback is None and not obj_fun.model_env.has_external_callables():
             return self._optimize_fused(obj_fun, x0, _noise, _model_noise)
         shape = tuple(x0.shape)
         dims = int(np.prod(shape))
