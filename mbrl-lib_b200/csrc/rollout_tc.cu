@@ -1,20 +1,24 @@
 // Tensor-core rollout of the ensemble MLP on sm_90a: bf16 operands, fp32 accumulation in registers (wgmma).
 //
-// One persistent CTA per SM walks 128-row tiles through steps [t0, t1) of the horizon without leaving the chip:
+// Persistent CTAs walk row tiles through steps [t0, t1) of the horizon without leaving the chip.  A CTA has NWG consumer
+// warpgroups and owns 64 * NWG rows.  NWG = 2: one CTA per SM, a whole 128-row tile.  NWG = 1: two CTAs per SM, each one
+// half of a 128-row tile; the two interleave their MMAs, epilogues and barrier waits without an explicit schedule, but
+// each streams its own copy of the weights.  NWG = 1 is used for launches with fewer 128-row tiles than SMs (the other
+// shape would leave SMs idle) whose plan fits twice in an SM's shared memory:
 //  * row state (observation, return, dead flag, actions) stays in shared memory / registers;
-//  * two consumer warpgroups own 64 rows each.  A layer is a chain of wgmma.mma_async (M=64, K=16, N <= 128 per
+//  * each consumer warpgroup owns 64 rows.  A layer is a chain of wgmma.mma_async (M=64, K=16, N <= 128 per
 //    instruction, two instructions per K step for layers wider than 128) that reads the warpgroup's activations from
 //    its own shared-memory operand buffer; the accumulators stay in registers until the layer's last K step, then the
 //    epilogue writes the activated, bf16-packed columns back into the same buffer (the next layer's A operand) or, for
 //    the output layer, the fp32 accumulators into a staging area that aliases it;
 //  * the B operand (weights) is streamed from the L2-resident packed image in K slices of up to 4 x 16 rows
 //    by 1-D TMA bulk copies (cp.async.bulk + mbarrier expect_tx) into a ring of shared-memory slots: a producer warp
-//    keeps the ring full across layers, steps and tiles, and a slot is released as soon as both warpgroups' MMAs that
+//    keeps the ring full across layers, steps and tiles, and a slot is released as soon as every warpgroup's MMAs that
 //    read it have completed (wgmma.wait_group 1);
 //  * propagation "expectation" runs M member passes per step.
 //
-// Warp roles (256 + 32 threads): warps 0-3 = warpgroup 0 (tile rows 0-63), warps 4-7 = warpgroup 1 (rows 64-127),
-// warp 8 = weight producer (one lane).  Thread (row r, half h) of a warpgroup builds / samples half of the row's
+// Warp roles (128 NWG + 32 threads): warps 0-3 = warpgroup 0 (CTA rows 0-63), warps 4-7 = warpgroup 1 (rows 64-127,
+// NWG = 2 only), warp 4 * NWG (4 or 8) = weight producer (one lane).  Thread (row r, half h) of a warpgroup builds / samples half of the row's
 // columns; half 0 owns the row's scalar state.
 //
 // Bias is folded into the GEMM: every A tile carries two constant-one columns after the real inputs and the
@@ -29,6 +33,7 @@
 using namespace sm90;
 
 struct TcPlan {
+  int nwg;              // consumer warpgroups per CTA: 1 (64 rows, two CTAs per SM) or 2 (128 rows, one CTA per SM)
   int nlayers;
   int kp_max;           // widest layer input (K columns of the operand buffers)
   int kslice;           // K steps (16 rows of the weight image each) per ring slot
@@ -39,18 +44,20 @@ struct TcPlan {
   uint32_t off_A, off_ring, off_obs, off_act, off_const, off_cout, off_bar;
   int obs_ld, act_ld;
   uint32_t smem_bytes;
-  uint32_t off_exp;  // [128][exp_ld] member sums of mean / log2-variance terms (propagation "expectation" launches only)
+  uint32_t off_exp;  // [rows][exp_ld] member sums of mean / log2-variance terms (propagation "expectation" launches only)
   int exp_ld;
 };
 
 namespace {
 
-constexpr int kTileM = 128;
-constexpr int kThreads = 256 + 32;
+constexpr int kTileM = 128;  // rows of a tile: a shuffle group, a member's slot range chunk, an expectation chunk
+template <int NWG>
+constexpr int threads_of() { return 128 * NWG + 32; }
+constexpr int kTailWarps = 9;  // cem_tail_refit's reduction order: partial sums over 9 strided element sets
 constexpr int kSliceK16 = 4;       // longest ring slot in K steps (16 rows of the weight image each)
 constexpr int kMaxStages = 16;
 constexpr int kCemTabDims = 1024;  // horizon * act_dim supported by the fused CEM iteration
-constexpr uint32_t kTailScratch = 256 + 2048 * 9 + (kThreads / 32 + 1) * kCemTabDims * 4;  // cem_tail_refit's scratch
+constexpr uint32_t kTailScratch = 256 + 2048 * 9 + (kTailWarps + 1) * kCemTabDims * 4;  // cem_tail_refit's scratch
 
 __device__ __forceinline__ float tanh_approx(float x) {
   float y;
@@ -283,7 +290,7 @@ static __device__ __noinline__ void cem_tail_refit(const TailArgs* ap, int dims,
   float* sv = reinterpret_cast<float*>(scratch);
   int* eidx = reinterpret_cast<int*>(sv + 2048);
   unsigned char* sf = reinterpret_cast<unsigned char*>(eidx + 2048);
-  float* partial = reinterpret_cast<float*>(sf + 2048);  // [nwarp + 1][dims]
+  float* partial = reinterpret_cast<float*>(sf + 2048);  // [kTailWarps + 1][dims]
   for (int i = tid; i < n; i += nthr) {
     float s = 0.f;
     for (int pp = 0; pp < P; ++pp) s += a.total_state[(size_t)i * P + pp];
@@ -315,33 +322,36 @@ static __device__ __noinline__ void cem_tail_refit(const TailArgs* ap, int dims,
   const int bi = *sh_best;
   const float bv = sv[bi];
   const float* pop = a.pop_out;
-  for (int d = lane; d < dims; d += 32) {
-    float acc = 0.f;
-    for (int e = warp; e < k; e += nwarp) acc += pop[(size_t)eidx[e] * dims + d];
-    partial[warp * dims + d] = acc;
-  }
+  // elite sums in kTailWarps strided partial sums whatever the CTA's warp count: the same order at every CTA shape
+  for (int w = warp; w < kTailWarps; w += nwarp)
+    for (int d = lane; d < dims; d += 32) {
+      float acc = 0.f;
+      for (int e = w; e < k; e += kTailWarps) acc += pop[(size_t)eidx[e] * dims + d];
+      partial[w * dims + d] = acc;
+    }
   __syncthreads();
   for (int d = tid; d < dims; d += nthr) {
     float acc = 0.f;
-    for (int w = 0; w < nwarp; ++w) acc += partial[w * dims + d];
-    partial[nwarp * dims + d] = acc / (float)k;
+    for (int w = 0; w < kTailWarps; ++w) acc += partial[w * dims + d];
+    partial[kTailWarps * dims + d] = acc / (float)k;
   }
   __syncthreads();
-  for (int d = lane; d < dims; d += 32) {
-    const float mean = partial[nwarp * dims + d];
-    float acc = 0.f;
-    for (int e = warp; e < k; e += nwarp) {
-      const float df = pop[(size_t)eidx[e] * dims + d] - mean;
-      acc += df * df;
+  for (int w = warp; w < kTailWarps; w += nwarp)
+    for (int d = lane; d < dims; d += 32) {
+      const float mean = partial[kTailWarps * dims + d];
+      float acc = 0.f;
+      for (int e = w; e < k; e += kTailWarps) {
+        const float df = pop[(size_t)eidx[e] * dims + d] - mean;
+        acc += df * df;
+      }
+      partial[w * dims + d] = acc;
     }
-    partial[warp * dims + d] = acc;
-  }
   __syncthreads();
   const bool better = bv > *a.tail_best_value;
   for (int d = tid; d < dims; d += nthr) {
     float acc = 0.f;
-    for (int w = 0; w < nwarp; ++w) acc += partial[w * dims + d];
-    const float mean = partial[nwarp * dims + d];
+    for (int w = 0; w < kTailWarps; ++w) acc += partial[w * dims + d];
+    const float mean = partial[kTailWarps * dims + d];
     const float var = acc / (float)(k - 1);
     const float nd = a.cem_clipped ? sqrtf(var) : var;
     a.tail_mu[d] = a.tail_alpha * a.tail_mu[d] + (1.0f - a.tail_alpha) * mean;
@@ -355,12 +365,14 @@ static __device__ __noinline__ void cem_tail_refit(const TailArgs* ap, int dims,
   }
 }
 
-template <int ACT, bool CEMF, bool EXP = false, bool TRAJ = false>
+template <int ACT, bool CEMF, bool EXP = false, bool TRAJ = false, int NWG = 2>
 // EXP: propagation "expectation" (member passes)
 // CEMF: fused-CEM features compiled in (in-kernel sampling, last-CTA refit)
 // TRAJ: per-step trajectory stores compiled in (b200pets_eval_trajectory); the other variants are compiled without them
 //       so that their schedule stays what it was
-__global__ void __launch_bounds__(kThreads, 1)
+// NWG: consumer warpgroups (TcPlan::nwg).  CTA tile u is half u % 2 of 128-row tile u / 2 when NWG = 1, tile u itself
+//      when NWG = 2; either way a row keeps its member, keys, operands and K order.
+__global__ void __launch_bounds__(threads_of<NWG>(), NWG == 1 ? 2 : 1)
 rollout_tc_kernel(const __grid_constant__ ModelDev m, const __grid_constant__ RolloutArgs a, const __grid_constant__ TcPlan p,
                   const long long num_tiles) {
   extern __shared__ __align__(128) uint8_t smem[];
@@ -376,6 +388,8 @@ rollout_tc_kernel(const __grid_constant__ ModelDev m, const __grid_constant__ Ro
   uint64_t* bar_full = reinterpret_cast<uint64_t*>(smem + p.off_bar);
   uint64_t* bar_empty = bar_full + kMaxStages;
 
+  constexpr int kThreads = threads_of<NWG>();
+  constexpr int kSplit = 2 / NWG;  // CTA tiles per 128-row tile
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int S = p.nstages;
   // Programmatic dependent launch (common.cuh): let the next kernel of the chain become resident now; everything up
@@ -387,7 +401,7 @@ rollout_tc_kernel(const __grid_constant__ ModelDev m, const __grid_constant__ Ro
   if (threadIdx.x == 0) {
     for (int s = 0; s < S; ++s) {
       mbar_init(&bar_full[s], 1);
-      mbar_init(&bar_empty[s], 8);  // one arrival per consumer warp
+      mbar_init(&bar_empty[s], 4 * NWG);  // one arrival per consumer warp
     }
     mbar_fence_init();
   }
@@ -430,12 +444,13 @@ rollout_tc_kernel(const __grid_constant__ ModelDev m, const __grid_constant__ Ro
   const int nlayers = p.nlayers;
   const int L = nlayers - 1;  // index of the output layer
 
-  if (warp == 8) {
+  if (warp == 4 * NWG) {
     // =========================== weight producer ===========================
     if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      for (long long u = blockIdx.x; u < num_tiles; u += gridDim.x) {
+        const long long tile = u / kSplit;
         const int member = (shuffle || expect) ? 0 : (int)(tile / tpm);
         for (int t = a.t0; t < a.t1; ++t)
         for (int pass = 0; pass < passes; ++pass) {
@@ -463,7 +478,7 @@ rollout_tc_kernel(const __grid_constant__ ModelDev m, const __grid_constant__ Ro
     const int wg = warp >> 2;
     const int wt = threadIdx.x & 127;
     const int r = wt & 63, h = wt >> 6;  // row of the warpgroup, half of the row's work
-    const int i = wg * 64 + r;           // tile row
+    const int i = wg * 64 + r;           // CTA row
     const bool owner = h == 0;           // the row's scalar state: observation / actions load, score, store
     const bool cem = CEMF && a.cem_mu != nullptr;
     const bool sampler = cem && h == 1;  // the thread of this row that draws its sequence's actions
@@ -507,18 +522,20 @@ rollout_tc_kernel(const __grid_constant__ ModelDev m, const __grid_constant__ Ro
     };
 
     pdl_wait();  // actions / observation / row state are the previous kernels' outputs; ours are written after this
-    for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    for (long long u = blockIdx.x; u < num_tiles; u += gridDim.x) {
+      const long long tile = u / kSplit;
+      const int ti = i + 64 * (int)(u % kSplit);  // row of the 128-row tile
       bool valid;
       long long rid, rid_glob;  // local row id (n * P + p: indexes actions / state / injected noise), global one (RNG key)
       if (shuffle) {
-        rid = shuffle_row(a, geom, tile, i, &valid, &rid_glob);
+        rid = shuffle_row(a, geom, tile, ti, &valid, &rid_glob);
         if (!valid) rid = 0;
       } else {
         const int member = (int)(tile / tpm);
         const int c = (int)(tile % tpm);
         const long long slot0 = (long long)member * Bm + (long long)c * kTileM;
-        valid = i < (int)min((long long)kTileM, Bm - (long long)c * kTileM);
-        rid = valid ? slot_to_rid(a, slot0 + i) : 0;
+        valid = ti < (int)min((long long)kTileM, Bm - (long long)c * kTileM);
+        rid = valid ? slot_to_rid(a, slot0 + ti) : 0;
         rid_glob = rid + (long long)a.seq0 * a.P;
       }
       float tot = 0.f;
@@ -777,21 +794,31 @@ __global__ void __launch_bounds__(128, 1) wgmma_selftest_kernel(int k, int n, in
 // ---------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------
-static int g_sm_count = 0, g_max_smem = 0, g_limits_dev = -1;
+static int g_sm_count = 0, g_max_smem = 0, g_pair_smem = 0, g_limits_dev = -1;
 
 static int tc_device_limits() {  // cached per device (a process may drive several)
-  int dev = 0;
+  int dev = 0, sm_smem = 0, reserved = 0;
   CUDA_TRY(cudaGetDevice(&dev));
   if (dev == g_limits_dev) return B200PETS_OK;
   CUDA_TRY(cudaDeviceGetAttribute(&g_sm_count, cudaDevAttrMultiProcessorCount, dev));
   CUDA_TRY(cudaDeviceGetAttribute(&g_max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  CUDA_TRY(cudaDeviceGetAttribute(&sm_smem, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev));
+  CUDA_TRY(cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev));
+  // dynamic shared memory of a 64-row CTA that fits twice per SM: half the SM's, less the per-CTA reservation and the
+  // static shared memory of the variant that has the most (the fused-CEM one)
+  cudaFuncAttributes fa;
+  CUDA_TRY(cudaFuncGetAttributes(&fa, rollout_tc_kernel<B200PETS_ACT_SILU, true, false, false, 1>));
+  g_pair_smem = min(g_max_smem, sm_smem / 2 - reserved - (int)fa.sharedSizeBytes);
   g_limits_dev = dev;
   return B200PETS_OK;
 }
 
-// smem plan for a model; returns false when the tensor-core path does not cover the dimensions
-bool tc_make_plan(const ModelDev& m, int max_smem, TcPlan* out, bool expectation = false, bool cem = false) {
+// smem plan for a model and CTA shape (nwg consumer warpgroups); returns false when the tensor-core path does not
+// cover the dimensions or the plan does not fit in max_smem
+static bool tc_make_plan(const ModelDev& m, int nwg, int max_smem, TcPlan* out, bool expectation, bool cem) {
   TcPlan p{};
+  p.nwg = nwg;
+  const uint32_t rows = 64u * (uint32_t)nwg;
   p.nlayers = m.L + 1;
   if (m.in + 2 > 256 || m.hid + 2 > 256 || m.nout > 256 || m.D > 256) return false;
   int kp_max = 0;
@@ -807,9 +834,9 @@ bool tc_make_plan(const ModelDev& m, int max_smem, TcPlan* out, bool expectation
   p.obs_ld = max(m.D, outq) | 1;  // a row holds the D observation words, the learned-reward word and the output padding
   p.act_ld = m.A | 1;
   uint32_t off = 0;
-  p.off_A = off; off += 2u * p.wg_bytes;
-  p.off_obs = off; off += (uint32_t)kTileM * p.obs_ld * 4;
-  p.off_act = off; off += (uint32_t)kTileM * p.act_ld * 4;
+  p.off_A = off; off += (uint32_t)nwg * p.wg_bytes;
+  p.off_obs = off; off += rows * p.obs_ld * 4;
+  p.off_act = off; off += rows * p.act_ld * 4;
   off = (off + 15u) & ~15u;
   p.off_const = off; off += (uint32_t)(2 * m.Kp[0]) * 4;
   off = (off + 15u) & ~15u;
@@ -817,7 +844,7 @@ bool tc_make_plan(const ModelDev& m, int max_smem, TcPlan* out, bool expectation
   off = (off + 15u) & ~15u;
   p.off_exp = off;
   p.exp_ld = (2 * outq) | 1;
-  if (expectation) off += (uint32_t)kTileM * p.exp_ld * 4;
+  if (expectation) off += rows * p.exp_ld * 4;
   off = (off + 15u) & ~15u;
   p.off_bar = off; off += 2 * kMaxStages * 8;
   off = (off + 127u) & ~127u;
@@ -840,30 +867,49 @@ bool tc_make_plan(const ModelDev& m, int max_smem, TcPlan* out, bool expectation
   return true;
 }
 
+// The plan of a launch of `tiles` 128-row tiles.  Fewer tiles than SMs: 64-row CTAs two per SM when that plan fits in
+// half an SM's shared memory, so that every SM gets work.  Otherwise 128-row CTAs one per SM with the whole opt-in shared
+// memory: once every SM has a tile, two 64-row CTAs per SM measured slower than one 128-row CTA (they fetch the
+// weights twice).  Every model with a 64-row plan also has a 128-row one.  Call after tc_device_limits().
+static bool tc_choose_plan(const ModelDev& m, long long tiles, TcPlan* out, bool expectation = false, bool cem = false) {
+  if (tiles < g_sm_count && tc_make_plan(m, 1, g_pair_smem, out, expectation, cem)) return true;
+  return tc_make_plan(m, 2, g_max_smem, out, expectation, cem);
+}
+
 bool tc_supported(const ModelDev& m) {
   if (tc_device_limits() != B200PETS_OK) return false;
   TcPlan p;
-  return tc_make_plan(m, g_max_smem, &p);
+  return tc_choose_plan(m, g_sm_count, &p);
 }
 
-// the plan launch_rollout_tc uses for an evaluation / step (no fused CEM iteration) with or without "expectation"
+// the plan launch_rollout_tc uses for an evaluation / step (no fused CEM iteration) with or without "expectation" that
+// has a 128-row tile for every SM (launches with fewer tiles may run 64-row CTAs, see tc_choose_plan)
 int tc_plan_info(const ModelDev& m, bool expectation, int* kslice, int* nstages, int* smem_bytes) {
   int rc = tc_device_limits();
   if (rc) return rc;
   TcPlan p;
-  const bool ok = tc_make_plan(m, g_max_smem, &p, expectation, false);
+  const bool ok = tc_choose_plan(m, g_sm_count, &p, expectation, false);
   *kslice = ok ? p.kslice : 0;
   *nstages = ok ? p.nstages : 0;
   *smem_bytes = ok ? (int)p.smem_bytes : 0;
   return B200PETS_OK;
 }
 
-// the variant with per-step trajectory stores (b200pets_eval_trajectory) for an activation
-template <bool EXP>
-static void (*traj_kernel(int act))(const ModelDev, const RolloutArgs, const TcPlan, const long long) {
-  return act == B200PETS_ACT_SILU   ? rollout_tc_kernel<B200PETS_ACT_SILU, false, EXP, true>
-         : act == B200PETS_ACT_RELU ? rollout_tc_kernel<B200PETS_ACT_RELU, false, EXP, true>
-                                    : rollout_tc_kernel<B200PETS_ACT_LEAKY_RELU, false, EXP, true>;
+using TcKernel = void (*)(const ModelDev, const RolloutArgs, const TcPlan, const long long);
+
+// the variant of a launch: fused CEM iteration, "expectation", per-step trajectory stores (b200pets_eval_trajectory)
+template <int ACT, int NWG>
+static TcKernel tc_variant(bool cemf, bool expect, bool traj) {
+  if (traj) return expect ? rollout_tc_kernel<ACT, false, true, true, NWG> : rollout_tc_kernel<ACT, false, false, true, NWG>;
+  if (expect) return rollout_tc_kernel<ACT, false, true, false, NWG>;
+  return cemf ? rollout_tc_kernel<ACT, true, false, false, NWG> : rollout_tc_kernel<ACT, false, false, false, NWG>;
+}
+
+template <int NWG>
+static TcKernel tc_kernel(int act, bool cemf, bool expect, bool traj) {
+  return act == B200PETS_ACT_SILU   ? tc_variant<B200PETS_ACT_SILU, NWG>(cemf, expect, traj)
+         : act == B200PETS_ACT_RELU ? tc_variant<B200PETS_ACT_RELU, NWG>(cemf, expect, traj)
+                                    : tc_variant<B200PETS_ACT_LEAKY_RELU, NWG>(cemf, expect, traj);
 }
 
 int launch_rollout_tc(const ModelDev& m, const RolloutArgs& a, cudaStream_t stream) {
@@ -871,12 +917,10 @@ int launch_rollout_tc(const ModelDev& m, const RolloutArgs& a, cudaStream_t stre
   if (rc) return rc;
   const bool expect = a.propagation == B200PETS_PROP_EXPECTATION;
   const bool cemf = a.cem_mu != nullptr || a.tail_counter != nullptr;
+  const bool traj = a.traj_obs || a.traj_reward || a.traj_done;
   if (expect && cemf) return b200pets_set_error(B200PETS_EUNSUPPORTED, "fused CEM iteration does not cover propagation='expectation'");
-  TcPlan p;
-  if (!tc_make_plan(m, g_max_smem, &p, expect, cemf))
-    return b200pets_set_error(B200PETS_EUNSUPPORTED, "model dimensions outside the tensor-core path (in %d hid %d out %d)",
-                              m.in, m.hid, m.out);
-  long long tiles;
+  if (traj && cemf) return b200pets_set_error(B200PETS_EUNSUPPORTED, "fused CEM iteration has no trajectory outputs");
+  long long tiles;  // 128-row tiles
   if (expect) {  // every row through every member: plain 128-row tiles, no member binding
     tiles = (a.B + kTileM - 1) / kTileM;
   } else if (a.slot_mode >= 1) {
@@ -885,32 +929,18 @@ int launch_rollout_tc(const ModelDev& m, const RolloutArgs& a, cudaStream_t stre
     long long Bm = a.B / m.M;
     tiles = (long long)m.M * ((Bm + kTileM - 1) / kTileM);
   }
-  const unsigned grid = (unsigned)min((long long)g_sm_count, tiles);
-  void (*kern)(const ModelDev, const RolloutArgs, const TcPlan, const long long) = nullptr;
-  if (expect) {
-    kern = m.act == B200PETS_ACT_SILU   ? rollout_tc_kernel<B200PETS_ACT_SILU, false, true>
-           : m.act == B200PETS_ACT_RELU ? rollout_tc_kernel<B200PETS_ACT_RELU, false, true>
-                                        : rollout_tc_kernel<B200PETS_ACT_LEAKY_RELU, false, true>;
-  } else {
-    switch (m.act) {
-      case B200PETS_ACT_SILU:
-        kern = cemf ? rollout_tc_kernel<B200PETS_ACT_SILU, true> : rollout_tc_kernel<B200PETS_ACT_SILU, false>;
-        break;
-      case B200PETS_ACT_RELU:
-        kern = cemf ? rollout_tc_kernel<B200PETS_ACT_RELU, true> : rollout_tc_kernel<B200PETS_ACT_RELU, false>;
-        break;
-      default:
-        kern = cemf ? rollout_tc_kernel<B200PETS_ACT_LEAKY_RELU, true> : rollout_tc_kernel<B200PETS_ACT_LEAKY_RELU, false>;
-        break;
-    }
-  }
-  if (a.traj_obs || a.traj_reward || a.traj_done) {
-    if (cemf) return b200pets_set_error(B200PETS_EUNSUPPORTED, "fused CEM iteration has no trajectory outputs");
-    kern = expect ? traj_kernel<true>(m.act) : traj_kernel<false>(m.act);
-  }
+  TcPlan p;
+  if (!tc_choose_plan(m, tiles, &p, expect, cemf))
+    return b200pets_set_error(B200PETS_EUNSUPPORTED, "model dimensions outside the tensor-core path (in %d hid %d out %d)",
+                              m.in, m.hid, m.out);
+  const TcKernel kern = p.nwg == 1 ? tc_kernel<1>(m.act, cemf, expect, traj) : tc_kernel<2>(m.act, cemf, expect, traj);
+  const int threads = p.nwg == 1 ? threads_of<1>() : threads_of<2>();
+  const long long cta_tiles = tiles * (2 / p.nwg);
   const size_t smem_launch = (size_t)p.smem_bytes + (cemf ? (size_t)2 * kCemTabDims * sizeof(float) : 0);
   CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_launch));
-  CUDA_TRY(launch_pdl(kern, dim3(grid), dim3(kThreads), smem_launch, stream, m, a, p, tiles));
+  // 64-row CTAs: fewer than two per SM, all resident (registers: tests/test_sass_occupancy.py; shared memory: the plan)
+  const unsigned grid = (unsigned)min((long long)g_sm_count * (2 / p.nwg), cta_tiles);
+  CUDA_TRY(launch_pdl(kern, dim3(grid), dim3(threads), smem_launch, stream, m, a, p, cta_tiles));
   return B200PETS_OK;
 }
 
