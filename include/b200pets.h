@@ -338,6 +338,35 @@ int b200pets_cem_plan(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, 
                       const float* z, const float* eps, const int64_t* perms, float* solution,
                       float* values_out, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Batches of independent problems (a vectorised environment, several episodes or seeds side by side): K evaluations or
+ * K CEM plans that share the model, the action bounds and the configuration, each with its own initial observation,
+ * warm start, sampling distribution, elites and solution, run in one launch per rollout / refit instead of K.  Problem k
+ * gives, bit for bit, the single call's result for its inputs made with the Philox offset the batch assigns to it:
+ *   b200pets_eval_sequences_batch: cfg->offset + k * 1024 (the offset of a single evaluation k ModelEnv calls later);
+ *   b200pets_cem_plan_batch:       rcfg->offset + k (a single plan turns it into (offset + k) * 1024 + iteration).
+ * Every array of a single call takes a leading [K] dimension (problem k's slice is the array its single call takes);
+ * lower / upper are shared:
+ *   obs0 [dev] float[K][D]; actions [dev] float[K][N][H][A]; perms [dev] int64[K][H or 1][B] or NULL;
+ *   eps [dev] float[K][H][B][out] or NULL; returns [dev] float[K][N]; row_returns [dev] float[K][B] or NULL;
+ *   plan: x0 [dev] float[K][H*A]; z [dev] float[K][it][N][H*A], eps [dev] float[K][it][H][B][out],
+ *   perms [dev] int64[K][it][H or 1][B] (each or NULL); solution [dev] float[K][H*A];
+ *   values_out [dev] float[K][it][N] or NULL.
+ * The plan runs the default structure of b200pets_cem_plan (rollout, then refit + next population: two launches per
+ * iteration for the whole batch).  Refused: num_problems < 1, a sharded cfg (first_sequence != 0 or global_population
+ * other than 0 / population), external reward / termination callables. */
+size_t b200pets_eval_batch_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* cfg, int32_t num_problems);
+int b200pets_eval_sequences_batch(b200pets_model_t model, const b200pets_rollout_cfg* cfg, int32_t num_problems,
+                                  const float* obs0, const float* actions, const int64_t* perms, const float* eps,
+                                  float* returns, float* row_returns, void* workspace, size_t workspace_bytes,
+                                  void* stream);
+size_t b200pets_cem_plan_batch_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* rcfg,
+                                               const b200pets_cem_cfg* ccfg, int32_t num_problems);
+int b200pets_cem_plan_batch(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg,
+                            int32_t num_problems, const float* obs0, const float* x0, const float* lower,
+                            const float* upper, const float* z, const float* eps, const int64_t* perms,
+                            float* solution, float* values_out, void* workspace, size_t workspace_bytes,
+                            void* stream);
+
 /* Self test of the wgmma building block: D[128][n] = A[128][k] * B[n][k]^T with bf16 operands staged in the
  * no-swizzle canonical layouts, the weight ring and the accumulator fragments the rollout kernel uses.  a, b [dev] float
  * (rounded to bf16 inside), d [dev] float[128][n].  k, n multiples of 16, <= 256.  A negative k writes A as bf16 pairs

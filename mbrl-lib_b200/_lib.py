@@ -89,6 +89,12 @@ _SIGNATURES = {
     "b200pets_cem_plan_workspace_bytes": (C.c_size_t, [_P, C.POINTER(RolloutCfg), C.POINTER(CemCfg)]),
     "b200pets_cem_plan": (C.c_int, [_P, C.POINTER(RolloutCfg), C.POINTER(CemCfg), _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
                                     C.c_size_t, _P]),
+    "b200pets_eval_batch_workspace_bytes": (C.c_size_t, [_P, C.POINTER(RolloutCfg), C.c_int32]),
+    "b200pets_eval_sequences_batch": (C.c_int, [_P, C.POINTER(RolloutCfg), C.c_int32, _P, _P, _P, _P, _P, _P, _P, C.c_size_t,
+                                                _P]),
+    "b200pets_cem_plan_batch_workspace_bytes": (C.c_size_t, [_P, C.POINTER(RolloutCfg), C.POINTER(CemCfg), C.c_int32]),
+    "b200pets_cem_plan_batch": (C.c_int, [_P, C.POINTER(RolloutCfg), C.POINTER(CemCfg), C.c_int32, _P, _P, _P, _P, _P, _P, _P,
+                                          _P, _P, _P, C.c_size_t, _P]),
     "b200pets_peer_buffer_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "b200pets_peer_alloc": (C.c_int, [C.c_size_t, C.POINTER(C.c_void_p), C.c_char_p]),
     "b200pets_peer_open": (C.c_int, [C.c_char_p, C.POINTER(C.c_void_p)]),

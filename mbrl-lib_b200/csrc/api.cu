@@ -14,8 +14,17 @@
 int launch_rollout_f32(const ModelDev& m, const RolloutArgs& a, cudaStream_t stream);
 int launch_rollout_tc(const ModelDev& m, const RolloutArgs& a, cudaStream_t stream);
 int launch_wgmma_selftest(int k, int n, const float* a, const float* b, float* d, cudaStream_t stream);
+int launch_rollout_f32_batch(const ModelDev& m, const RolloutArgs& a, int num_problems, BatchArgs bt, cudaStream_t stream);
+int launch_rollout_tc_batch(const ModelDev& m, const RolloutArgs& a, int num_problems, BatchArgs bt, cudaStream_t stream);
 int launch_particle_mean(int N, int P, const float* total, float* returns, cudaStream_t stream);
 bool cem_refit_sample_supported(int population, int dims, int elite_num);
+int launch_cem_refit_sample_batch(int num_problems, int population, int dims, int elite_num, float alpha, int use_std,
+                                  const float* row_totals, long long rows_stride, int particles, float* values, long long values_stride,
+                                  float* mu, float* dispersion, float* best_solution, long long dims_stride, float* best_value,
+                                  long long best_stride, void* workspace, long long ws_stride_bytes, size_t workspace_bytes, int refit,
+                                  int sample, const float* lb, const float* ub, const float* z_next, long long z_stride,
+                                  unsigned long long seed, unsigned long long offset, unsigned long long offset_step, int clipped,
+                                  unsigned int tag, float* pop, long long pop_stride, void* stream);
 int launch_cem_refit_sample(int population, int dims, int elite_num, float alpha, int use_std, const float* row_totals,
                             int particles, float* values, float* mu, float* dispersion, float* best_value, float* best_solution,
                             void* workspace, size_t workspace_bytes, int refit, int sample, const float* lb, const float* ub,
@@ -327,6 +336,17 @@ static int dispatch(const b200pets_model_s* mdl, int precision, const RolloutArg
   return b200pets_set_error(B200PETS_EINVAL, "unknown precision %d", precision);
 }
 
+// a batched launch (BatchArgs) of `num_problems` copies of `a_in`
+static int dispatch_batch(const b200pets_model_s* mdl, int precision, const RolloutArgs& a, int num_problems, const BatchArgs& bt,
+                          cudaStream_t stream) {
+  if (precision == B200PETS_PREC_BF16_TC) {
+    if (!mdl->tc_ok) return b200pets_set_error(B200PETS_EUNSUPPORTED, "tensor-core path does not cover this model; use B200PETS_PREC_F32");
+    return launch_rollout_tc_batch(mdl->dev, a, num_problems, bt, stream);
+  }
+  if (precision == B200PETS_PREC_F32) return launch_rollout_f32_batch(mdl->dev, a, num_problems, bt, stream);
+  return b200pets_set_error(B200PETS_EINVAL, "unknown precision %d", precision);
+}
+
 static size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 size_t b200pets_eval_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* cfg) {
@@ -350,11 +370,12 @@ static int check_eval(b200pets_model_t model, const b200pets_rollout_cfg* cfg, c
 // Rollout launches for steps [t0, t1) of the evaluation `cfg` describes.  Between launches a row's observation is carried
 // in obs_state [B][D] (stored when keep_obs, or when the window is split into per-step launches); its reward total and
 // dead flag in total / dead when those are given (NULL: the kernel's own accumulation is not kept).  traj_* (or NULL)
-// receive every step's next observation, reward and done at [t - t0][row].
+// receive every step's next observation, reward and done at [t - t0][row].  bt (or NULL): the launches are batched over
+// num_problems problems with these per-problem strides; every pointer is then problem 0's.
 static int rollout_steps(b200pets_model_t model, const b200pets_rollout_cfg* cfg, int t0, int t1, bool keep_obs,
                          const float* obs0, const float* actions, const int64_t* perms, const float* eps, float* obs_state,
                          float* total, uint8_t* dead, float* traj_obs, float* traj_reward, uint8_t* traj_done,
-                         cudaStream_t stream) {
+                         cudaStream_t stream, int num_problems = 1, const BatchArgs* bt = nullptr) {
   const b200pets_model_desc& d = model->desc;
   const int N = cfg->population, H = cfg->horizon, P = cfg->particles;
   const long long B = (long long)N * P;
@@ -384,7 +405,7 @@ static int rollout_steps(b200pets_model_t model, const b200pets_rollout_cfg* cfg
       s.traj_obs = traj_obs ? traj_obs + (size_t)(t - t0) * B * d.obs_dim : nullptr;
       s.traj_reward = traj_reward ? traj_reward + (size_t)(t - t0) * B : nullptr;
       s.traj_done = traj_done ? traj_done + (size_t)(t - t0) * B : nullptr;
-      int rc = dispatch(model, precision, s, stream);
+      int rc = bt ? dispatch_batch(model, precision, s, num_problems, *bt, stream) : dispatch(model, precision, s, stream);
       if (rc) return rc;
     }
   } else {
@@ -400,7 +421,7 @@ static int rollout_steps(b200pets_model_t model, const b200pets_rollout_cfg* cfg
     } else {             // in-kernel member draw: per (tile, step) for TS1, per tile for TSinf
       a.slot_mode = ts1 ? 1 : 2; a.perm = nullptr;
     }
-    int rc = dispatch(model, precision, a, stream);
+    int rc = bt ? dispatch_batch(model, precision, a, num_problems, *bt, stream) : dispatch(model, precision, a, stream);
     if (rc) return rc;
   }
   return B200PETS_OK;
@@ -692,6 +713,208 @@ int b200pets_cem_plan(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, 
     if (values_out) CUDA_TRY(cudaMemcpyAsync(values_out + (size_t)it * N, values, sizeof(float) * N, cudaMemcpyDeviceToDevice, stream));
   }
   CUDA_TRY(cudaMemcpyAsync(solution, ccfg->return_mean_elites ? mu : best_sol, sizeof(float) * dims, cudaMemcpyDeviceToDevice, stream));
+  return B200PETS_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// batches of independent problems: one launch per rollout / refit for all of them
+// ---------------------------------------------------------------------------------------------------------
+
+// checks shared by the batched entry points
+static int check_batch(b200pets_model_t model, const b200pets_rollout_cfg* cfg, int32_t num_problems, const char* what) {
+  if (num_problems < 1) return b200pets_set_error(B200PETS_EINVAL, "%s: num_problems must be at least 1 (got %d)", what, num_problems);
+  { int rc = check_eval(model, cfg, what); if (rc) return rc; }
+  if (cfg->first_sequence != 0 || (cfg->global_population != 0 && cfg->global_population != cfg->population))
+    return b200pets_set_error(B200PETS_EUNSUPPORTED, "%s: a batch of problems cannot be sharded over GPUs "
+                                                     "(first_sequence %d, global_population %d)", what, cfg->first_sequence,
+                              cfg->global_population);
+  const b200pets_model_desc& d = model->desc;
+  if (d.reward_fn == B200PETS_REWARD_EXTERNAL || d.term_fn == B200PETS_TERM_EXTERNAL)
+    return b200pets_set_error(B200PETS_EUNSUPPORTED, "%s: external reward/termination callables cannot run inside this call; "
+                                                     "evaluate the problems one at a time", what);
+  return B200PETS_OK;
+}
+
+// evaluation workspace of a batch: observations [K][B][D], reward totals [K][B], dead flags [K][B]
+size_t b200pets_eval_batch_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* cfg, int32_t num_problems) {
+  if (!model || !cfg || num_problems < 1) return 0;
+  const size_t KB = (size_t)num_problems * cfg->population * cfg->particles;
+  return al256(KB * model->desc.obs_dim * sizeof(float)) + al256(KB * sizeof(float)) + al256(KB);
+}
+
+// The rollouts of K evaluations in batched launches: problem k starts from obs0 + k * D, reads actions + k * act_stride,
+// perms + k * perm_stride, eps + k * eps_stride and draws with Philox offset cfg->offset + k * 1024.  Per-row totals
+// land in `total` [K][B].
+static int eval_rows_batch(b200pets_model_t model, const b200pets_rollout_cfg* cfg, int K, const float* obs0, const float* actions,
+                           long long act_stride, const int64_t* perms, long long perm_stride, const float* eps, long long eps_stride,
+                           float* total, void* workspace, cudaStream_t stream) {
+  const b200pets_model_desc& d = model->desc;
+  const size_t B = (size_t)cfg->population * cfg->particles, KB = (size_t)K * B;
+  unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
+  float* obs_state = reinterpret_cast<float*>(ws);
+  uint8_t* dead = ws + al256(KB * d.obs_dim * sizeof(float)) + al256(KB * sizeof(float));
+  BatchArgs bt{};
+  bt.obs0 = d.obs_dim;
+  bt.obs_state = (long long)B * d.obs_dim;
+  bt.act = act_stride;
+  bt.rows = (long long)B;
+  bt.perm = perm_stride;
+  bt.eps = eps_stride;
+  bt.seed = cfg->seed;
+  bt.offset_step = 1024;
+  return rollout_steps(model, cfg, 0, cfg->horizon, false, obs0, actions, perms, eps, obs_state, total, dead, nullptr, nullptr,
+                       nullptr, stream, K, &bt);
+}
+
+int b200pets_eval_sequences_batch(b200pets_model_t model, const b200pets_rollout_cfg* cfg, int32_t num_problems,
+                                  const float* obs0, const float* actions, const int64_t* perms, const float* eps,
+                                  float* returns, float* row_returns, void* workspace, size_t workspace_bytes, void* stream_) {
+  if (!model || !cfg) return b200pets_set_error(B200PETS_EINVAL, "eval_sequences_batch: null argument");
+  { int rc = check_batch(model, cfg, num_problems, "eval_sequences_batch"); if (rc) return rc; }
+  if (!obs0 || !actions || !returns || !workspace) return b200pets_set_error(B200PETS_EINVAL, "eval_sequences_batch: null argument");
+  if (workspace_bytes < b200pets_eval_batch_workspace_bytes(model, cfg, num_problems))
+    return b200pets_set_error(B200PETS_EINVAL, "eval_sequences_batch: workspace too small");
+  const b200pets_model_desc& d = model->desc;
+  const int N = cfg->population, H = cfg->horizon;
+  const size_t B = (size_t)N * cfg->particles, KB = (size_t)num_problems * B;
+  const int nperm = cfg->propagation == B200PETS_PROP_FIXED_MODEL ? 1 : H;
+  float* total = row_returns ? row_returns
+                             : reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(workspace) + al256(KB * d.obs_dim * sizeof(float)));
+  cudaStream_t stream = (cudaStream_t)stream_;
+  int rc = eval_rows_batch(model, cfg, num_problems, obs0, actions, (long long)N * H * d.act_dim, perms, (long long)nperm * B, eps,
+                           (long long)H * B * d.out_size, total, workspace, stream);
+  if (rc) return rc;
+  // problem k's totals are rows k * B .. k * B + B - 1: one particle mean over K * N sequences
+  return launch_particle_mean(num_problems * N, cfg->particles, total, returns, stream);  // model_env.py:190-191
+}
+
+namespace {
+__global__ void cem_init_batch_kernel(int K, int dims, const float* __restrict__ x0, const float* __restrict__ lb,
+                                      const float* __restrict__ ub, int clipped, float* mu, float* disp, float* best_value) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (long long)K * dims) return;
+  const int k = (int)(idx / dims), d = (int)(idx % dims);
+  if (d == 0) {  // per problem: best value, the refit flag of cem_refit_sample_batch_kernel
+    best_value[(size_t)k * 64] = -INFINITY;
+    *reinterpret_cast<unsigned int*>(best_value + (size_t)k * 64 + 2) = 0u;
+  }
+  mu[idx] = x0[idx];
+  const float w = ub[d] - lb[d];
+  disp[idx] = clipped ? 1.0f : (w * w) / 16.0f;  // trajectory_opt.py:100-108
+}
+
+// the workspace of a batched plan: per-problem arrays side by side, [K][...] each
+struct PlanBatchLayout {
+  size_t pop, values, mu, disp, best_sol, best_val, upd, eval, total;
+  size_t upd_bytes;  // one problem's refit workspace
+};
+PlanBatchLayout plan_batch_layout(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg, int K) {
+  const size_t N = rcfg->population, dims = (size_t)rcfg->horizon * model->desc.act_dim;
+  PlanBatchLayout l{};
+  l.upd_bytes = al256(b200pets_cem_update_workspace_bytes((int)N, (int)dims, ccfg->elite_num));
+  size_t off = 0;
+  l.pop = off; off += al256(K * N * dims * 4);
+  l.values = off; off += al256(K * N * 4);
+  l.mu = off; off += al256(K * dims * 4);
+  l.disp = off; off += al256(K * dims * 4);
+  l.best_sol = off; off += al256(K * dims * 4);
+  l.best_val = off; off += (size_t)K * 256;  // per problem: best value, refit flag
+  l.upd = off; off += (size_t)K * l.upd_bytes;
+  l.eval = off; off += al256(b200pets_eval_batch_workspace_bytes(model, rcfg, K));
+  l.total = off;
+  return l;
+}
+}  // namespace
+
+size_t b200pets_cem_plan_batch_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg,
+                                               int32_t num_problems) {
+  if (!model || !rcfg || !ccfg || num_problems < 1) return 0;
+  return plan_batch_layout(model, rcfg, ccfg, num_problems).total;
+}
+
+int b200pets_cem_plan_batch(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg,
+                            int32_t num_problems, const float* obs0, const float* x0, const float* lower, const float* upper,
+                            const float* z, const float* eps, const int64_t* perms, float* solution, float* values_out,
+                            void* workspace, size_t workspace_bytes, void* stream_) {
+  if (!model || !rcfg || !ccfg) return b200pets_set_error(B200PETS_EINVAL, "cem_plan_batch: null argument");
+  { int rc = check_batch(model, rcfg, num_problems, "cem_plan_batch"); if (rc) return rc; }
+  if (!obs0 || !x0 || !lower || !upper || !solution || !workspace)
+    return b200pets_set_error(B200PETS_EINVAL, "cem_plan_batch: null argument");
+  const int K = num_problems;
+  if (workspace_bytes < b200pets_cem_plan_batch_workspace_bytes(model, rcfg, ccfg, K))
+    return b200pets_set_error(B200PETS_EINVAL, "cem_plan_batch: workspace too small");
+  cudaStream_t stream = (cudaStream_t)stream_;
+  const b200pets_model_desc& d = model->desc;
+  const int N = rcfg->population, H = rcfg->horizon, P = rcfg->particles, A = d.act_dim, iters = ccfg->num_iterations;
+  const int dims = H * A;
+  const long long B = (long long)N * P;
+  const PlanBatchLayout l = plan_batch_layout(model, rcfg, ccfg, K);
+  unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
+  float* pop = reinterpret_cast<float*>(ws + l.pop);
+  float* values = reinterpret_cast<float*>(ws + l.values);
+  float* mu = reinterpret_cast<float*>(ws + l.mu);
+  float* disp = reinterpret_cast<float*>(ws + l.disp);
+  float* best_sol = reinterpret_cast<float*>(ws + l.best_sol);
+  float* best_val = reinterpret_cast<float*>(ws + l.best_val);
+  unsigned char* upd_ws = ws + l.upd;
+  void* eval_ws = ws + l.eval;
+  float* totals = reinterpret_cast<float*>(ws + l.eval + al256((size_t)K * B * d.obs_dim * sizeof(float)));
+  const long long popk = (long long)N * dims;  // per-problem strides
+  const int nperm = rcfg->propagation == B200PETS_PROP_FIXED_MODEL ? 1 : H;
+
+  const long long tot = (long long)K * dims;
+  cem_init_batch_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, stream>>>(K, dims, x0, lower, upper, ccfg->clipped_normal, mu, disp,
+                                                                          best_val);
+  CUDA_TRY(cudaGetLastError());
+  // The default plan of b200pets_cem_plan for every problem: rollout, then one kernel that refits and draws the next
+  // population (2 launches per iteration for the whole batch).  Outside the single-CTA refit, the sample and refit kernels
+  // run once per problem around the batched rollout.
+  const bool merged = cem_refit_sample_supported(N, dims, ccfg->elite_num);
+  auto next_pop = [&](int it_next, int refit) -> int {  // refit of it_next - 1 (if any) + population of it_next
+    const int sample = it_next < iters;
+    return launch_cem_refit_sample_batch(K, N, dims, ccfg->elite_num, ccfg->alpha, ccfg->clipped_normal, refit ? totals : nullptr, B, P,
+                                         values, N, mu, disp, best_sol, dims, best_val, 64, upd_ws, (long long)l.upd_bytes,
+                                         l.upd_bytes, refit, sample, lower, upper,
+                                         (z && sample) ? z + (size_t)it_next * N * dims : nullptr, (long long)iters * N * dims,
+                                         rcfg->seed, rcfg->offset * 1024 + (unsigned long long)it_next, 1024, ccfg->clipped_normal,
+                                         (unsigned int)it_next, pop, popk, stream);
+  };
+  if (merged) {
+    int rc0 = next_pop(0, 0);
+    if (rc0) return rc0;
+  }
+  for (int it = 0; it < iters; ++it) {
+    if (!merged)
+      for (int k = 0; k < K; ++k) {
+        int rcs = b200pets_cem_sample_shard(N, 0, dims, mu + (size_t)k * dims, disp + (size_t)k * dims, lower, upper,
+                                            z ? z + ((size_t)k * iters + it) * N * dims : nullptr, rcfg->seed,
+                                            (rcfg->offset + k) * 1024 + it, ccfg->clipped_normal, pop + (size_t)k * popk, stream);
+        if (rcs) return rcs;
+      }
+    b200pets_rollout_cfg rc_it = *rcfg;
+    rc_it.offset = rcfg->offset * 1024 + it;
+    int rc = eval_rows_batch(model, &rc_it, K, obs0, pop, popk, perms ? perms + (size_t)it * nperm * B : nullptr,
+                             (long long)iters * nperm * B, eps ? eps + (size_t)it * H * B * d.out_size : nullptr,
+                             (long long)iters * H * B * d.out_size, totals, eval_ws, stream);
+    if (rc) return rc;
+    if (merged) {
+      rc = next_pop(it + 1, 1);
+      if (rc) return rc;
+    } else {
+      for (int k = 0; k < K; ++k) {
+        rc = launch_cem_update_rows(N, dims, ccfg->elite_num, ccfg->alpha, 1, ccfg->clipped_normal, pop + (size_t)k * popk,
+                                    totals + (size_t)k * B, P, values + (size_t)k * N, mu + (size_t)k * dims,
+                                    disp + (size_t)k * dims, best_val + (size_t)k * 64, best_sol + (size_t)k * dims,
+                                    upd_ws + (size_t)k * l.upd_bytes, l.upd_bytes, stream);
+        if (rc) return rc;
+      }
+    }
+    if (values_out)  // problem k's values of iteration it -> values_out[k][it]
+      CUDA_TRY(cudaMemcpy2DAsync(values_out + (size_t)it * N, sizeof(float) * iters * N, values, sizeof(float) * N, sizeof(float) * N,
+                                 K, cudaMemcpyDeviceToDevice, stream));
+  }
+  CUDA_TRY(cudaMemcpyAsync(solution, ccfg->return_mean_elites ? mu : best_sol, sizeof(float) * K * dims, cudaMemcpyDeviceToDevice,
+                           stream));
   return B200PETS_OK;
 }
 

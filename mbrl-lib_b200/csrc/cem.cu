@@ -579,6 +579,60 @@ cem_refit_sample_kernel(const SelArgs s, const float* __restrict__ row_totals, i
   }
 }
 
+// cem_refit_sample_kernel for K independent problems in one launch.  Problem k works on base + k * stride of every
+// per-problem array and draws with Philox offset q.offset + k * offset_step; its work is the single kernel's, split the
+// same way.  CTA k < K is problem k's refit CTA (and its first sampling CTA); CTA K + j is sampling CTA 1 + j % (G - 1)
+// of problem j / (G - 1).  A CTA that waits for a refit therefore waits only for a CTA of lower index, which the
+// hardware dispatches no later than itself.
+struct RefitBatch {
+  int K, G;                                    // problems, CTAs per problem (the single kernel's grid)
+  long long pop, values, dims, best, ws, rows, z;  // element strides: population, values, mu / dispersion / best
+                                                   // solution, best value + refit flag, elite indices, row totals, z
+  unsigned long long seed, offset_step;        // seed before rng_key
+};
+
+__global__ void __launch_bounds__(kSelThreads, 1)
+cem_refit_sample_batch_kernel(const SelArgs s0, const float* __restrict__ row_totals, int P, const NextPop q0, const RefitBatch rb) {
+  pdl_trigger();
+  pdl_wait();
+  const int c = blockIdx.x;
+  const int k = c < rb.K ? c : (c - rb.K) / (rb.G - 1);
+  const int slice = c < rb.K ? 0 : 1 + (c - rb.K) % (rb.G - 1);
+  SelArgs s = s0;
+  s.pop += k * rb.pop; s.values += k * rb.values; s.mu += k * rb.dims; s.disp += k * rb.dims;
+  s.best_value += k * rb.best; s.best_solution += k * rb.dims; s.elite_idx += k * rb.ws;
+  unsigned int* flag = q0.flag + k * rb.best;
+  if (q0.refit) {
+    if (slice == 0) {
+      select_small_body(s, row_totals ? row_totals + k * rb.rows : nullptr, P);
+      __syncthreads();  // every read of the old population (elite rows, best row) is done
+      if (threadIdx.x == 0) {
+        __threadfence();
+        asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(flag), "r"(q0.tag) : "memory");
+      }
+    } else {
+      if (threadIdx.x == 0) {
+        unsigned int v;
+        do {
+          asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(flag) : "memory");
+        } while (v != q0.tag);
+      }
+      __syncthreads();
+    }
+  }
+  if (!q0.sample) return;
+  const unsigned long long offset = q0.offset + (unsigned long long)k * rb.offset_step;
+  const unsigned long long seed = rng_key(rb.seed, offset);
+  const float* z = q0.z ? q0.z + k * rb.z : nullptr;
+  float* pop_out = q0.pop_out + k * rb.pop;
+  const long long tot = (long long)q0.n_pop * s.dims;
+  for (long long idx = (long long)slice * blockDim.x + threadIdx.x; idx < tot; idx += (long long)rb.G * blockDim.x) {
+    const int d = (int)(idx % s.dims);
+    pop_out[idx] = cem_sample_element(idx, s.dims, __ldcg(s.mu + d), __ldcg(s.disp + d), q0.lb[d], q0.ub[d], z, seed, offset,
+                                      q0.clipped, q0.seq0);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------------
 // MPPI (mbrl/planning/trajectory_opt.py:191-311)
 // ------------------------------------------------------------------------------------------------------
@@ -1186,6 +1240,43 @@ int launch_cem_refit_sample(int population, int dims, int elite_num, float alpha
   const size_t esm = (size_t)k * dims * sizeof(float);
   CUDA_TRY(cudaFuncSetAttribute(cem_refit_sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 150 * 1024));
   CUDA_TRY(launch_pdl(cem_refit_sample_kernel, dim3(grid), dim3(kSelThreads), esm, (cudaStream_t)stream, s, row_totals, particles, q));
+  return B200PETS_OK;
+}
+
+// launch_cem_refit_sample for `num_problems` problems whose per-problem arrays lie `*_stride` elements apart (see
+// RefitBatch); seed is the unkeyed seed, problem k draws with offset + k * offset_step
+int launch_cem_refit_sample_batch(int num_problems, int population, int dims, int elite_num, float alpha, int use_std,
+                                  const float* row_totals, long long rows_stride, int particles, float* values, long long values_stride,
+                                  float* mu, float* dispersion, float* best_solution, long long dims_stride, float* best_value,
+                                  long long best_stride, void* workspace, long long ws_stride_bytes, size_t workspace_bytes, int refit,
+                                  int sample, const float* lb, const float* ub, const float* z_next, long long z_stride,
+                                  unsigned long long seed, unsigned long long offset, unsigned long long offset_step, int clipped,
+                                  unsigned int tag, float* pop, long long pop_stride, void* stream) {
+  const int n = population, k = elite_num;
+  if (!(n <= kSmallN && (size_t)k * dims * sizeof(float) <= 150 * 1024)) return B200PETS_EUNSUPPORTED;
+  if (refit && (k < 2 || k > n)) return b200pets_set_error(B200PETS_EINVAL, "cem_update: need 2 <= elite_num (%d) <= population (%d)", k, n);
+  if (workspace_bytes < b200pets_cem_update_workspace_bytes(n, dims, k)) return b200pets_set_error(B200PETS_EINVAL, "cem_update: workspace too small");
+  SelArgs s{};
+  s.n = n; s.dims = dims; s.k = k; s.alpha = alpha; s.unbiased = 1; s.use_std = use_std; s.mode = 0;
+  s.pop = pop; s.pstride = dims; s.values = values; s.vstride = 1; s.mu = mu; s.disp = dispersion;
+  s.best_value = best_value; s.best_solution = best_solution;
+  s.partial = reinterpret_cast<float*>(workspace);
+  s.elite_idx = reinterpret_cast<int*>(reinterpret_cast<float*>(workspace) + 33 * (size_t)dims);
+  NextPop q{};
+  q.refit = refit; q.sample = sample; q.n_pop = n; q.lb = lb; q.ub = ub; q.z = z_next; q.offset = offset;
+  q.clipped = clipped; q.seq0 = 0; q.flag = reinterpret_cast<unsigned int*>(best_value + 2); q.tag = tag; q.pop_out = pop;
+  const long long tot = (long long)n * dims;
+  unsigned G = sample ? (unsigned)min((long long)64, (tot + kSelThreads - 1) / kSelThreads) : 1u;
+  if (G < 1) G = 1;
+  RefitBatch rb{};
+  rb.K = num_problems; rb.G = (int)G;
+  rb.pop = pop_stride; rb.values = values_stride; rb.dims = dims_stride; rb.best = best_stride;
+  rb.ws = ws_stride_bytes / (long long)sizeof(int); rb.rows = rows_stride; rb.z = z_stride;
+  rb.seed = seed; rb.offset_step = offset_step;
+  const size_t esm = (size_t)k * dims * sizeof(float);
+  CUDA_TRY(cudaFuncSetAttribute(cem_refit_sample_batch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 150 * 1024));
+  CUDA_TRY(launch_pdl(cem_refit_sample_batch_kernel, dim3((unsigned)num_problems * G), dim3(kSelThreads), esm, (cudaStream_t)stream, s,
+                      row_totals, particles, q, rb));
   return B200PETS_OK;
 }
 

@@ -87,6 +87,20 @@ struct RolloutArgs {
   float tail_alpha;
 };
 
+// A batched launch: K independent evaluations of one configuration in one grid.  Tiles are problem-major (tile =
+// k * tiles + local tile); problem k reads and writes base + k * stride of every per-problem array of RolloutArgs and
+// draws with Philox offset `offset + k * offset_step` (keyed from the unkeyed `seed` as the C entry points do).  Every
+// other field of RolloutArgs is shared, and a problem's rows do exactly what they do in a single launch.
+struct BatchArgs {
+  long long tiles;                 // tiles of one problem: the count a single launch of the configuration has
+  long long obs0;                  // [D] initial observation
+  long long obs_state;             // obs_in / obs_out [B][D]
+  long long act;                   // action source
+  long long rows;                  // total_state / dead_state [B]
+  long long perm, eps;             // injected permutation / model noise
+  unsigned long long seed, offset_step;
+};
+
 // Launch plans, chosen on the host from the model's shape and the device's opt-in shared memory (the launchers and
 // b200pets_model_plan_info call the same functions).
 struct F32Plan {
@@ -321,8 +335,31 @@ __device__ __forceinline__ int shuffle_member(unsigned long long seed, unsigned 
 
 // Kernels put the low 32 bits of the stream offset into a Philox counter word; the high 32 bits go into the key so
 // that long runs (> 2^32 offsets) never replay a stream.  Applied once at every C entry point.
-static inline unsigned long long rng_key(unsigned long long seed, unsigned long long offset) {
+static __host__ __device__ inline unsigned long long rng_key(unsigned long long seed, unsigned long long offset) {
   return seed ^ (offset & 0xFFFFFFFF00000000ull);
+}
+
+// Problem k of a batched launch (BatchArgs): the element offset of its slice of a per-problem array, its Philox offset
+// and key.  With BATCH = false (single launches) these are 0, a.offset and a.seed, and `bt` is never read.
+template <bool BATCH>
+__device__ __forceinline__ long long prob_off(const BatchArgs* bt, long long k, long long BatchArgs::*stride) {
+  if constexpr (BATCH) return k * (bt->*stride);
+  else return 0;
+}
+template <bool BATCH>
+__device__ __forceinline__ unsigned long long prob_offset(const RolloutArgs& a, const BatchArgs* bt, long long k) {
+  if constexpr (BATCH) return a.offset + (unsigned long long)k * bt->offset_step;
+  else return a.offset;
+}
+template <bool BATCH>
+__device__ __forceinline__ unsigned long long prob_seed(const RolloutArgs& a, const BatchArgs* bt, long long k) {
+  if constexpr (BATCH) return rng_key(bt->seed, prob_offset<BATCH>(a, bt, k));
+  else return a.seed;
+}
+template <bool BATCH>
+__device__ __forceinline__ long long prob_rid(const RolloutArgs& a, const BatchArgs* bt, long long k, long long slot) {
+  if constexpr (BATCH) return a.perm ? a.perm[k * bt->perm + slot] : slot;
+  else return slot_to_rid(a, slot);
 }
 
 // ------------------------------------------------------------------------------------------------------

@@ -83,8 +83,10 @@ __device__ __forceinline__ void dense_layer(const float* __restrict__ W, const f
   }
 }
 
-template <int TR>
-__global__ void __launch_bounds__(kThreads) rollout_f32_kernel(const ModelDev m, const RolloutArgs a, int LD) {
+// The kernels' body.  BATCH: K independent problems in one launch (common.cuh BatchArgs): CTA j runs local tile
+// j % bt->tiles of problem j / bt->tiles, and everything after that decode is the single-problem code.
+template <int TR, bool BATCH>
+__device__ __forceinline__ void rollout_f32_body(const ModelDev& m, const RolloutArgs& a, int LD, const BatchArgs* bt) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   float* bufA = reinterpret_cast<float*>(smem_raw);
   float* bufB = bufA + TR * LD;
@@ -98,7 +100,9 @@ __global__ void __launch_bounds__(kThreads) rollout_f32_kernel(const ModelDev m,
   int* dead_s = reinterpret_cast<int*>(gid_s + TR);             // [TR]
 
   const int tid = threadIdx.x;
-  const int tile = blockIdx.x;
+  int tile = blockIdx.x;
+  long long kp = 0;  // problem of a batched launch
+  if constexpr (BATCH) { kp = tile / bt->tiles; tile -= (int)(kp * bt->tiles); }
   const bool expectation = a.propagation == B200PETS_PROP_EXPECTATION;
   // nv: rows of this tile that may hold a row (row i is live iff rid_s[i] >= 0)
   int nv, member = 0;
@@ -129,7 +133,7 @@ __global__ void __launch_bounds__(kThreads) rollout_f32_kernel(const ModelDev m,
       nv = (int)min((long long)TR, Bm - (long long)c * TR);
     }
     for (int i = tid; i < TR; i += kThreads) {
-      rid_s[i] = i < nv ? slot_to_rid(a, slot0 + i) : -1;
+      rid_s[i] = i < nv ? prob_rid<BATCH>(a, bt, kp, slot0 + i) : -1;
       gid_s[i] = rid_s[i] + (long long)a.seq0 * a.P;
     }
   }
@@ -139,24 +143,29 @@ __global__ void __launch_bounds__(kThreads) rollout_f32_kernel(const ModelDev m,
   for (int idx = tid; idx < TR * m.D; idx += kThreads) {
     int i = idx / m.D, d = idx % m.D;
     float v = 0.f;
-    if (rid_s[i] >= 0) v = a.init_from_obs0 ? a.obs0[d] : a.obs_in[rid_s[i] * m.D + d];
+    if (rid_s[i] >= 0)
+      v = a.init_from_obs0 ? a.obs0[prob_off<BATCH>(bt, kp, &BatchArgs::obs0) + d]
+                           : a.obs_in[prob_off<BATCH>(bt, kp, &BatchArgs::obs_state) + rid_s[i] * m.D + d];
     obs_s[idx] = v;
   }
   for (int i = tid; i < TR; i += kThreads) {
     bool ld = a.load_state && rid_s[i] >= 0;
-    tot_s[i] = ld ? a.total_state[rid_s[i]] : 0.f;
-    dead_s[i] = ld ? (int)a.dead_state[rid_s[i]] : 0;
+    tot_s[i] = ld ? a.total_state[prob_off<BATCH>(bt, kp, &BatchArgs::rows) + rid_s[i]] : 0.f;
+    dead_s[i] = ld ? (int)a.dead_state[prob_off<BATCH>(bt, kp, &BatchArgs::rows) + rid_s[i]] : 0;
   }
   __syncthreads();
 
   const int nlayers = m.L + 1;
   for (int t = a.t0; t < a.t1; ++t) {
-    if (shuffle) member = shuffle_member(a.seed, a.offset, a.slot_mode, shuffle_global_group(geom, group), t, m.M);
+    if (shuffle)
+      member = shuffle_member(prob_seed<BATCH>(a, bt, kp), prob_offset<BATCH>(a, bt, kp), a.slot_mode, shuffle_global_group(geom, group),
+                              t, m.M);
     // ---- actions ------------------------------------------------------------------------------
     for (int idx = tid; idx < TR * m.A; idx += kThreads) {
       int i = idx / m.A, j = idx % m.A;
       float v = 0.f;
-      if (rid_s[i] >= 0) v = a.act[(rid_s[i] / a.act_div) * a.act_row_stride + (long long)t * a.act_t_stride + j];
+      if (rid_s[i] >= 0)
+        v = a.act[prob_off<BATCH>(bt, kp, &BatchArgs::act) + (rid_s[i] / a.act_div) * a.act_row_stride + (long long)t * a.act_t_stride + j];
       act_s[idx] = v;
     }
     __syncthreads();
@@ -214,11 +223,11 @@ __global__ void __launch_bounds__(kThreads) rollout_f32_kernel(const ModelDev m,
             float sd = sqrtf(expf(lv));
             float e;
             if (a.eps) {
-              e = a.eps[((size_t)(t - a.t0) * a.B + rid_s[i]) * m.out + o];
+              e = a.eps[prob_off<BATCH>(bt, kp, &BatchArgs::eps) + ((size_t)(t - a.t0) * a.B + rid_s[i]) * m.out + o];
             } else {
               float z[4];
-              philox_normal4((uint32_t)gid_s[i], (uint32_t)t, RNG_STREAM_EPS | (uint32_t)(o >> 2), (uint32_t)a.offset,
-                             a.seed, z);
+              philox_normal4((uint32_t)gid_s[i], (uint32_t)t, RNG_STREAM_EPS | (uint32_t)(o >> 2), (uint32_t)prob_offset<BATCH>(a, bt, kp),
+                             prob_seed<BATCH>(a, bt, kp), z);
               e = z[o & 3];
             }
             pred = mean + sd * e;
@@ -245,11 +254,11 @@ __global__ void __launch_bounds__(kThreads) rollout_f32_kernel(const ModelDev m,
           float sd = sqrtf(expf(lv));
           float e;
           if (a.eps) {
-            e = a.eps[((size_t)(t - a.t0) * a.B + rid_s[i]) * m.out + o];
+            e = a.eps[prob_off<BATCH>(bt, kp, &BatchArgs::eps) + ((size_t)(t - a.t0) * a.B + rid_s[i]) * m.out + o];
           } else {
             float z[4];
-            philox_normal4((uint32_t)gid_s[i], (uint32_t)t, RNG_STREAM_EPS | (uint32_t)(o >> 2), (uint32_t)a.offset,
-                           a.seed, z);
+            philox_normal4((uint32_t)gid_s[i], (uint32_t)t, RNG_STREAM_EPS | (uint32_t)(o >> 2), (uint32_t)prob_offset<BATCH>(a, bt, kp),
+                           prob_seed<BATCH>(a, bt, kp), z);
             e = z[o & 3];
           }
           pred = mean + sd * e;
@@ -293,14 +302,27 @@ __global__ void __launch_bounds__(kThreads) rollout_f32_kernel(const ModelDev m,
     if (a.obs_out)
       for (int idx = tid; idx < nv * m.D; idx += kThreads) {
         int i = idx / m.D, d = idx % m.D;
-        if (rid_s[i] >= 0) a.obs_out[rid_s[i] * m.D + d] = obs_s[idx];
+        if (rid_s[i] >= 0) a.obs_out[prob_off<BATCH>(bt, kp, &BatchArgs::obs_state) + rid_s[i] * m.D + d] = obs_s[idx];
       }
     for (int i = tid; i < nv; i += kThreads) {
       if (rid_s[i] < 0) continue;
-      if (a.total_state) a.total_state[rid_s[i]] = tot_s[i];
-      if (a.dead_state) a.dead_state[rid_s[i]] = (uint8_t)dead_s[i];
+      if (a.total_state) a.total_state[prob_off<BATCH>(bt, kp, &BatchArgs::rows) + rid_s[i]] = tot_s[i];
+      if (a.dead_state) a.dead_state[prob_off<BATCH>(bt, kp, &BatchArgs::rows) + rid_s[i]] = (uint8_t)dead_s[i];
     }
   }
+}
+
+template <int TR>
+__global__ void __launch_bounds__(kThreads) rollout_f32_kernel(const ModelDev m, const RolloutArgs a, int LD) {
+  rollout_f32_body<TR, false>(m, a, LD, nullptr);
+}
+
+// K independent evaluations in one launch
+template <int TR>
+__global__ void __launch_bounds__(kThreads) rollout_f32_batch_kernel(const __grid_constant__ ModelDev m,
+                                                                     const __grid_constant__ RolloutArgs a, int LD,
+                                                                     const __grid_constant__ BatchArgs bt) {
+  rollout_f32_body<TR, true>(m, a, LD, &bt);
 }
 
 }  // namespace
@@ -354,6 +376,23 @@ int launch_rollout_f32(const ModelDev& m, const RolloutArgs& a, cudaStream_t str
   } else {
     return b200pets_set_error(B200PETS_EUNSUPPORTED, "layer width %d needs more shared memory than a CTA has", p.wmax);
   }
+  CUDA_TRY(cudaGetLastError());
+  return B200PETS_OK;
+}
+
+// `num_problems` evaluations of the launch `a` describes in one grid (bt: per-problem strides, bt.tiles is set here)
+int launch_rollout_f32_batch(const ModelDev& m, const RolloutArgs& a, int num_problems, BatchArgs bt, cudaStream_t stream) {
+  if (a.traj_obs || a.traj_reward || a.traj_done || a.reward_out || a.done_out)
+    return b200pets_set_error(B200PETS_EUNSUPPORTED, "batched rollout: evaluation outputs only");
+  F32Plan p;
+  int rc = f32_tile_plan(m, &p);
+  if (rc) return rc;
+  if (p.rows == 0) return b200pets_set_error(B200PETS_EUNSUPPORTED, "layer width %d needs more shared memory than a CTA has", p.wmax);
+  bt.tiles = f32_num_tiles(m, a, p.rows);
+  const unsigned grid = (unsigned)(bt.tiles * num_problems);
+  auto kern = p.rows == 64 ? rollout_f32_batch_kernel<64> : p.rows == 32 ? rollout_f32_batch_kernel<32> : rollout_f32_batch_kernel<16>;
+  CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
+  kern<<<grid, kThreads, p.smem, stream>>>(m, a, p.LD, bt);
   CUDA_TRY(cudaGetLastError());
   return B200PETS_OK;
 }

@@ -365,16 +365,18 @@ static __device__ __noinline__ void cem_tail_refit(const TailArgs* ap, int dims,
   }
 }
 
-template <int ACT, bool CEMF, bool EXP = false, bool TRAJ = false, int NWG = 2>
+// The rollout kernels' body, inlined into each kernel (ptxas serialises wgmma chains in a called function, C7510).
 // EXP: propagation "expectation" (member passes)
 // CEMF: fused-CEM features compiled in (in-kernel sampling, last-CTA refit)
 // TRAJ: per-step trajectory stores compiled in (b200pets_eval_trajectory); the other variants are compiled without them
 //       so that their schedule stays what it was
 // NWG: consumer warpgroups (TcPlan::nwg).  CTA tile u is half u % 2 of 128-row tile u / 2 when NWG = 1, tile u itself
 //      when NWG = 2; either way a row keeps its member, keys, operands and K order.
-__global__ void __launch_bounds__(threads_of<NWG>(), NWG == 1 ? 2 : 1)
-rollout_tc_kernel(const __grid_constant__ ModelDev m, const __grid_constant__ RolloutArgs a, const __grid_constant__ TcPlan p,
-                  const long long num_tiles) {
+// BATCH: K independent problems in one launch (common.cuh BatchArgs): 128-row tile j is local tile j % bt->tiles of
+//      problem j / bt->tiles, and everything after that decode is the single-problem code.
+template <int ACT, bool CEMF, bool EXP, bool TRAJ, int NWG, bool BATCH>
+__device__ __forceinline__ void rollout_tc_body(const ModelDev& m, const RolloutArgs& a, const TcPlan& p, const long long num_tiles,
+                                                const BatchArgs* bt) {
   extern __shared__ __align__(128) uint8_t smem[];
   uint8_t* ring = smem + p.off_ring;
   float* obs_s = reinterpret_cast<float*>(smem + p.off_obs);
@@ -450,11 +452,14 @@ rollout_tc_kernel(const __grid_constant__ ModelDev m, const __grid_constant__ Ro
       int stage = 0;
       uint32_t phase = 0;
       for (long long u = blockIdx.x; u < num_tiles; u += gridDim.x) {
-        const long long tile = u / kSplit;
+        long long tile = u / kSplit;
+        long long kp = 0;  // problem of a batched launch
+        if constexpr (BATCH) { kp = tile / bt->tiles; tile -= kp * bt->tiles; }
         const int member = (shuffle || expect) ? 0 : (int)(tile / tpm);
         for (int t = a.t0; t < a.t1; ++t)
         for (int pass = 0; pass < passes; ++pass) {
-          const int mem = expect ? pass : (shuffle ? shuffle_member(a.seed, a.offset, a.slot_mode, shuffle_global_group(geom, tile), t, m.M) : member);
+          const int mem = expect ? pass : (shuffle ? shuffle_member(prob_seed<BATCH>(a, bt, kp), prob_offset<BATCH>(a, bt, kp), a.slot_mode,
+                                                                    shuffle_global_group(geom, tile), t, m.M) : member);
           const uint8_t* base = m.img + (size_t)(blockIdx.x % m.img_replicas) * m.img_replica_stride + (size_t)mem * m.img_member_stride;
           for (int l = 0; l < nlayers; ++l) {
             // K steps are contiguous in the image (16 rows x Np columns each): a slice is one bulk copy
@@ -523,7 +528,9 @@ rollout_tc_kernel(const __grid_constant__ ModelDev m, const __grid_constant__ Ro
 
     pdl_wait();  // actions / observation / row state are the previous kernels' outputs; ours are written after this
     for (long long u = blockIdx.x; u < num_tiles; u += gridDim.x) {
-      const long long tile = u / kSplit;
+      long long tile = u / kSplit;
+      long long kp = 0;  // problem of a batched launch
+      if constexpr (BATCH) { kp = tile / bt->tiles; tile -= kp * bt->tiles; }
       const int ti = i + 64 * (int)(u % kSplit);  // row of the 128-row tile
       bool valid;
       long long rid, rid_glob;  // local row id (n * P + p: indexes actions / state / injected noise), global one (RNG key)
@@ -535,12 +542,12 @@ rollout_tc_kernel(const __grid_constant__ ModelDev m, const __grid_constant__ Ro
         const int c = (int)(tile % tpm);
         const long long slot0 = (long long)member * Bm + (long long)c * kTileM;
         valid = ti < (int)min((long long)kTileM, Bm - (long long)c * kTileM);
-        rid = valid ? slot_to_rid(a, slot0 + ti) : 0;
+        rid = valid ? prob_rid<BATCH>(a, bt, kp, slot0 + ti) : 0;
         rid_glob = rid + (long long)a.seq0 * a.P;
       }
       float tot = 0.f;
       int dead = 0;
-      const float* act_row = cem ? nullptr : a.act + (rid / a.act_div) * a.act_row_stride;
+      const float* act_row = cem ? nullptr : a.act + prob_off<BATCH>(bt, kp, &BatchArgs::act) + (rid / a.act_div) * a.act_row_stride;
       const int seq_n = (int)(rid / a.P);
       float* pop_row = (cem && a.pop_out && valid && rid % a.P == 0) ? a.pop_out + (size_t)seq_n * cem_dims : nullptr;  // in-kernel draw only
       // this step's actions into the row's action words: from the action tensor, or drawn in-kernel (fused CEM)
@@ -557,13 +564,15 @@ rollout_tc_kernel(const __grid_constant__ ModelDev m, const __grid_constant__ Ro
       wg_bar(wg);  // previous tile fully consumed before its row state is overwritten
       if (owner) {
         if (a.load_state && valid) {
-          tot = a.total_state[rid];
-          dead = a.dead_state[rid];
+          tot = a.total_state[prob_off<BATCH>(bt, kp, &BatchArgs::rows) + rid];
+          dead = a.dead_state[prob_off<BATCH>(bt, kp, &BatchArgs::rows) + rid];
         }
 #pragma unroll 1
         for (int d = 0; d < m.D; ++d) {
           float v = 0.f;
-          if (valid) v = a.init_from_obs0 ? a.obs0[d] : a.obs_in[rid * m.D + d];
+          if (valid)
+            v = a.init_from_obs0 ? a.obs0[prob_off<BATCH>(bt, kp, &BatchArgs::obs0) + d]
+                                 : a.obs_in[prob_off<BATCH>(bt, kp, &BatchArgs::obs_state) + rid * m.D + d];
           my_obs[d] = v;
         }
       }
@@ -627,10 +636,11 @@ rollout_tc_kernel(const __grid_constant__ ModelDev m, const __grid_constant__ Ro
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
                   const int oc = min(4 * gq + e, m.out - 1);
-                  z[e] = valid ? a.eps[((size_t)(t - a.t0) * a.B + rid) * m.out + oc] : 0.f;
+                  z[e] = valid ? a.eps[prob_off<BATCH>(bt, kp, &BatchArgs::eps) + ((size_t)(t - a.t0) * a.B + rid) * m.out + oc] : 0.f;
                 }
               } else {
-                philox_normal4((uint32_t)rid_glob, (uint32_t)t, RNG_STREAM_EPS | (uint32_t)gq, (uint32_t)a.offset, a.seed, z);
+                philox_normal4((uint32_t)rid_glob, (uint32_t)t, RNG_STREAM_EPS | (uint32_t)gq, (uint32_t)prob_offset<BATCH>(a, bt, kp),
+                               prob_seed<BATCH>(a, bt, kp), z);
               }
             }
             const float4* cg = c_out + 4 * gq;
@@ -684,10 +694,10 @@ rollout_tc_kernel(const __grid_constant__ ModelDev m, const __grid_constant__ Ro
       if (owner && a.store_state && valid) {
         if (a.obs_out) {
 #pragma unroll 1
-          for (int d = 0; d < m.D; ++d) a.obs_out[rid * m.D + d] = my_obs[d];
+          for (int d = 0; d < m.D; ++d) a.obs_out[prob_off<BATCH>(bt, kp, &BatchArgs::obs_state) + rid * m.D + d] = my_obs[d];
         }
-        if (a.total_state) a.total_state[rid] = tot;
-        if (a.dead_state) a.dead_state[rid] = (uint8_t)dead;
+        if (a.total_state) a.total_state[prob_off<BATCH>(bt, kp, &BatchArgs::rows) + rid] = tot;
+        if (a.dead_state) a.dead_state[prob_off<BATCH>(bt, kp, &BatchArgs::rows) + rid] = (uint8_t)dead;
       }
     }
   }
@@ -714,6 +724,21 @@ rollout_tc_kernel(const __grid_constant__ ModelDev m, const __grid_constant__ Ro
       cem_tail_refit(ta, cem_dims, ring + 256, &sh_tail[1]);
     }
   }
+}
+
+template <int ACT, bool CEMF, bool EXP = false, bool TRAJ = false, int NWG = 2>
+__global__ void __launch_bounds__(threads_of<NWG>(), NWG == 1 ? 2 : 1)
+rollout_tc_kernel(const __grid_constant__ ModelDev m, const __grid_constant__ RolloutArgs a, const __grid_constant__ TcPlan p,
+                  const long long num_tiles) {
+  rollout_tc_body<ACT, CEMF, EXP, TRAJ, NWG, false>(m, a, p, num_tiles, nullptr);
+}
+
+// K independent evaluations in one launch (plain and "expectation"; no fused-CEM or trajectory variants)
+template <int ACT, bool EXP, int NWG>
+__global__ void __launch_bounds__(threads_of<NWG>(), NWG == 1 ? 2 : 1)
+rollout_tc_batch_kernel(const __grid_constant__ ModelDev m, const __grid_constant__ RolloutArgs a, const __grid_constant__ TcPlan p,
+                        const long long num_tiles, const __grid_constant__ BatchArgs bt) {
+  rollout_tc_body<ACT, false, EXP, false, NWG, true>(m, a, p, num_tiles, &bt);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -896,6 +921,7 @@ int tc_plan_info(const ModelDev& m, bool expectation, int* kslice, int* nstages,
 }
 
 using TcKernel = void (*)(const ModelDev, const RolloutArgs, const TcPlan, const long long);
+using TcBatchKernel = void (*)(const ModelDev, const RolloutArgs, const TcPlan, const long long, const BatchArgs);
 
 // the variant of a launch: fused CEM iteration, "expectation", per-step trajectory stores (b200pets_eval_trajectory)
 template <int ACT, int NWG>
@@ -912,6 +938,45 @@ static TcKernel tc_kernel(int act, bool cemf, bool expect, bool traj) {
                                     : tc_variant<B200PETS_ACT_LEAKY_RELU, NWG>(cemf, expect, traj);
 }
 
+// 128-row tiles of one launch
+static long long tc_launch_tiles(const ModelDev& m, const RolloutArgs& a) {
+  if (a.propagation == B200PETS_PROP_EXPECTATION)  // every row through every member: plain 128-row tiles, no member binding
+    return (a.B + kTileM - 1) / kTileM;
+  if (a.slot_mode >= 1) return (long long)a.P * shuffle_geom(a.seq0, a.N, a.n_glob).C_loc;
+  long long Bm = a.B / m.M;
+  return (long long)m.M * ((Bm + kTileM - 1) / kTileM);
+}
+
+template <int NWG>
+static TcBatchKernel tc_batch_kernel(int act, bool expect) {
+  if (act == B200PETS_ACT_SILU) return expect ? rollout_tc_batch_kernel<B200PETS_ACT_SILU, true, NWG> : rollout_tc_batch_kernel<B200PETS_ACT_SILU, false, NWG>;
+  if (act == B200PETS_ACT_RELU) return expect ? rollout_tc_batch_kernel<B200PETS_ACT_RELU, true, NWG> : rollout_tc_batch_kernel<B200PETS_ACT_RELU, false, NWG>;
+  return expect ? rollout_tc_batch_kernel<B200PETS_ACT_LEAKY_RELU, true, NWG> : rollout_tc_batch_kernel<B200PETS_ACT_LEAKY_RELU, false, NWG>;
+}
+
+// `num_problems` evaluations of the launch `a` describes in one grid (bt: per-problem strides, bt.tiles is set here).
+// The CTA shape follows the total tile count, as for a single launch of that many tiles.
+int launch_rollout_tc_batch(const ModelDev& m, const RolloutArgs& a, int num_problems, BatchArgs bt, cudaStream_t stream) {
+  int rc = tc_device_limits();
+  if (rc) return rc;
+  if (a.cem_mu || a.tail_counter || a.traj_obs || a.traj_reward || a.traj_done || a.reward_out || a.done_out)
+    return b200pets_set_error(B200PETS_EUNSUPPORTED, "batched rollout: evaluation outputs only");
+  const bool expect = a.propagation == B200PETS_PROP_EXPECTATION;
+  bt.tiles = tc_launch_tiles(m, a);
+  const long long tiles = bt.tiles * num_problems;
+  TcPlan p;
+  if (!tc_choose_plan(m, tiles, &p, expect, false))
+    return b200pets_set_error(B200PETS_EUNSUPPORTED, "model dimensions outside the tensor-core path (in %d hid %d out %d)",
+                              m.in, m.hid, m.out);
+  const TcBatchKernel kern = p.nwg == 1 ? tc_batch_kernel<1>(m.act, expect) : tc_batch_kernel<2>(m.act, expect);
+  const int threads = p.nwg == 1 ? threads_of<1>() : threads_of<2>();
+  const long long cta_tiles = tiles * (2 / p.nwg);
+  CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem_bytes));
+  const unsigned grid = (unsigned)min((long long)g_sm_count * (2 / p.nwg), cta_tiles);
+  CUDA_TRY(launch_pdl(kern, dim3(grid), dim3(threads), (size_t)p.smem_bytes, stream, m, a, p, cta_tiles, bt));
+  return B200PETS_OK;
+}
+
 int launch_rollout_tc(const ModelDev& m, const RolloutArgs& a, cudaStream_t stream) {
   int rc = tc_device_limits();
   if (rc) return rc;
@@ -920,15 +985,7 @@ int launch_rollout_tc(const ModelDev& m, const RolloutArgs& a, cudaStream_t stre
   const bool traj = a.traj_obs || a.traj_reward || a.traj_done;
   if (expect && cemf) return b200pets_set_error(B200PETS_EUNSUPPORTED, "fused CEM iteration does not cover propagation='expectation'");
   if (traj && cemf) return b200pets_set_error(B200PETS_EUNSUPPORTED, "fused CEM iteration has no trajectory outputs");
-  long long tiles;  // 128-row tiles
-  if (expect) {  // every row through every member: plain 128-row tiles, no member binding
-    tiles = (a.B + kTileM - 1) / kTileM;
-  } else if (a.slot_mode >= 1) {
-    tiles = (long long)a.P * shuffle_geom(a.seq0, a.N, a.n_glob).C_loc;
-  } else {
-    long long Bm = a.B / m.M;
-    tiles = (long long)m.M * ((Bm + kTileM - 1) / kTileM);
-  }
+  const long long tiles = tc_launch_tiles(m, a);  // 128-row tiles
   TcPlan p;
   if (!tc_choose_plan(m, tiles, &p, expect, cemf))
     return b200pets_set_error(B200PETS_EUNSUPPORTED, "model dimensions outside the tensor-core path (in %d hid %d out %d)",

@@ -307,6 +307,64 @@ class ModelEnv:
                     "eval_sequences")
             return returns
 
+    def _eval_perms(self, prop: str, population: int, horizon: int, num_particles: int) -> Optional[torch.Tensor]:
+        """The permutations :meth:`evaluate_action_sequences` draws for one evaluation (None: members drawn in kernel)."""
+        B = population * num_particles
+        if prop == "fixed_model":
+            if B % len(self.staged.members()) != 0:
+                raise ValueError("To use GaussianMLP's ensemble propagation, the batch size must "
+                                 "be a multiple of the number of models in the ensemble.")
+            if self.ts1 == "perms" or self._few_groups(population, num_particles):
+                return torch.randperm(B, device=self.device).view(1, B)
+        elif prop == "random_model" and (self.ts1 == "perms" or self._few_groups(population, num_particles)):
+            return torch.stack([torch.randperm(B, device=self.device) for _ in range(horizon)])
+        return None
+
+    def evaluate_action_sequences_batch(self, action_sequences: torch.Tensor, initial_states: np.ndarray, num_particles: int, *,
+                                        _perms: Optional[torch.Tensor] = None, _eps: Optional[torch.Tensor] = None,
+                                        _row_returns: Optional[torch.Tensor] = None,
+                                        _offset: Optional[int] = None) -> torch.Tensor:
+        """:meth:`evaluate_action_sequences` for K independent problems in one call: ``action_sequences [K, N, H, A]``
+        from ``initial_states [K, D]``, returns ``[K, N]``.  Each problem gets exactly what a single call would give it:
+        the same permutation decision, drawn in the same order, and the Philox offset of the k-th of K consecutive
+        single calls (the call reserves K counter values).  The rollouts of all problems run in one launch per step
+        window, which fills the GPU where one problem's population does not.  Reward or termination callables the
+        kernels do not know are not supported here (``NotImplementedError``): call :meth:`evaluate_action_sequences`
+        per problem."""
+        with torch.no_grad():
+            assert len(action_sequences.shape) == 4  # problems, population, horizon, action_dim
+            K, population_size, horizon, action_dim = action_sequences.shape
+            initial_states = np.asarray(initial_states)
+            if initial_states.ndim != 2 or initial_states.shape[0] != K:
+                raise ValueError(f"initial_states must be [K={K}, obs_dim], got {tuple(initial_states.shape)}")
+            if self.has_external_callables():
+                raise NotImplementedError("evaluate_action_sequences_batch runs known reward / termination functions only; "
+                                          "with a callable, call evaluate_action_sequences once per problem")
+            self._fresh()
+            actions = action_sequences.to(self.device, torch.float32).contiguous()
+            prop = self._propagation()
+            perms = _perms
+            if perms is None:
+                per = [self._eval_perms(prop, population_size, horizon, num_particles) for _ in range(K)]
+                perms = None if not per or per[0] is None else torch.stack(per)
+            if perms is not None:
+                perms = perms.to(torch.int64).contiguous()
+            if _offset is None:
+                _offset = self._call_offset()
+                self._offset += K - 1  # problem k uses the offset of the k-th of K consecutive calls
+            cfg = _lib.RolloutCfg(population_size, horizon, num_particles, _lib.PREC[self.precision_for(prop)], _lib.PROP[prop],
+                                  _lib.TS1_PERMS if perms is not None else _lib.TS1_TILE_SHUFFLE, self._seed, _offset, 0, 0)
+            obs0 = torch.from_numpy(np.ascontiguousarray(initial_states, dtype=np.float32)).to(self.device)
+            returns = torch.empty(K, population_size, dtype=torch.float32, device=self.device)
+            need = self.lib.b200pets_eval_batch_workspace_bytes(self.staged.handle, C.byref(cfg), K)
+            ws = self._workspace(need)
+            with torch.cuda.device(self.device):
+                _lib.check(self.lib.b200pets_eval_sequences_batch(
+                    self.staged.handle, C.byref(cfg), K, _lib.ptr(obs0), _lib.ptr(actions), _lib.ptr(perms), _lib.ptr(_eps),
+                    _lib.ptr(returns), _lib.ptr(_row_returns), _lib.ptr(ws), ws.numel(), _lib.stream_ptr()),
+                    "eval_sequences_batch")
+            return returns
+
     def _evaluate_with_callables(self, cfg, actions, obs0, perms, eps, returns, row_returns, window):
         """The evaluation ``cfg`` describes with the caller's reward / termination callables: per window of T steps one
         trajectory launch (next observations, kernel-side reward / done), the callables on the window's T * B rows, and

@@ -54,6 +54,13 @@ class Optimizer(_RefOptimizer):  # mbrl/planning/trajectory_opt.py:21-40
     def optimize(self, obj_fun, x0=None, **kwargs):
         raise NotImplementedError
 
+    def optimize_batch(self, obj_funs, x0=None, callback=None, **kwargs):
+        """One plan per objective of ``obj_funs`` from the warm starts ``x0 [K, H, A]``.  Only CEMOptimizer keeps no state
+        between calls besides the warm start; an optimiser that does (iCEM's kept elites, MPPI's mean) would have to split
+        it per problem, which is not implemented."""
+        raise NotImplementedError(f"{type(self).__name__} does not plan for a batch of observations; "
+                                  "CEMOptimizer is the optimiser that supports act_batch")
+
 
 class _FusedObjective:
     """Callable handed to the optimiser when the objective is ModelEnv.evaluate_action_sequences."""
@@ -64,6 +71,16 @@ class _FusedObjective:
     def __call__(self, action_sequences: torch.Tensor) -> torch.Tensor:
         return self.model_env.evaluate_action_sequences(action_sequences, initial_state=self.obs,
                                                         num_particles=self.num_particles)
+
+
+class _FusedBatchObjective:
+    """The objectives of K observations when they all are ModelEnv.evaluate_action_sequences of one environment."""
+
+    def __init__(self, model_env, obs: np.ndarray, num_particles: int):
+        self.model_env, self.obs, self.num_particles = model_env, obs, num_particles
+
+    def entries(self) -> List[_FusedObjective]:
+        return [_FusedObjective(self.model_env, o, self.num_particles) for o in self.obs]
 
 
 def _next_seed_offset(obj) -> int:
@@ -92,6 +109,7 @@ class CEMOptimizer(Optimizer):
         self._seed = int(torch.initial_seed()) & 0xFFFFFFFFFFFFFFFF
         self._ws = None
         self._plan_ws = None
+        self._plan_batch_ws = None
         self.record_values = False
         self.last_values = None
 
@@ -147,6 +165,64 @@ class CEMOptimizer(Optimizer):
                     _lib.ptr(b["best_sol"]), None, None, _lib.ptr(b["ws"]), b["ws"].numel(), stream), "cem_update")
         out = mu if self.return_mean_elites else b["best_sol"]
         return out.view(shape).clone()
+
+    def optimize_batch(self, obj_funs, x0: torch.Tensor, callback=None, *, _noise=None, _model_noise=None,
+                       **kwargs) -> torch.Tensor:
+        """K independent plans from the warm starts ``x0 [K, H, A]``; returns ``[K, H, A]``.  ``obj_funs`` is a
+        :class:`_FusedBatchObjective` (the model's objective for K observations) or a list of K objectives.  The model's
+        objective with no callback and no reward / termination callable runs as one batched device-resident plan
+        (``b200pets_cem_plan_batch``); anything else runs :meth:`optimize` once per entry, each from its own warm start."""
+        x0 = x0.to(self.device, torch.float32).contiguous()
+        if isinstance(obj_funs, _FusedBatchObjective):
+            if callback is None and not obj_funs.model_env.has_external_callables():
+                return self._optimize_fused_batch(obj_funs, x0, _noise, _model_noise)
+            obj_funs = obj_funs.entries()
+        if len(obj_funs) != x0.shape[0]:
+            raise ValueError(f"{len(obj_funs)} objectives for {x0.shape[0]} warm starts")
+        return torch.stack([self.optimize(f, x0=x0[k], callback=callback) for k, f in enumerate(obj_funs)])
+
+    def _optimize_fused_batch(self, obj: _FusedBatchObjective, x0, noise, model_noise) -> torch.Tensor:
+        env = obj.model_env
+        env._fresh()
+        K, H, A = x0.shape
+        obs = np.asarray(obj.obs)
+        if obs.ndim != 2 or obs.shape[0] != K:
+            raise ValueError(f"observations must be [K={K}, obs_dim], got {tuple(obs.shape)}")
+        prop = env._propagation()
+        perms = eps = None
+        if model_noise is not None:
+            perms, eps = model_noise
+        if perms is None and prop in ("random_model", "fixed_model") and (
+                env.ts1 == "perms" or env._few_groups(self.population_size, obj.num_particles)):
+            B = self.population_size * obj.num_particles
+            n = H if prop == "random_model" else 1
+            perms = torch.stack([torch.stack([torch.stack([torch.randperm(B, device=self.device) for _ in range(n)])
+                                              for _ in range(self.num_iterations)]) for _ in range(K)])
+        # problem k plans with counter value first + k: the one its own single plan would take k calls later
+        rcfg = _lib.RolloutCfg(self.population_size, H, obj.num_particles, _lib.PREC[env.precision_for(prop)], _lib.PROP[prop],
+                               _lib.TS1_PERMS if perms is not None else _lib.TS1_TILE_SHUFFLE, env._seed,
+                               env._next_offset())
+        env._offset += K - 1
+        ccfg = _lib.CemCfg(self.num_iterations, self.elite_num, float(self.alpha), int(self.return_mean_elites),
+                           int(self._clipped_normal))
+        need = self.lib.b200pets_cem_plan_batch_workspace_bytes(env.staged.handle, C.byref(rcfg), C.byref(ccfg), K)
+        if self._plan_batch_ws is None or self._plan_batch_ws.numel() < need:
+            self._plan_batch_ws = torch.empty(max(need, 1), dtype=torch.uint8, device=self.device)
+        obs0 = torch.from_numpy(np.ascontiguousarray(obs, dtype=np.float32)).to(self.device)
+        sol = torch.empty(K, H * A, dtype=torch.float32, device=self.device)
+        z = None if noise is None else noise.to(self.device, torch.float32).contiguous()
+        if perms is not None:
+            perms = perms.to(torch.int64).contiguous()
+        self.last_values = None
+        if self.record_values:
+            self.last_values = torch.empty(K, self.num_iterations, self.population_size, device=self.device)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.b200pets_cem_plan_batch(
+                env.staged.handle, C.byref(rcfg), C.byref(ccfg), K, _lib.ptr(obs0), _lib.ptr(x0), _lib.ptr(self.lower_bound),
+                _lib.ptr(self.upper_bound), _lib.ptr(z), _lib.ptr(eps), _lib.ptr(perms), _lib.ptr(sol),
+                _lib.ptr(self.last_values), _lib.ptr(self._plan_batch_ws), self._plan_batch_ws.numel(), _lib.stream_ptr()),
+                "cem_plan_batch")
+        return sol.view(K, H, A)
 
     def _optimize_fused(self, obj: _FusedObjective, x0, noise, model_noise) -> torch.Tensor:
         env = obj.model_env
@@ -374,6 +450,8 @@ class TrajectoryOptimizer:
         self.horizon = planning_horizon
         self.lib = _lib.load()
         self._pin = None  # pinned staging buffer for the plan, allocated on first use
+        self.previous_solutions: Optional[torch.Tensor] = None  # [K, H, A] warm starts of optimize_batch
+        self._pin_batch = None
 
     def optimize(self, trajectory_eval_fn, callback: Optional[Callable] = None) -> np.ndarray:
         best = self.optimizer.optimize(trajectory_eval_fn, x0=self.previous_solution, callback=callback).contiguous()
@@ -392,6 +470,36 @@ class TrajectoryOptimizer:
     def reset(self):
         self.previous_solution = self.initial_solution.clone()
 
+    def optimize_batch(self, trajectory_eval_fns, num_problems: int, callback: Optional[Callable] = None) -> np.ndarray:
+        """:meth:`optimize` for K observations at once: K plans from K warm starts (kept in ``previous_solutions``,
+        created on the first call and re-created when K changes, shifted after each plan with the rule of
+        :meth:`optimize`).  Returns the plans ``[K, H, A]`` through one device-to-host copy."""
+        K = num_problems
+        if self.previous_solutions is None or self.previous_solutions.shape[0] != K:
+            self.previous_solutions = self.initial_solution.repeat(K, 1, 1).contiguous()
+        best = self.optimizer.optimize_batch(trajectory_eval_fns, x0=self.previous_solutions, callback=callback).contiguous()
+        if self.keep_last_solution:
+            _, H, A = best.shape
+            with torch.cuda.device(best.device):
+                for k in range(K):
+                    _lib.check(self.lib.b200pets_shift_solution(H, A, self.replan_freq, _lib.ptr(best[k]),
+                                                                _lib.ptr(self.initial_solution),
+                                                                _lib.ptr(self.previous_solutions[k]), _lib.stream_ptr()),
+                               "shift_solution")
+        if self._pin_batch is None or self._pin_batch.shape != best.shape:
+            self._pin_batch = torch.empty(best.shape, dtype=torch.float32).pin_memory()
+        self._pin_batch.copy_(best, non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        return self._pin_batch.numpy().copy()
+
+    def reset_batch(self, indices: Optional[Sequence[int]] = None):
+        """Restore the warm starts of the batch entries ``indices`` (all of them when None)."""
+        if indices is None or self.previous_solutions is None:
+            self.previous_solutions = None
+            return
+        idx = torch.as_tensor(list(indices), dtype=torch.int64, device=self.previous_solutions.device)
+        self.previous_solutions[idx] = self.initial_solution
+
 
 class TrajectoryOptimizerAgent(Agent):
     """trajectory_opt.py:575-716."""
@@ -409,6 +517,7 @@ class TrajectoryOptimizerAgent(Agent):
         self.verbose = verbose
         self._fused_env = None
         self._fused_particles = 1
+        self._batch_actions: List[np.ndarray] = []  # [K, A] actions of the batch's last plan still to be used
 
     def set_trajectory_eval_fn(self, trajectory_eval_fn):
         self.trajectory_eval_fn = trajectory_eval_fn
@@ -454,6 +563,39 @@ class TrajectoryOptimizerAgent(Agent):
         if self.trajectory_eval_fn is None:
             raise RuntimeError("Please call `set_trajectory_eval_fn()` before using TrajectoryOptimizerAgent")
         return self.optimizer.optimize(self._objective(obs))
+
+    def act_batch(self, obs: np.ndarray, optimizer_callback: Optional[Callable] = None, **_kwargs) -> np.ndarray:
+        """:meth:`act` for K observations at once (a vectorised environment, several episodes or seeds): returns the
+        actions ``[K, A]``.  Each entry plans as :meth:`act` would, from its own warm start; with the model's objective
+        the K plans run as one batched device-resident plan.  With ``replan_freq > 1`` every entry replans at the same
+        steps.  The batch keeps its own warm starts and cached actions: :meth:`act` / :meth:`reset` do not touch them,
+        :meth:`reset_batch` restores them."""
+        if self.trajectory_eval_fn is None:
+            raise RuntimeError("Please call `set_trajectory_eval_fn()` before using TrajectoryOptimizerAgent")
+        obs = np.asarray(obs)
+        K = obs.shape[0]
+        if self._batch_actions and self._batch_actions[0].shape[0] != K:
+            self._batch_actions = []
+        plan_time = 0.0
+        if not self._batch_actions:
+            if self._fused_env is not None:
+                objective = _FusedBatchObjective(self._fused_env, obs, self._fused_particles)
+            else:
+                objective = [self._objective(o) for o in obs]
+            start_time = time.time()
+            plans = self.optimizer.optimize_batch(objective, K, callback=optimizer_callback)
+            plan_time = time.time() - start_time
+            self._batch_actions = [plans[:, i] for i in range(min(self.replan_freq, plans.shape[1]))]
+        actions = self._batch_actions.pop(0)
+        if self.verbose:
+            print(f"Planning time: {plan_time:.3f}")
+        return actions
+
+    def reset_batch(self, indices: Optional[Sequence[int]] = None):
+        """Restore the warm starts of the batch entries ``indices`` (every entry when None) and drop the cached actions,
+        so that the next :meth:`act_batch` replans."""
+        self.optimizer.reset_batch(indices)
+        self._batch_actions = []
 
 
 _KNOWN_TARGETS["TrajectoryOptimizerAgent"] = TrajectoryOptimizerAgent
