@@ -292,7 +292,8 @@ int b200pets_cem_elites_refit(int32_t local_population, int32_t first_sequence, 
                               uint32_t* tag_word, float* population_out, void* stream);
 
 /* iCEM sampling (trajectory_opt.py:433-441 + util/math.py:318-396): coloured noise along the horizon from
- * N(0,1) draws sr, si [dev] float[n][A][H/2+1] (or NULL = Philox), scaled by sqrt(var) + mu and clipped. */
+ * N(0,1) draws sr, si [dev] float[n][A][H/2+1] (or NULL = Philox), scaled by sqrt(var) + mu and clipped.
+ * horizon < 2 is refused (B200PETS_EINVAL): a one-sample series has no frequency to normalise the noise by. */
 int b200pets_icem_sample(int32_t n, int32_t horizon, int32_t act_dim, float exponent, const float* mu,
                          const float* var, const float* lower, const float* upper, const float* sr,
                          const float* si, uint64_t seed, uint64_t offset, float* population_out,

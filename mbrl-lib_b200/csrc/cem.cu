@@ -1141,6 +1141,11 @@ int b200pets_icem_sample(int32_t n, int32_t horizon, int32_t act_dim, float expo
                          uint64_t seed, uint64_t offset, float* population_out, void* stream) {
   if (n <= 0 || horizon <= 0 || act_dim <= 0) return b200pets_set_error(B200PETS_EINVAL, "icem_sample: empty population");
   if ((sr == nullptr) != (si == nullptr)) return b200pets_set_error(B200PETS_EINVAL, "icem_sample: sr and si go together");
+  // a one-sample series has no frequency above DC, so the noise's normalising sigma is 0 (the reference's
+  // powerlaw_psd_gaussian fails on it too); refuse rather than return a population of +-inf clipped to the bounds
+  if (horizon < 2)
+    return b200pets_set_error(B200PETS_EINVAL, "icem_sample: coloured noise needs a horizon of at least 2 (a one-step "
+                                               "series has no frequency above DC to normalise by)");
   long long tot = (long long)n * act_dim;
   icem_sample_kernel<<<(unsigned)((tot + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
       n, horizon, act_dim, exponent, mu, var, lower, upper, sr, si, rng_key(seed, offset), offset, population_out);

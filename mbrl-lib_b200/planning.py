@@ -305,8 +305,11 @@ class ICEMOptimizer(Optimizer):
         return sizes
 
     def optimize(self, obj_fun, x0: Optional[torch.Tensor] = None, callback=None, *, _noise=None, **kwargs) -> torch.Tensor:
-        x0 = x0.to(self.device, torch.float32).contiguous()
         H, A = x0.shape
+        if H < 2:  # b200pets_icem_sample refuses it too; checked here before anything is launched
+            raise ValueError(f"ICEMOptimizer needs a planning horizon of at least 2, got {H}: coloured noise over a "
+                             "one-step series has no frequency above DC to normalise by")
+        x0 = x0.to(self.device, torch.float32).contiguous()
         dims = H * A
         dev = self.device
         mu = x0.reshape(-1).clone()

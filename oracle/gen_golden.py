@@ -4,7 +4,7 @@ container only:
     PYTHONPATH=oracle/ref_shims:oracle/_ref python oracle/gen_golden.py [NAME ...]
 
 With NAMEs, only the rollout goldens of those synthetic cases are (re)written, e.g. `... gen_golden.py plan_k3`; every
-other file under tests/golden stays as it is.  The reference's RNG calls (torch.randperm, torch.normal, truncated_normal_) are monkey-fed the same
+other file under tests/golden stays as it is; `... gen_golden.py --icem-noise` writes only tests/golden/icem_noise.npz.  The reference's RNG calls (torch.randperm, torch.normal, truncated_normal_) are monkey-fed the same
 injected draws that `mbrl_lib_b200.synthetic` regenerates from numpy seeds anywhere, so the committed
 `tests/golden/*.npz` hold only outputs + input checksums.  TEST INFRASTRUCTURE; nothing shipped uses it.
 """
@@ -240,6 +240,26 @@ def gen_icem():
     print("icem", sols[1][0].tolist())
 
 
+ICEM_NOISE_H = (2, 3, 7, 8, 10, 25, 30, 40, 41)
+ICEM_NOISE_EXPONENTS = (0.0, 0.5, 1.0, 2.0, 2.5, 4.0)
+
+
+def gen_icem_noise():
+    """The reference's powerlaw_psd_gaussian on a [3, 2, H] batch, fed unit normals as gen_icem feeds it, at every
+    horizon (odd and even) and exponent the GPU tests of the coloured-noise kernel use."""
+    g = np.random.default_rng(2024)
+    out = {"horizons": np.array(ICEM_NOISE_H), "exponents": np.array(ICEM_NOISE_EXPONENTS)}
+    for H in ICEM_NOISE_H:
+        for ei, beta in enumerate(ICEM_NOISE_EXPONENTS):
+            sr = g.standard_normal((3, 2, H // 2 + 1)).astype(np.float32)
+            si = g.standard_normal((3, 2, H // 2 + 1)).astype(np.float32)
+            with FeedRNG(normals=[torch.from_numpy(sr), torch.from_numpy(si)]):
+                y = mbrl.util.math.powerlaw_psd_gaussian(beta, (3, 2, H), "cpu")
+            out[f"h{H}_e{ei}_sr"], out[f"h{H}_e{ei}_si"], out[f"h{H}_e{ei}_y"] = sr, si, y.numpy()
+    np.savez(os.path.join(GOLD, "icem_noise.npz"), **out)
+    print("icem_noise", len(ICEM_NOISE_H) * len(ICEM_NOISE_EXPONENTS), "series sets")
+
+
 def gen_mppi():
     g = np.random.default_rng(99)
     N, H, A, iters = 48, 6, 2, 3
@@ -305,6 +325,9 @@ def gen_counter_world():
 if __name__ == "__main__":
     torch.manual_seed(0)
     os.makedirs(GOLD, exist_ok=True)
+    if sys.argv[1:] == ["--icem-noise"]:
+        gen_icem_noise()
+        sys.exit(0)
     if len(sys.argv) > 1:
         for nm in sys.argv[1:]:
             gen_rollout(nm)
@@ -319,6 +342,7 @@ if __name__ == "__main__":
     gen_cem("trunc_mean", clipped=False, return_mean=True)
     gen_cem("clipped_best", clipped=True, return_mean=False)
     gen_icem()
+    gen_icem_noise()
     gen_mppi()
     gen_cem_model()
     gen_counter_world()

@@ -35,6 +35,9 @@ REFIT_SHAPES = {
     "single_cta": (500, 180, 50, 1, 0, True),
     "counting_config3": (1000, 680, 100, 1, 1, True),
     "counting_global_partials": (1500, 1300, 40, 0, 0, False),
+    # iCEM's flags (biased variance, no std, elite rows out) at bench config 3's first and last populations
+    "counting_icem_first": (1030, 680, 100, 0, 0, True),
+    "counting_icem_last": (356, 680, 100, 0, 0, True),
     "radix_config5": (64000, 36, 6400, 1, 0, False),
     "radix_global_partials": (5000, 1300, 60, 0, 1, True),
 }

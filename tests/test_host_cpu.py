@@ -89,6 +89,30 @@ def test_icem_schedule_matches_reference_rule():
     assert opt.elite_num == 100 and opt.keep_elite_size == 35  # SURVEY.md section 8 a4
 
 
+def test_icem_sample_refuses_a_one_step_horizon():
+    """A one-sample series has no frequency above DC, so the coloured noise's sigma is 0 and the samples would be
+    +-inf clipped to the bounds: the ABI refuses horizon 1 before any CUDA call, with a message that says why."""
+    from mbrl_lib_b200 import _lib
+
+    lib = _lib.load()
+    rc = lib.b200pets_icem_sample(8, 1, 3, 2.0, None, None, None, None, None, None, 0, 0, None, None)
+    assert rc == -1  # B200PETS_EINVAL
+    msg = lib.b200pets_last_error().decode()
+    assert "horizon of at least 2" in msg, msg
+    rc = lib.b200pets_icem_sample(8, 0, 3, 2.0, None, None, None, None, None, None, 0, 0, None, None)
+    assert rc == -1 and "empty population" in lib.b200pets_last_error().decode()
+
+
+def test_icem_optimizer_refuses_a_one_step_horizon():
+    import mbrl_lib_b200 as bp
+
+    opt = bp.ICEMOptimizer(2, 0.1, 50, 1.3, 2.0, [[-1.0, -1.0]], [[1.0, 1.0]], 0.3, 0.1, "cpu")
+    calls = []
+    with pytest.raises(ValueError, match="horizon of at least 2"):
+        opt.optimize(lambda pop: calls.append(pop), x0=torch.zeros(1, 2))
+    assert not calls and opt.elite is None
+
+
 def test_target_strings_select_b200_classes():
     from mbrl_lib_b200 import planning
 

@@ -109,6 +109,25 @@ def test_icem_matches_reference(golden_dir):
         np.testing.assert_allclose(elite.numpy(), g[f"c{call}_elite"], rtol=1e-5, atol=1e-6)
 
 
+def test_colored_noise_matches_reference(golden_dir):
+    """po.powerlaw_psd_from_normals against the reference's powerlaw_psd_gaussian at every horizon (odd and even) and
+    exponent the GPU tests of the coloured-noise kernel use."""
+    from test_gpu_optimizers import colored64
+
+    g = _load(golden_dir, "icem_noise.npz")
+    horizons, exponents = g["horizons"].tolist(), g["exponents"].tolist()
+    assert {2, 3, 7, 8, 10, 30, 40, 41} <= set(horizons) and {0.0, 1.0, 2.0, 2.5, 4.0} <= set(exponents)
+    for H in horizons:
+        for ei, beta in enumerate(exponents):
+            sr, si, want = (g[f"h{H}_e{ei}_{k}"] for k in ("sr", "si", "y"))
+            assert sr.shape == (3, 2, H // 2 + 1) and want.shape == (3, 2, H)
+            got = po.powerlaw_psd_from_normals(beta, torch.from_numpy(sr), torch.from_numpy(si), H).numpy()
+            np.testing.assert_allclose(got, want, rtol=1e-6, atol=1e-6 * np.abs(want).max(), err_msg=f"H {H} exponent {beta}")
+            # the float64 restatement tests/test_gpu_optimizers.py judges the kernel by
+            np.testing.assert_allclose(colored64(sr, si, H, beta), want, rtol=1e-5, atol=1e-5 * np.abs(want).max(),
+                                       err_msg=f"H {H} exponent {beta}")
+
+
 def test_mppi_matches_reference(golden_dir):
     g = _load(golden_dir, "mppi.npz")
     t = lambda k: torch.from_numpy(g[k])  # noqa: E731
