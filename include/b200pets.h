@@ -321,8 +321,11 @@ int b200pets_shift_solution(int32_t horizon, int32_t act_dim, int32_t replan_fre
                             const float* initial_row, float* previous_solution, void* stream);
 
 /* Fused CEM plan over the model (CEMOptimizer.optimize driving evaluate_action_sequences,
- * trajectory_opt.py:142-188): enqueues num_iterations x (sample -> rollout -> refit) on `stream` with no
- * host round trip.  z / eps / perms as above with a leading [num_iterations] dimension, or NULL.
+ * trajectory_opt.py:142-188): enqueues the first population, then per iteration the rollout and one kernel that refits
+ * and draws the next population (two launches per iteration), on `stream` with no host round trip.  Outside that
+ * kernel's single-CTA refit (more than 2048 sequences, fewer than 2 elites, or elite rows over 150 KB) the plan runs
+ * sample -> rollout -> refit instead (three launches per iteration).  z / eps / perms as above with a leading
+ * [num_iterations] dimension, or NULL.
  *   x0 [dev] float[H*A]; lower/upper [dev] float[H*A]
  *   solution [dev] float[H*A]; values_out [dev] float[num_iterations][N] or NULL */
 typedef struct {

@@ -1,7 +1,6 @@
 // C ABI of libb200pets: model staging (pack), rollout dispatch, fused CEM plan.  See include/b200pets.h.
 #include <stdarg.h>
 #include <stdio.h>
-#include <stdlib.h>
 #include <string.h>
 
 #include <cuda_bf16.h>
@@ -570,7 +569,6 @@ __global__ void cem_init_kernel(int dims, const float* __restrict__ x0, const fl
   const int d = blockIdx.x * blockDim.x + threadIdx.x;
   if (d == 0) {
     *best_value = -INFINITY;
-    *reinterpret_cast<unsigned int*>(best_value + 1) = 0u;  // tail counter of the fused iteration kernel
     *reinterpret_cast<unsigned int*>(best_value + 2) = 0u;  // "refit done" tag of cem_refit_sample_kernel
   }
   if (d >= dims) return;
@@ -611,22 +609,10 @@ int b200pets_cem_plan(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, 
 
   cem_init_kernel<<<(dims + 255) / 256, 256, 0, stream>>>(dims, x0, lower, upper, ccfg->clipped_normal, mu, disp, best_val);
   CUDA_TRY(cudaGetLastError());
-  // Default: sample -> rollout -> refit (3 launches per iteration; the refit kernel fuses the particle mean).  B200PETS_CEM_FUSED=1 selects the fused variants (parity-tested, not the default): refit by the last CTA of the
-  // rollout kernel (2 launches / iteration) and, with B200PETS_CEM_SAMPLE_IN_KERNEL=1, the population drawn inside the
-  // rollout kernel too (1 launch / iteration: every particle row re-derives its sequence's actions).
-  const char* env_fuse = getenv("B200PETS_CEM_FUSED");
-  const bool fuse = (env_fuse && env_fuse[0] == '1') && rcfg->precision == B200PETS_PREC_BF16_TC && model->tc_ok && !z &&
-                    !perms && N <= 2048 && dims <= 1024 && ccfg->elite_num >= 2 && ccfg->elite_num <= N &&
-                    rcfg->propagation != B200PETS_PROP_EXPECTATION && B % model->desc.num_members == 0 &&
-                    model->desc.reward_fn != B200PETS_REWARD_EXTERNAL && model->desc.term_fn != B200PETS_TERM_EXTERNAL;
-  const char* env_sik = getenv("B200PETS_CEM_SAMPLE_IN_KERNEL");
-  const bool sample_in_kernel = env_sik && env_sik[0] == '1';
-  // Default: 2 launches per iteration -- rollout, then ONE kernel that refits (particle mean + top-k + mean / variance) and
-  // draws the next iteration's population (cem.cu cem_refit_sample_kernel); the first population comes from the same
-  // kernel in sample-only mode.  B200PETS_CEM_MERGED=0 (or a population outside the single-CTA refit) keeps the three
-  // separate kernels.
-  static const bool merged_env = [] { const char* e = getenv("B200PETS_CEM_MERGED"); return !(e && e[0] == '0'); }();
-  const bool merged = merged_env && !fuse && cem_refit_sample_supported(N, dims, ccfg->elite_num);
+  // Per iteration: the rollout, then ONE kernel that refits (particle mean + top-k + mean / variance) and draws the next
+  // iteration's population (cem.cu cem_refit_sample_kernel); the first population comes from the same kernel in
+  // sample-only mode.  A population outside that kernel's single-CTA refit runs sample -> rollout -> refit instead.
+  const bool merged = cem_refit_sample_supported(N, dims, ccfg->elite_num);
   unsigned int* refit_flag = reinterpret_cast<unsigned int*>(best_val + 2);
   auto next_pop = [&](int it_next, int refit, const float* totals) -> int {  // refit of it_next - 1 (if any) + population of it_next
     const int sample = it_next < ccfg->num_iterations;
@@ -641,73 +627,25 @@ int b200pets_cem_plan(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, 
     if (rc0) return rc0;
   }
   for (int it = 0; it < ccfg->num_iterations; ++it) {
-    if (merged) {
-      b200pets_rollout_cfg rc_it = *rcfg;
-      rc_it.offset = rcfg->offset * 1024 + it;
-      const int nperm = rcfg->propagation == B200PETS_PROP_FIXED_MODEL ? 1 : H;
-      float* totals = nullptr;
-      int rc = eval_rows(model, &rc_it, obs0, pop, perms ? perms + (size_t)it * nperm * B : nullptr,
-                         eps ? eps + (size_t)it * H * B * model->desc.out_size : nullptr, nullptr, eval_ws, eval_bytes, stream,
-                         &totals);
-      if (rc) return rc;
-      rc = next_pop(it + 1, 1, totals);
-      if (rc) return rc;
-      if (values_out) CUDA_TRY(cudaMemcpyAsync(values_out + (size_t)it * N, values, sizeof(float) * N, cudaMemcpyDeviceToDevice, stream));
-      continue;
+    if (!merged) {
+      int rcs = b200pets_cem_sample_shard(N, rcfg->first_sequence, dims, mu, disp, lower, upper,
+                                          z ? z + (size_t)it * N * dims : nullptr, rcfg->seed, rcfg->offset * 1024 + it,
+                                          ccfg->clipped_normal, pop, stream);
+      if (rcs) return rcs;
     }
-    if (fuse) {
-      // default: population drawn by cem_sample_kernel, rollout + refit in one kernel (2 launches per iteration);
-      // B200PETS_CEM_SAMPLE_IN_KERNEL=1 also draws the population inside the rollout kernel (1 launch per iteration,
-      // measured slower: every particle row re-derives its sequence's actions on the epilogue's critical path)
-      if (!sample_in_kernel) {
-        int rcs = b200pets_cem_sample_shard(N, rcfg->first_sequence, dims, mu, disp, lower, upper, nullptr, rcfg->seed,
-                                            rcfg->offset * 1024 + it, ccfg->clipped_normal, pop, stream);
-        if (rcs) return rcs;
-      }
-      unsigned char* ews = reinterpret_cast<unsigned char*>(eval_ws);
-      const size_t o1 = ((size_t)B * model->desc.obs_dim * sizeof(float) + 255) & ~(size_t)255;
-      RolloutArgs a{};
-      a.N = N; a.H = H; a.P = P; a.B = B;
-      a.t0 = 0; a.t1 = H;
-      a.propagation = rcfg->propagation;
-      a.slot_mode = rcfg->propagation == B200PETS_PROP_RANDOM_MODEL ? 1 : 2;
-      a.sample = 1;
-      a.offset = rcfg->offset * 1024 + it; a.seed = rng_key(rcfg->seed, a.offset);
-      { int rcs = shard_of(rcfg, &a.seq0, &a.n_glob); if (rcs) return rcs; }
-      a.eps = eps ? eps + (size_t)it * H * B * model->desc.out_size : nullptr;
-      a.obs0 = obs0; a.init_from_obs0 = 1; a.store_state = 1;
-      a.total_state = reinterpret_cast<float*>(ews + o1);
-      a.dead_state = ews + o1 + (((size_t)B * sizeof(float) + 255) & ~(size_t)255);
-      a.act = pop; a.act_div = P; a.act_row_stride = (long long)H * A; a.act_t_stride = A;
-      if (sample_in_kernel) {
-        a.cem_mu = mu; a.cem_disp = disp; a.cem_lb = lower; a.cem_ub = upper;
-        a.cem_offset = rcfg->offset * 1024 + it;
-      }
-      a.cem_clipped = ccfg->clipped_normal;
-      a.pop_out = pop;
-      a.tail_counter = reinterpret_cast<unsigned int*>(best_val + 1);
-      a.tail_values = values; a.tail_mu = mu; a.tail_disp = disp; a.tail_best_value = best_val; a.tail_best_solution = best_sol;
-      a.tail_elite_num = ccfg->elite_num; a.tail_alpha = ccfg->alpha;
-      int rc = dispatch(model, B200PETS_PREC_BF16_TC, a, stream);
-      if (rc) return rc;
-      if (values_out) CUDA_TRY(cudaMemcpyAsync(values_out + (size_t)it * N, values, sizeof(float) * N, cudaMemcpyDeviceToDevice, stream));
-      continue;
-    }
-    int rc = b200pets_cem_sample_shard(N, rcfg->first_sequence, dims, mu, disp, lower, upper,
-                                       z ? z + (size_t)it * N * dims : nullptr, rcfg->seed, rcfg->offset * 1024 + it,
-                                       ccfg->clipped_normal, pop, stream);
-    if (rc) return rc;
     b200pets_rollout_cfg rc_it = *rcfg;
     rc_it.offset = rcfg->offset * 1024 + it;
     const int nperm = rcfg->propagation == B200PETS_PROP_FIXED_MODEL ? 1 : H;
     float* totals = nullptr;
-    rc = eval_rows(model, &rc_it, obs0, pop, perms ? perms + (size_t)it * nperm * B : nullptr,
-                   eps ? eps + (size_t)it * H * B * model->desc.out_size : nullptr, nullptr, eval_ws, eval_bytes, stream,
-                   &totals);
+    int rc = eval_rows(model, &rc_it, obs0, pop, perms ? perms + (size_t)it * nperm * B : nullptr,
+                       eps ? eps + (size_t)it * H * B * model->desc.out_size : nullptr, nullptr, eval_ws, eval_bytes, stream,
+                       &totals);
     if (rc) return rc;
-    // particle mean + NaN rule + top-k + refit in ONE kernel (3 launches per iteration: sample, rollout, refit)
-    rc = launch_cem_update_rows(N, dims, ccfg->elite_num, ccfg->alpha, 1, ccfg->clipped_normal, pop, totals, P, values, mu,
-                                disp, best_val, best_sol, upd_ws, upd_bytes, stream);
+    if (merged)
+      rc = next_pop(it + 1, 1, totals);
+    else  // particle mean + NaN rule + top-k + refit in one kernel
+      rc = launch_cem_update_rows(N, dims, ccfg->elite_num, ccfg->alpha, 1, ccfg->clipped_normal, pop, totals, P, values, mu,
+                                  disp, best_val, best_sol, upd_ws, upd_bytes, stream);
     if (rc) return rc;
     // NB: values_out then holds the values AFTER the reference's in-place NaN rule (trajectory_opt.py:178)
     if (values_out) CUDA_TRY(cudaMemcpyAsync(values_out + (size_t)it * N, values, sizeof(float) * N, cudaMemcpyDeviceToDevice, stream));

@@ -69,22 +69,6 @@ struct RolloutArgs {
   float* traj_obs;         // [t1-t0][B][D] next observation
   float* traj_reward;      // [t1-t0][B] the learned column or the known reward function, 0 for an external one
   uint8_t* traj_done;      // [t1-t0][B] the known termination function, 0 for an external one
-  // ---- fused CEM iteration (tensor-core kernel only): population sampled in-kernel, refit by the last CTA ----
-  const float* cem_mu;     // [H*A] sampling mean; non-NULL switches the action source to in-kernel sampling
-  const float* cem_disp;   // [H*A] variance (truncated normal) or std (clipped normal)
-  const float* cem_lb;     // [H*A]
-  const float* cem_ub;     // [H*A]
-  int cem_clipped;
-  unsigned long long cem_offset;  // Philox offset of the population draw (same keying as b200pets_cem_sample)
-  float* pop_out;          // [N][H][A] population, written by each sequence's particle-0 row
-  unsigned int* tail_counter;     // zero-initialised; non-NULL: the last CTA to finish refits (mu, sigma) in place
-  float* tail_values;      // [N] particle-mean returns (out)
-  float* tail_mu;          // [H*A] in/out
-  float* tail_disp;        // [H*A] in/out
-  float* tail_best_value;  // [1] in/out
-  float* tail_best_solution;  // [H*A] in/out
-  int tail_elite_num;
-  float tail_alpha;
 };
 
 // A batched launch: K independent evaluations of one configuration in one grid.  Tiles are problem-major (tile =
@@ -369,18 +353,13 @@ __device__ __forceinline__ long long prob_rid(const RolloutArgs& a, const BatchA
 // constant tables, the first weight prefetches -- memory no kernel of the chain writes) and blocks in pdl_wait() until
 // the predecessor grid has completed and flushed, BEFORE its first access to anything the chain produces.  Every
 // kernel of the chain waits before it finishes, so completion is transitive along the chain.  Launch gaps and the
-// rollout kernel's ~6 us prologue thereby overlap the tail of the previous kernel.  B200PETS_PDL=0 disables it.
+// rollout kernel's ~6 us prologue thereby overlap the tail of the previous kernel.
 // ------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
 #ifdef __CUDACC__
-#include <stdlib.h>
 #include <utility>
-static inline bool pdl_enabled() {
-  static const bool on = [] { const char* e = getenv("B200PETS_PDL"); return !(e && e[0] == '0'); }();
-  return on;
-}
 template <typename... KArgs, typename... Args>
 static inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
                                      Args&&... args) {
@@ -391,7 +370,7 @@ static inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 blo
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kern, std::forward<Args>(args)...);

@@ -53,11 +53,8 @@ namespace {
 constexpr int kTileM = 128;  // rows of a tile: a shuffle group, a member's slot range chunk, an expectation chunk
 template <int NWG>
 constexpr int threads_of() { return 128 * NWG + 32; }
-constexpr int kTailWarps = 9;  // cem_tail_refit's reduction order: partial sums over 9 strided element sets
 constexpr int kSliceK16 = 4;       // longest ring slot in K steps (16 rows of the weight image each)
 constexpr int kMaxStages = 16;
-constexpr int kCemTabDims = 1024;  // horizon * act_dim supported by the fused CEM iteration
-constexpr uint32_t kTailScratch = 256 + 2048 * 9 + (kTailWarps + 1) * kCemTabDims * 4;  // cem_tail_refit's scratch
 
 __device__ __forceinline__ float tanh_approx(float x) {
   float y;
@@ -232,149 +229,15 @@ __device__ __forceinline__ uint32_t run_layer(const LayerArgs& la, uint32_t ring
   return ring_pos;
 }
 
-// Actions of (sequence n, step t) drawn from the CEM sampling distribution with exactly the Philox keying of
-// cem_sample_kernel (cem.cu): element d = t * A + j of sequence n <- block (n, d >> 2, RNG_STREAM_CEM | attempt)[d & 3],
-// redrawn until inside [-2, 2] (util/math.py:83-92) unless clipped_normal.  tab_mu / tab_sd: staged mean and
-// sqrt(constrained variance) (or std for clipped_normal).  Not inlined (cold, once per step per row).
-static __device__ __noinline__ void cem_sample_actions(unsigned long long seed, unsigned long long cem_offset, int clipped,
-                                                       const float* lb, const float* ub, const float* tab_mu,
-                                                       const float* tab_sd, int n, int t, int A, float* dst, float* pop_row) {
-  for (int j0 = 0; j0 < A;) {
-    const int d0 = t * A + j0;
-    const int blk = d0 >> 2;
-    float g[4];
-    philox_normal4((uint32_t)n, (uint32_t)blk, RNG_STREAM_CEM, (uint32_t)cem_offset, seed, g);
-    for (int e = d0 & 3; e < 4 && j0 < A; ++e, ++j0) {
-      const int d = t * A + j0;
-      float zz = g[e];
-      if (!clipped) {
-        uint32_t attempt = 0;
-        while (!(zz >= -2.0f && zz <= 2.0f) && attempt < 64) {
-          ++attempt;
-          float g2[4];
-          philox_normal4((uint32_t)n, (uint32_t)blk, RNG_STREAM_CEM | attempt, (uint32_t)cem_offset, seed, g2);
-          zz = g2[e];
-        }
-        zz = fminf(fmaxf(zz, -2.0f), 2.0f);
-      }
-      float v;
-      if (clipped) {
-        v = tab_mu[d] + tab_sd[d] * zz;
-        v = v > lb[d] ? v : lb[d];
-        v = v < ub[d] ? v : ub[d];
-      } else {
-        v = zz * tab_sd[d] + tab_mu[d];
-      }
-      dst[j0] = v;
-      if (pop_row) pop_row[d] = v;
-    }
-  }
-}
-
-// Refit of (mu, sigma) by the last CTA to finish a fused CEM iteration: particle means, NaN rule, top-k by counting
-// rank (ties -> lowest index), mean / unbiased variance (or std) of the elites, momentum, best-so-far.
-// Same arithmetic as cem_select_kernel (cem.cu) for populations <= 2048; scratch lives in the (now idle) weight ring.
-struct TailArgs {
-  int N, P, tail_elite_num, cem_clipped;
-  float tail_alpha;
-  const float* total_state;
-  const float* pop_out;
-  float *tail_values, *tail_mu, *tail_disp, *tail_best_value, *tail_best_solution;
-  unsigned int* tail_counter;
-};
-
-static __device__ __noinline__ void cem_tail_refit(const TailArgs* ap, int dims, uint8_t* scratch, int* sh_best) {
-  const TailArgs a = *ap;
-  const int tid = threadIdx.x, nthr = blockDim.x, lane = tid & 31, warp = tid >> 5, nwarp = nthr >> 5;
-  const int n = a.N, k = a.tail_elite_num, P = a.P;
-  float* sv = reinterpret_cast<float*>(scratch);
-  int* eidx = reinterpret_cast<int*>(sv + 2048);
-  unsigned char* sf = reinterpret_cast<unsigned char*>(eidx + 2048);
-  float* partial = reinterpret_cast<float*>(sf + 2048);  // [kTailWarps + 1][dims]
-  for (int i = tid; i < n; i += nthr) {
-    float s = 0.f;
-    for (int pp = 0; pp < P; ++pp) s += a.total_state[(size_t)i * P + pp];
-    float v = s / (float)P;
-    if (isnan(v)) v = -1e-10f;
-    sv[i] = v;
-    a.tail_values[i] = v;
-  }
-  __syncthreads();
-  for (int i = tid; i < n; i += nthr) {
-    const float vi = sv[i];
-    int rank = 0;
-    for (int j = 0; j < n; ++j) {
-      const float vj = sv[j];
-      rank += (vj > vi || (vj == vi && j < i)) ? 1 : 0;
-    }
-    sf[i] = rank < k ? 1 : 0;
-    if (rank == 0) *sh_best = i;
-  }
-  __syncthreads();
-  for (int i = tid; i < n; i += nthr) {
-    if (sf[i]) {
-      int pos = 0;
-      for (int j = 0; j < i; ++j) pos += sf[j];
-      eidx[pos] = i;
-    }
-  }
-  __syncthreads();
-  const int bi = *sh_best;
-  const float bv = sv[bi];
-  const float* pop = a.pop_out;
-  // elite sums in kTailWarps strided partial sums whatever the CTA's warp count: the same order at every CTA shape
-  for (int w = warp; w < kTailWarps; w += nwarp)
-    for (int d = lane; d < dims; d += 32) {
-      float acc = 0.f;
-      for (int e = w; e < k; e += kTailWarps) acc += pop[(size_t)eidx[e] * dims + d];
-      partial[w * dims + d] = acc;
-    }
-  __syncthreads();
-  for (int d = tid; d < dims; d += nthr) {
-    float acc = 0.f;
-    for (int w = 0; w < kTailWarps; ++w) acc += partial[w * dims + d];
-    partial[kTailWarps * dims + d] = acc / (float)k;
-  }
-  __syncthreads();
-  for (int w = warp; w < kTailWarps; w += nwarp)
-    for (int d = lane; d < dims; d += 32) {
-      const float mean = partial[kTailWarps * dims + d];
-      float acc = 0.f;
-      for (int e = w; e < k; e += kTailWarps) {
-        const float df = pop[(size_t)eidx[e] * dims + d] - mean;
-        acc += df * df;
-      }
-      partial[w * dims + d] = acc;
-    }
-  __syncthreads();
-  const bool better = bv > *a.tail_best_value;
-  for (int d = tid; d < dims; d += nthr) {
-    float acc = 0.f;
-    for (int w = 0; w < kTailWarps; ++w) acc += partial[w * dims + d];
-    const float mean = partial[kTailWarps * dims + d];
-    const float var = acc / (float)(k - 1);
-    const float nd = a.cem_clipped ? sqrtf(var) : var;
-    a.tail_mu[d] = a.tail_alpha * a.tail_mu[d] + (1.0f - a.tail_alpha) * mean;
-    a.tail_disp[d] = a.tail_alpha * a.tail_disp[d] + (1.0f - a.tail_alpha) * nd;
-    if (better) a.tail_best_solution[d] = pop[(size_t)bi * dims + d];
-  }
-  __syncthreads();
-  if (tid == 0) {
-    if (better) *a.tail_best_value = bv;
-    *a.tail_counter = 0u;  // ready for the next iteration's launch
-  }
-}
-
 // The rollout kernels' body, inlined into each kernel (ptxas serialises wgmma chains in a called function, C7510).
 // EXP: propagation "expectation" (member passes)
-// CEMF: fused-CEM features compiled in (in-kernel sampling, last-CTA refit)
 // TRAJ: per-step trajectory stores compiled in (b200pets_eval_trajectory); the other variants are compiled without them
 //       so that their schedule stays what it was
 // NWG: consumer warpgroups (TcPlan::nwg).  CTA tile u is half u % 2 of 128-row tile u / 2 when NWG = 1, tile u itself
 //      when NWG = 2; either way a row keeps its member, keys, operands and K order.
 // BATCH: K independent problems in one launch (common.cuh BatchArgs): 128-row tile j is local tile j % bt->tiles of
 //      problem j / bt->tiles, and everything after that decode is the single-problem code.
-template <int ACT, bool CEMF, bool EXP, bool TRAJ, int NWG, bool BATCH>
+template <int ACT, bool EXP, bool TRAJ, int NWG, bool BATCH>
 __device__ __forceinline__ void rollout_tc_body(const ModelDev& m, const RolloutArgs& a, const TcPlan& p, const long long num_tiles,
                                                 const BatchArgs* bt) {
   extern __shared__ __align__(128) uint8_t smem[];
@@ -398,7 +261,6 @@ __device__ __forceinline__ void rollout_tc_body(const ModelDev& m, const Rollout
   // to the pdl_wait() below (barriers, constant tables, the producer's first weight copies) reads only the staged
   // model, which no kernel of a plan writes.
   pdl_trigger();
-  if (CEMF) pdl_wait();  // the fused-CEM variants stage the sampling distribution in their prologue
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < S; ++s) {
@@ -411,27 +273,11 @@ __device__ __forceinline__ void rollout_tc_body(const ModelDev& m, const Rollout
     c_norm[j] = (j < m.in && m.norm_mode) ? make_float2(m.norm_mean_f[j], m.norm_istd_f[j]) : make_float2(0.f, 1.f);
   // logvar clamp folded into two per-output constants (see the output-layer maths):
   //   var = exp(min + softplus(max - softplus(max - lv) - min)) = exp(min) * (1 + exp(max - min) / (1 + exp(max - lv)))
-  // [2][kCemTabDims]: sampling mean, sqrt(constrained variance): behind the weight ring, allocated for fused-CEM launches only
-  float* cem_tab = reinterpret_cast<float*>(smem + p.smem_bytes);
-  __shared__ int sh_tail[2];
   for (int j = threadIdx.x; j < outq; j += kThreads) {
     const bool real = j < m.out;
     const float mn = (m.deterministic || !real) ? 0.f : m.min_lv[j], mx = (m.deterministic || !real) ? 0.f : m.max_lv[j];
     const bool delta = real && j < m.D && m.target_is_delta && !m.no_delta[j];
     c_out[j] = make_float4(mx * 1.4426950408889634f, expf(mx - mn), expf(0.5f * mn), delta ? 1.f : 0.f);
-  }
-  const int cem_dims = a.H * m.A;
-  if (CEMF && a.cem_mu) {
-    for (int d = threadIdx.x; d < cem_dims; d += kThreads) {
-      const float mu = a.cem_mu[d], dp = a.cem_disp[d];
-      float sd = dp;
-      if (!a.cem_clipped) {  // trajectory_opt.py:122-125
-        const float l2 = (mu - a.cem_lb[d]) / 2.0f, u2 = (a.cem_ub[d] - mu) / 2.0f;
-        sd = sqrtf(fminf(fminf(l2 * l2, u2 * u2), dp));
-      }
-      cem_tab[d] = mu;
-      cem_tab[kCemTabDims + d] = sd;
-    }
   }
   __syncthreads();
 
@@ -485,8 +331,6 @@ __device__ __forceinline__ void rollout_tc_body(const ModelDev& m, const Rollout
     const int r = wt & 63, h = wt >> 6;  // row of the warpgroup, half of the row's work
     const int i = wg * 64 + r;           // CTA row
     const bool owner = h == 0;           // the row's scalar state: observation / actions load, score, store
-    const bool cem = CEMF && a.cem_mu != nullptr;
-    const bool sampler = cem && h == 1;  // the thread of this row that draws its sequence's actions
     uint8_t* abuf = smem + p.off_A + (size_t)wg * p.wg_bytes;
     const float* stg = reinterpret_cast<const float*>(abuf) + r * p.stg_ld;  // this row's output accumulators
     float* my_obs = obs_s + i * p.obs_ld;
@@ -547,19 +391,14 @@ __device__ __forceinline__ void rollout_tc_body(const ModelDev& m, const Rollout
       }
       float tot = 0.f;
       int dead = 0;
-      const float* act_row = cem ? nullptr : a.act + prob_off<BATCH>(bt, kp, &BatchArgs::act) + (rid / a.act_div) * a.act_row_stride;
-      const int seq_n = (int)(rid / a.P);
-      float* pop_row = (cem && a.pop_out && valid && rid % a.P == 0) ? a.pop_out + (size_t)seq_n * cem_dims : nullptr;  // in-kernel draw only
-      // this step's actions into the row's action words: from the action tensor, or drawn in-kernel (fused CEM)
+      const float* act_row = a.act + prob_off<BATCH>(bt, kp, &BatchArgs::act) + (rid / a.act_div) * a.act_row_stride;
+      // this step's actions from the action tensor into the row's action words
       auto load_actions = [&](int t) {
-        if (owner && !cem) {
+        if (owner) {
           const float* ap = act_row + (long long)t * a.act_t_stride;
 #pragma unroll 1
           for (int j = 0; j < m.A; ++j) my_act[j] = valid ? ap[j] : 0.f;
         }
-        if (CEMF && sampler)
-          cem_sample_actions(a.seed, a.cem_offset, a.cem_clipped, a.cem_lb, a.cem_ub, cem_tab, cem_tab + kCemTabDims, a.seq0 + seq_n,
-                             t, m.A, my_act, pop_row);
       };
       wg_bar(wg);  // previous tile fully consumed before its row state is overwritten
       if (owner) {
@@ -703,42 +542,21 @@ __device__ __forceinline__ void rollout_tc_body(const ModelDev& m, const Rollout
   }
 
   __syncthreads();
-  // ---- fused CEM iteration: the last CTA to get here refits the sampling distribution ----
-  if (CEMF && a.tail_counter) {
-    if (threadIdx.x == 0) {
-      __threadfence();
-      sh_tail[0] = atomicAdd(a.tail_counter, 1u) == gridDim.x - 1 ? 1 : 0;
-    }
-    __syncthreads();
-    if (sh_tail[0]) {
-      __threadfence();
-      TailArgs* ta = reinterpret_cast<TailArgs*>(ring);  // the weight ring is idle now: argument block + scratch
-      if (threadIdx.x == 0) {
-        ta->N = a.N; ta->P = a.P; ta->tail_elite_num = a.tail_elite_num; ta->cem_clipped = a.cem_clipped;
-        ta->tail_alpha = a.tail_alpha; ta->total_state = a.total_state; ta->pop_out = a.pop_out;
-        ta->tail_values = a.tail_values; ta->tail_mu = a.tail_mu; ta->tail_disp = a.tail_disp;
-        ta->tail_best_value = a.tail_best_value; ta->tail_best_solution = a.tail_best_solution;
-        ta->tail_counter = a.tail_counter;
-      }
-      __syncthreads();
-      cem_tail_refit(ta, cem_dims, ring + 256, &sh_tail[1]);
-    }
-  }
 }
 
-template <int ACT, bool CEMF, bool EXP = false, bool TRAJ = false, int NWG = 2>
+template <int ACT, bool EXP, bool TRAJ, int NWG>
 __global__ void __launch_bounds__(threads_of<NWG>(), NWG == 1 ? 2 : 1)
 rollout_tc_kernel(const __grid_constant__ ModelDev m, const __grid_constant__ RolloutArgs a, const __grid_constant__ TcPlan p,
                   const long long num_tiles) {
-  rollout_tc_body<ACT, CEMF, EXP, TRAJ, NWG, false>(m, a, p, num_tiles, nullptr);
+  rollout_tc_body<ACT, EXP, TRAJ, NWG, false>(m, a, p, num_tiles, nullptr);
 }
 
-// K independent evaluations in one launch (plain and "expectation"; no fused-CEM or trajectory variants)
+// K independent evaluations in one launch (plain and "expectation"; no trajectory variants)
 template <int ACT, bool EXP, int NWG>
 __global__ void __launch_bounds__(threads_of<NWG>(), NWG == 1 ? 2 : 1)
 rollout_tc_batch_kernel(const __grid_constant__ ModelDev m, const __grid_constant__ RolloutArgs a, const __grid_constant__ TcPlan p,
                         const long long num_tiles, const __grid_constant__ BatchArgs bt) {
-  rollout_tc_body<ACT, false, EXP, false, NWG, true>(m, a, p, num_tiles, &bt);
+  rollout_tc_body<ACT, EXP, false, NWG, true>(m, a, p, num_tiles, &bt);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -830,9 +648,9 @@ static int tc_device_limits() {  // cached per device (a process may drive sever
   CUDA_TRY(cudaDeviceGetAttribute(&sm_smem, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev));
   CUDA_TRY(cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev));
   // dynamic shared memory of a 64-row CTA that fits twice per SM: half the SM's, less the per-CTA reservation and the
-  // static shared memory of the variant that has the most (the fused-CEM one)
+  // static shared memory of the kernel (every 64-row variant, batched or not, has the same)
   cudaFuncAttributes fa;
-  CUDA_TRY(cudaFuncGetAttributes(&fa, rollout_tc_kernel<B200PETS_ACT_SILU, true, false, false, 1>));
+  CUDA_TRY(cudaFuncGetAttributes(&fa, rollout_tc_kernel<B200PETS_ACT_SILU, false, false, 1>));
   g_pair_smem = min(g_max_smem, sm_smem / 2 - reserved - (int)fa.sharedSizeBytes);
   g_limits_dev = dev;
   return B200PETS_OK;
@@ -840,7 +658,7 @@ static int tc_device_limits() {  // cached per device (a process may drive sever
 
 // smem plan for a model and CTA shape (nwg consumer warpgroups); returns false when the tensor-core path does not
 // cover the dimensions or the plan does not fit in max_smem
-static bool tc_make_plan(const ModelDev& m, int nwg, int max_smem, TcPlan* out, bool expectation, bool cem) {
+static bool tc_make_plan(const ModelDev& m, int nwg, int max_smem, TcPlan* out, bool expectation) {
   TcPlan p{};
   p.nwg = nwg;
   const uint32_t rows = 64u * (uint32_t)nwg;
@@ -874,20 +692,19 @@ static bool tc_make_plan(const ModelDev& m, int nwg, int max_smem, TcPlan* out, 
   p.off_bar = off; off += 2 * kMaxStages * 8;
   off = (off + 127u) & ~127u;
   p.off_ring = off;
-  const int cem_tab = cem ? 2 * kCemTabDims * (int)sizeof(float) : 0;
   // longest slices that still leave three slots (one in use, two in flight); wide models get shorter slices
   int S = 0;
   for (p.kslice = kSliceK16;; --p.kslice) {
     uint32_t slot = 0;
     for (int l = 0; l < p.nlayers; ++l) slot = max(slot, (uint32_t)min(m.Kp[l] >> 4, p.kslice) * m.Np[l] * 32u);
     p.slot_bytes = (slot + 127u) & ~127u;
-    S = ((int)max_smem - cem_tab - (int)off) / (int)p.slot_bytes;
+    S = ((int)max_smem - (int)off) / (int)p.slot_bytes;
     if (S >= 3 || p.kslice == 1) break;
   }
   if (S < 2) return false;
   p.nstages = min(S, kMaxStages);
-  p.smem_bytes = off + max((uint32_t)p.nstages * p.slot_bytes, cem ? kTailScratch : 0u);
-  if ((int)p.smem_bytes + cem_tab > max_smem) return false;
+  p.smem_bytes = off + (uint32_t)p.nstages * p.slot_bytes;
+  if ((int)p.smem_bytes > max_smem) return false;
   *out = p;
   return true;
 }
@@ -896,9 +713,9 @@ static bool tc_make_plan(const ModelDev& m, int nwg, int max_smem, TcPlan* out, 
 // half an SM's shared memory, so that every SM gets work.  Otherwise 128-row CTAs one per SM with the whole opt-in shared
 // memory: once every SM has a tile, two 64-row CTAs per SM measured slower than one 128-row CTA (they fetch the
 // weights twice).  Every model with a 64-row plan also has a 128-row one.  Call after tc_device_limits().
-static bool tc_choose_plan(const ModelDev& m, long long tiles, TcPlan* out, bool expectation = false, bool cem = false) {
-  if (tiles < g_sm_count && tc_make_plan(m, 1, g_pair_smem, out, expectation, cem)) return true;
-  return tc_make_plan(m, 2, g_max_smem, out, expectation, cem);
+static bool tc_choose_plan(const ModelDev& m, long long tiles, TcPlan* out, bool expectation = false) {
+  if (tiles < g_sm_count && tc_make_plan(m, 1, g_pair_smem, out, expectation)) return true;
+  return tc_make_plan(m, 2, g_max_smem, out, expectation);
 }
 
 bool tc_supported(const ModelDev& m) {
@@ -907,13 +724,13 @@ bool tc_supported(const ModelDev& m) {
   return tc_choose_plan(m, g_sm_count, &p);
 }
 
-// the plan launch_rollout_tc uses for an evaluation / step (no fused CEM iteration) with or without "expectation" that
+// the plan launch_rollout_tc uses for an evaluation / step with or without "expectation" that
 // has a 128-row tile for every SM (launches with fewer tiles may run 64-row CTAs, see tc_choose_plan)
 int tc_plan_info(const ModelDev& m, bool expectation, int* kslice, int* nstages, int* smem_bytes) {
   int rc = tc_device_limits();
   if (rc) return rc;
   TcPlan p;
-  const bool ok = tc_choose_plan(m, g_sm_count, &p, expectation, false);
+  const bool ok = tc_choose_plan(m, g_sm_count, &p, expectation);
   *kslice = ok ? p.kslice : 0;
   *nstages = ok ? p.nstages : 0;
   *smem_bytes = ok ? (int)p.smem_bytes : 0;
@@ -923,19 +740,18 @@ int tc_plan_info(const ModelDev& m, bool expectation, int* kslice, int* nstages,
 using TcKernel = void (*)(const ModelDev, const RolloutArgs, const TcPlan, const long long);
 using TcBatchKernel = void (*)(const ModelDev, const RolloutArgs, const TcPlan, const long long, const BatchArgs);
 
-// the variant of a launch: fused CEM iteration, "expectation", per-step trajectory stores (b200pets_eval_trajectory)
+// the variant of a launch: "expectation", per-step trajectory stores (b200pets_eval_trajectory)
 template <int ACT, int NWG>
-static TcKernel tc_variant(bool cemf, bool expect, bool traj) {
-  if (traj) return expect ? rollout_tc_kernel<ACT, false, true, true, NWG> : rollout_tc_kernel<ACT, false, false, true, NWG>;
-  if (expect) return rollout_tc_kernel<ACT, false, true, false, NWG>;
-  return cemf ? rollout_tc_kernel<ACT, true, false, false, NWG> : rollout_tc_kernel<ACT, false, false, false, NWG>;
+static TcKernel tc_variant(bool expect, bool traj) {
+  if (traj) return expect ? rollout_tc_kernel<ACT, true, true, NWG> : rollout_tc_kernel<ACT, false, true, NWG>;
+  return expect ? rollout_tc_kernel<ACT, true, false, NWG> : rollout_tc_kernel<ACT, false, false, NWG>;
 }
 
 template <int NWG>
-static TcKernel tc_kernel(int act, bool cemf, bool expect, bool traj) {
-  return act == B200PETS_ACT_SILU   ? tc_variant<B200PETS_ACT_SILU, NWG>(cemf, expect, traj)
-         : act == B200PETS_ACT_RELU ? tc_variant<B200PETS_ACT_RELU, NWG>(cemf, expect, traj)
-                                    : tc_variant<B200PETS_ACT_LEAKY_RELU, NWG>(cemf, expect, traj);
+static TcKernel tc_kernel(int act, bool expect, bool traj) {
+  return act == B200PETS_ACT_SILU   ? tc_variant<B200PETS_ACT_SILU, NWG>(expect, traj)
+         : act == B200PETS_ACT_RELU ? tc_variant<B200PETS_ACT_RELU, NWG>(expect, traj)
+                                    : tc_variant<B200PETS_ACT_LEAKY_RELU, NWG>(expect, traj);
 }
 
 // 128-row tiles of one launch
@@ -959,13 +775,13 @@ static TcBatchKernel tc_batch_kernel(int act, bool expect) {
 int launch_rollout_tc_batch(const ModelDev& m, const RolloutArgs& a, int num_problems, BatchArgs bt, cudaStream_t stream) {
   int rc = tc_device_limits();
   if (rc) return rc;
-  if (a.cem_mu || a.tail_counter || a.traj_obs || a.traj_reward || a.traj_done || a.reward_out || a.done_out)
+  if (a.traj_obs || a.traj_reward || a.traj_done || a.reward_out || a.done_out)
     return b200pets_set_error(B200PETS_EUNSUPPORTED, "batched rollout: evaluation outputs only");
   const bool expect = a.propagation == B200PETS_PROP_EXPECTATION;
   bt.tiles = tc_launch_tiles(m, a);
   const long long tiles = bt.tiles * num_problems;
   TcPlan p;
-  if (!tc_choose_plan(m, tiles, &p, expect, false))
+  if (!tc_choose_plan(m, tiles, &p, expect))
     return b200pets_set_error(B200PETS_EUNSUPPORTED, "model dimensions outside the tensor-core path (in %d hid %d out %d)",
                               m.in, m.hid, m.out);
   const TcBatchKernel kern = p.nwg == 1 ? tc_batch_kernel<1>(m.act, expect) : tc_batch_kernel<2>(m.act, expect);
@@ -981,23 +797,19 @@ int launch_rollout_tc(const ModelDev& m, const RolloutArgs& a, cudaStream_t stre
   int rc = tc_device_limits();
   if (rc) return rc;
   const bool expect = a.propagation == B200PETS_PROP_EXPECTATION;
-  const bool cemf = a.cem_mu != nullptr || a.tail_counter != nullptr;
   const bool traj = a.traj_obs || a.traj_reward || a.traj_done;
-  if (expect && cemf) return b200pets_set_error(B200PETS_EUNSUPPORTED, "fused CEM iteration does not cover propagation='expectation'");
-  if (traj && cemf) return b200pets_set_error(B200PETS_EUNSUPPORTED, "fused CEM iteration has no trajectory outputs");
   const long long tiles = tc_launch_tiles(m, a);  // 128-row tiles
   TcPlan p;
-  if (!tc_choose_plan(m, tiles, &p, expect, cemf))
+  if (!tc_choose_plan(m, tiles, &p, expect))
     return b200pets_set_error(B200PETS_EUNSUPPORTED, "model dimensions outside the tensor-core path (in %d hid %d out %d)",
                               m.in, m.hid, m.out);
-  const TcKernel kern = p.nwg == 1 ? tc_kernel<1>(m.act, cemf, expect, traj) : tc_kernel<2>(m.act, cemf, expect, traj);
+  const TcKernel kern = p.nwg == 1 ? tc_kernel<1>(m.act, expect, traj) : tc_kernel<2>(m.act, expect, traj);
   const int threads = p.nwg == 1 ? threads_of<1>() : threads_of<2>();
   const long long cta_tiles = tiles * (2 / p.nwg);
-  const size_t smem_launch = (size_t)p.smem_bytes + (cemf ? (size_t)2 * kCemTabDims * sizeof(float) : 0);
-  CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_launch));
+  CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem_bytes));
   // 64-row CTAs: fewer than two per SM, all resident (registers: tests/test_sass_occupancy.py; shared memory: the plan)
   const unsigned grid = (unsigned)min((long long)g_sm_count * (2 / p.nwg), cta_tiles);
-  CUDA_TRY(launch_pdl(kern, dim3(grid), dim3(threads), smem_launch, stream, m, a, p, cta_tiles));
+  CUDA_TRY(launch_pdl(kern, dim3(grid), dim3(threads), (size_t)p.smem_bytes, stream, m, a, p, cta_tiles));
   return B200PETS_OK;
 }
 

@@ -5,12 +5,10 @@ its plan fits twice in an SM's shared memory: CTA tile u is half u % 2 of 128-ro
 member's slot range or an expectation chunk is split over two CTAs that each walk the weights on their own.  Other
 launches run 128-row CTAs, one per SM.  A row's member, keys, operands and K order are the same in both shapes, so
 results do not depend on the shape.  Here: halves with no valid row at shard edges (bit for bit against the unsharded
-evaluation), a launch of one 128-row tile, the 128-row CTA with more tiles than SMs, and the fused CEM iteration
-(in-kernel sampling and the last-CTA refit) on 64-row CTAs.  Small launches of models whose plan fits only once per SM
+evaluation), a launch of one 128-row tile, and the 128-row CTA with more tiles than SMs.  Small launches of models whose plan fits only once per SM
 (plan_ring2, plan_k1_out256) run in the tile-shuffle and parity tests.
 """
 import dataclasses
-import os
 
 import numpy as np
 import pytest
@@ -77,37 +75,3 @@ def test_one_per_sm_multi_tile_launch_matches_oracle():
         torch.from_numpy(inp["actions"]), inp["obs0"], spec.particles, torch.from_numpy(inp["perms"]),
         torch.from_numpy(inp["eps"])).numpy()
     assert_close_continuous(got, ref, 5e-3)
-
-
-def test_fused_iteration_on_64_row_ctas_equals_multi_kernel_plan():
-    """The fused CEM iteration with and without in-kernel sampling on 64-row CTAs (600 sequences x 20 particles: 100
-    tiles of 128 rows, 200 CTAs), against the sample -> rollout -> refit kernel sequence at the bars of
-    test_fused_iteration_kernel_equals_multi_kernel_plan."""
-    import mbrl_lib_b200 as bp
-    from mbrl_lib_b200.planning import _FusedObjective
-
-    spec = dataclasses.replace(syn.CASES["halfcheetah"], population=600, horizon=8)
-    assert _tc_tiles(spec, "tile_shuffle") < _sm_count()
-    H, A = spec.horizon, spec.act_dim
-    lb, ub = np.full((H, A), spec.action_lb).tolist(), np.full((H, A), spec.action_ub).tolist()
-    inp = syn.make_rollout_inputs(spec, with_noise=False)
-    out = {}
-    try:
-        for fused in ("1", "0", "sik"):
-            os.environ["B200PETS_CEM_FUSED"] = "0" if fused == "0" else "1"
-            os.environ["B200PETS_CEM_SAMPLE_IN_KERNEL"] = "1" if fused == "sik" else "0"
-            _, _, env = make_env("halfcheetah", "bf16_tc", ts1="tile_shuffle")
-            opt = bp.CEMOptimizer(3, 0.1, spec.population, lb, ub, 0.1, DEV, return_mean_elites=True)
-            opt.record_values = True
-            sol = opt.optimize(_FusedObjective(env, inp["obs0"], spec.particles), x0=torch.zeros(H, A, device=DEV))
-            torch.cuda.synchronize()
-            out[fused] = (sol.cpu().numpy(), opt.last_values.cpu().numpy())
-    finally:
-        os.environ.pop("B200PETS_CEM_FUSED", None)
-        os.environ.pop("B200PETS_CEM_SAMPLE_IN_KERNEL", None)
-    assert np.array_equal(out["sik"][1][0], out["0"][1][0])
-    np.testing.assert_allclose(out["sik"][0], out["0"][0], rtol=0, atol=1e-4)
-    assert np.array_equal(out["1"][1][0], out["0"][1][0])
-    np.testing.assert_allclose(out["1"][1], out["0"][1], rtol=0, atol=5e-3)
-    np.testing.assert_allclose(out["1"][0], out["0"][0], rtol=0, atol=1e-4)
-    assert np.isfinite(out["1"][0]).all()

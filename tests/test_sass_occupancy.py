@@ -16,7 +16,7 @@ CUOBJDUMP = shutil.which("cuobjdump") or os.path.join(os.path.dirname(NVCC), "cu
 
 
 def _resources():
-    """{kernel name: (registers, stack bytes)} of the library as build.py builds it."""
+    """{kernel name: (registers, stack bytes, static shared memory bytes)} of the library as build.py builds it."""
     if not (os.path.exists(NVCC) and os.path.exists(CUOBJDUMP)):
         pytest.skip("needs nvcc and cuobjdump")
     spec = importlib.util.spec_from_file_location("b200pets_build_occ", os.path.join(ROOT, "mbrl-lib_b200", "build.py"))
@@ -30,20 +30,24 @@ def _resources():
         if m:
             name = m.group(1)
             continue
-        m = re.search(r"REG:(\d+) STACK:(\d+)", line)
+        m = re.search(r"REG:(\d+) STACK:(\d+) SHARED:(\d+)", line)
         if m and name:
-            res[name] = (int(m.group(1)), int(m.group(2)))
+            res[name] = tuple(int(g) for g in m.groups())
             name = None
     return res
 
 
-def test_64_row_cta_fits_twice_per_sm():
+def test_64_row_variants_fit_twice_per_sm():
     res = _resources()
     # trailing template argument NWG = 1 (rollout_tc.cu): the 64-row, 160-thread variants
     small = {n: r for n, r in res.items() if "rollout_tc_kernel" in n and re.search(r"ELi1EEEv", n)}
-    assert len(small) == 15, sorted(small)  # 3 activations x (plain, fused CEM, expectation, 2 trajectory variants)
+    assert len(small) == 12, sorted(small)  # 3 activations x (plain, expectation, 2 trajectory variants)
+    # the launcher budgets every 64-row launch, batched or not, with the plain SiLU kernel's static shared memory
+    batch = {n: r for n, r in res.items() if "rollout_tc_batch_kernel" in n and re.search(r"ELi1EEEv", n)}
+    assert len(batch) == 6, sorted(batch)  # 3 activations x (plain, expectation)
+    assert len({r[2] for r in (*small.values(), *batch.values())}) == 1, {n: r[2] for n, r in {**small, **batch}.items()}
     warps = 2 * 160 // 32
-    for name, (regs, stack) in small.items():
+    for name, (regs, stack, _) in small.items():
         per_warp = -(-regs * 32 // 256) * 256
         assert warps * per_warp <= 65536, f"{name}: {regs} registers leave room for one 160-thread CTA per SM"
         assert stack <= 112, f"{name}: {stack} B stack frame"
