@@ -371,6 +371,35 @@ int b200pets_cem_plan_batch(b200pets_model_t model, const b200pets_rollout_cfg* 
                             float* solution, float* values_out, void* workspace, size_t workspace_bytes,
                             void* stream);
 
+/* K MPPIOptimizer.optimize calls over ModelEnv.evaluate_action_sequences (trajectory_opt.py:239-311), one per
+ * observation, each from its own carried mean.  The plan first shifts every problem's mean (mean[:-1] = mean[1:], past
+ * action = the shifted mean[0]), then runs per refinement four launches for the whole batch: sample, rollout, particle
+ * mean, update.  Problem k gives, bit for bit, the k-th of K consecutive single plans:
+ *   population noise of refinement r: Philox key sample_seed (the optimiser's seed), offset
+ *     (sample_counter + k) * 1024 + r;
+ *   rollout of refinement r: key rcfg->seed (the environment's), offset (rcfg->offset + k * R + r) * 1024, R =
+ *     num_iterations.  A batch therefore takes K optimiser and K * R environment counter values.
+ * Arrays (problem k's slice is the array its single call takes; lower / upper are shared):
+ *   obs0 [dev] float[K][D]; mean [dev] float[K][H][A]: the carried means in, the plans out;
+ *   lower / upper [dev] float[H][A]; z [dev] float[K][R][N][H][A] or NULL (Philox);
+ *   eps [dev] float[K][R][H][B][out] or NULL; perms [dev] int64[K][R][H or 1][B] or NULL (tile shuffle);
+ *   values_out [dev] float[K][R][N] (after the NaN rule) or NULL.
+ * num_iterations 0 returns the shifted means.  Refused: num_problems < 1, a sharded rcfg (first_sequence != 0 or
+ * global_population other than 0 / population), external reward / termination callables, a negative num_iterations,
+ * NULL obs0 / mean / lower / upper / workspace, a workspace smaller than b200pets_mppi_plan_batch_workspace_bytes. */
+typedef struct {
+  int32_t num_iterations; /* refinements R (0: the shift alone, as the single path does) */
+  float gamma, beta;
+  uint64_t sample_seed;    /* Philox key of the population noise: the optimiser's seed, not the environment's */
+  uint64_t sample_counter; /* problem k, refinement r draws with offset (sample_counter + k) * 1024 + r */
+} b200pets_mppi_cfg;
+size_t b200pets_mppi_plan_batch_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* rcfg,
+                                                const b200pets_mppi_cfg* mcfg, int32_t num_problems);
+int b200pets_mppi_plan_batch(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_mppi_cfg* mcfg,
+                             int32_t num_problems, const float* obs0, float* mean, const float* lower,
+                             const float* upper, const float* z, const float* eps, const int64_t* perms,
+                             float* values_out, void* workspace, size_t workspace_bytes, void* stream);
+
 /* Self test of the wgmma building block: D[128][n] = A[128][k] * B[n][k]^T with bf16 operands staged in the
  * no-swizzle canonical layouts, the weight ring and the accumulator fragments the rollout kernel uses.  a, b [dev] float
  * (rounded to bf16 inside), d [dev] float[128][n].  k, n multiples of 16, <= 256.  A negative k writes A as bf16 pairs

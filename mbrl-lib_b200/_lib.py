@@ -41,6 +41,11 @@ class CemCfg(C.Structure):
                 ("return_mean_elites", C.c_int32), ("clipped_normal", C.c_int32)]
 
 
+class MppiCfg(C.Structure):
+    _fields_ = [("num_iterations", C.c_int32), ("gamma", C.c_float), ("beta", C.c_float), ("sample_seed", C.c_uint64),
+                ("sample_counter", C.c_uint64)]
+
+
 _P = C.c_void_p
 _SIGNATURES = {
     "b200pets_version": (C.c_int, []),
@@ -95,6 +100,9 @@ _SIGNATURES = {
     "b200pets_cem_plan_batch_workspace_bytes": (C.c_size_t, [_P, C.POINTER(RolloutCfg), C.POINTER(CemCfg), C.c_int32]),
     "b200pets_cem_plan_batch": (C.c_int, [_P, C.POINTER(RolloutCfg), C.POINTER(CemCfg), C.c_int32, _P, _P, _P, _P, _P, _P, _P,
                                           _P, _P, _P, C.c_size_t, _P]),
+    "b200pets_mppi_plan_batch_workspace_bytes": (C.c_size_t, [_P, C.POINTER(RolloutCfg), C.POINTER(MppiCfg), C.c_int32]),
+    "b200pets_mppi_plan_batch": (C.c_int, [_P, C.POINTER(RolloutCfg), C.POINTER(MppiCfg), C.c_int32, _P, _P, _P, _P, _P, _P, _P,
+                                           _P, _P, C.c_size_t, _P]),
     "b200pets_peer_buffer_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "b200pets_peer_alloc": (C.c_int, [C.c_size_t, C.POINTER(C.c_void_p), C.c_char_p]),
     "b200pets_peer_open": (C.c_int, [C.c_char_p, C.POINTER(C.c_void_p)]),

@@ -33,6 +33,12 @@ int launch_cem_update_rows(int population, int dims, int elite_num, float alpha,
                            const float* population_in, const float* row_totals, int particles, float* values, float* mu,
                            float* dispersion, float* best_value, float* best_solution, void* workspace,
                            size_t workspace_bytes, void* stream);
+int launch_mppi_sample_batch(int num_problems, int population, int horizon, int act_dim, float beta, const float* mean,
+                             const float* past, const float* lower, const float* upper, const float* z, long long z_stride,
+                             unsigned long long seed, unsigned long long offset, unsigned long long offset_step, float* pop,
+                             cudaStream_t stream);
+int launch_mppi_update_batch(int num_problems, int population, int dims, float gamma, const float* pop, float* values,
+                             float* mean_out, float* workspace, long long ws_stride_floats, cudaStream_t stream);
 bool tc_supported(const ModelDev& m);
 
 // ---------------------------------------------------------------------------------------------------------
@@ -681,11 +687,11 @@ size_t b200pets_eval_batch_workspace_bytes(b200pets_model_t model, const b200pet
 }
 
 // The rollouts of K evaluations in batched launches: problem k starts from obs0 + k * D, reads actions + k * act_stride,
-// perms + k * perm_stride, eps + k * eps_stride and draws with Philox offset cfg->offset + k * 1024.  Per-row totals
-// land in `total` [K][B].
+// perms + k * perm_stride, eps + k * eps_stride and draws with Philox offset cfg->offset + k * offset_step.  Per-row
+// totals land in `total` [K][B].
 static int eval_rows_batch(b200pets_model_t model, const b200pets_rollout_cfg* cfg, int K, const float* obs0, const float* actions,
                            long long act_stride, const int64_t* perms, long long perm_stride, const float* eps, long long eps_stride,
-                           float* total, void* workspace, cudaStream_t stream) {
+                           float* total, void* workspace, cudaStream_t stream, unsigned long long offset_step) {
   const b200pets_model_desc& d = model->desc;
   const size_t B = (size_t)cfg->population * cfg->particles, KB = (size_t)K * B;
   unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
@@ -699,7 +705,7 @@ static int eval_rows_batch(b200pets_model_t model, const b200pets_rollout_cfg* c
   bt.perm = perm_stride;
   bt.eps = eps_stride;
   bt.seed = cfg->seed;
-  bt.offset_step = 1024;
+  bt.offset_step = offset_step;
   return rollout_steps(model, cfg, 0, cfg->horizon, false, obs0, actions, perms, eps, obs_state, total, dead, nullptr, nullptr,
                        nullptr, stream, K, &bt);
 }
@@ -720,7 +726,7 @@ int b200pets_eval_sequences_batch(b200pets_model_t model, const b200pets_rollout
                              : reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(workspace) + al256(KB * d.obs_dim * sizeof(float)));
   cudaStream_t stream = (cudaStream_t)stream_;
   int rc = eval_rows_batch(model, cfg, num_problems, obs0, actions, (long long)N * H * d.act_dim, perms, (long long)nperm * B, eps,
-                           (long long)H * B * d.out_size, total, workspace, stream);
+                           (long long)H * B * d.out_size, total, workspace, stream, 1024);
   if (rc) return rc;
   // problem k's totals are rows k * B .. k * B + B - 1: one particle mean over K * N sequences
   return launch_particle_mean(num_problems * N, cfg->particles, total, returns, stream);  // model_env.py:190-191
@@ -833,7 +839,7 @@ int b200pets_cem_plan_batch(b200pets_model_t model, const b200pets_rollout_cfg* 
     rc_it.offset = rcfg->offset * 1024 + it;
     int rc = eval_rows_batch(model, &rc_it, K, obs0, pop, popk, perms ? perms + (size_t)it * nperm * B : nullptr,
                              (long long)iters * nperm * B, eps ? eps + (size_t)it * H * B * d.out_size : nullptr,
-                             (long long)iters * H * B * d.out_size, totals, eval_ws, stream);
+                             (long long)iters * H * B * d.out_size, totals, eval_ws, stream, 1024);
     if (rc) return rc;
     if (merged) {
       rc = next_pop(it + 1, 1);
@@ -853,6 +859,102 @@ int b200pets_cem_plan_batch(b200pets_model_t model, const b200pets_rollout_cfg* 
   }
   CUDA_TRY(cudaMemcpyAsync(solution, ccfg->return_mean_elites ? mu : best_sol, sizeof(float) * K * dims, cudaMemcpyDeviceToDevice,
                            stream));
+  return B200PETS_OK;
+}
+
+namespace {
+// the start of MPPIOptimizer.optimize for each problem (trajectory_opt.py:257-258): mean[:-1] = mean[1:] in place, and the
+// past action is the shifted mean[0].  One thread per (problem, action dim) walks its column forward.
+__global__ void mppi_shift_batch_kernel(int K, int H, int A, float* __restrict__ mean, float* __restrict__ past) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (long long)K * A) return;
+  const long long k = idx / A;
+  const int a = (int)(idx % A);
+  float* m = mean + k * H * A;
+  for (int t = 0; t + 1 < H; ++t) m[(size_t)t * A + a] = m[(size_t)(t + 1) * A + a];
+  past[idx] = m[a];
+}
+
+// the workspace of a batched MPPI plan: per-problem arrays side by side, [K][...] each
+struct MppiBatchLayout {
+  size_t pop, values, past, upd, eval, total;
+  long long upd_floats;  // one problem's update workspace (weights [N], per-warp partial sums [32][H*A])
+};
+MppiBatchLayout mppi_batch_layout(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, int K) {
+  const size_t N = rcfg->population, A = model->desc.act_dim, dims = (size_t)rcfg->horizon * A;
+  MppiBatchLayout l{};
+  l.upd_floats = (long long)(N + 32 * dims);
+  size_t off = 0;
+  l.pop = off; off += al256(K * N * dims * 4);
+  l.values = off; off += al256(K * N * 4);
+  l.past = off; off += al256(K * A * 4);
+  l.upd = off; off += al256(K * (size_t)l.upd_floats * 4);
+  l.eval = off; off += al256(b200pets_eval_batch_workspace_bytes(model, rcfg, K));
+  l.total = off;
+  return l;
+}
+}  // namespace
+
+size_t b200pets_mppi_plan_batch_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_mppi_cfg* mcfg,
+                                                int32_t num_problems) {
+  if (!model || !rcfg || !mcfg || num_problems < 1) return 0;
+  return mppi_batch_layout(model, rcfg, num_problems).total;
+}
+
+int b200pets_mppi_plan_batch(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_mppi_cfg* mcfg,
+                             int32_t num_problems, const float* obs0, float* mean, const float* lower, const float* upper,
+                             const float* z, const float* eps, const int64_t* perms, float* values_out, void* workspace,
+                             size_t workspace_bytes, void* stream_) {
+  if (!model || !rcfg || !mcfg) return b200pets_set_error(B200PETS_EINVAL, "mppi_plan_batch: null argument");
+  { int rc = check_batch(model, rcfg, num_problems, "mppi_plan_batch"); if (rc) return rc; }
+  if (!obs0 || !mean || !lower || !upper || !workspace) return b200pets_set_error(B200PETS_EINVAL, "mppi_plan_batch: null argument");
+  if (mcfg->num_iterations < 0)
+    return b200pets_set_error(B200PETS_EINVAL, "mppi_plan_batch: num_iterations must not be negative (got %d)", mcfg->num_iterations);
+  const int K = num_problems;
+  if (workspace_bytes < b200pets_mppi_plan_batch_workspace_bytes(model, rcfg, mcfg, K))
+    return b200pets_set_error(B200PETS_EINVAL, "mppi_plan_batch: workspace too small");
+  cudaStream_t stream = (cudaStream_t)stream_;
+  const b200pets_model_desc& d = model->desc;
+  const int N = rcfg->population, H = rcfg->horizon, P = rcfg->particles, A = d.act_dim, R = mcfg->num_iterations;
+  const int dims = H * A;
+  const long long B = (long long)N * P;
+  const MppiBatchLayout l = mppi_batch_layout(model, rcfg, K);
+  unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
+  float* pop = reinterpret_cast<float*>(ws + l.pop);
+  float* values = reinterpret_cast<float*>(ws + l.values);
+  float* past = reinterpret_cast<float*>(ws + l.past);
+  float* upd_ws = reinterpret_cast<float*>(ws + l.upd);
+  void* eval_ws = ws + l.eval;
+  float* totals = reinterpret_cast<float*>(ws + l.eval + al256((size_t)K * B * d.obs_dim * sizeof(float)));
+  const long long popk = (long long)N * dims;  // per-problem strides
+  const int nperm = rcfg->propagation == B200PETS_PROP_FIXED_MODEL ? 1 : H;
+
+  const long long tot = (long long)K * A;
+  mppi_shift_batch_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, stream>>>(K, H, A, mean, past);
+  CUDA_TRY(cudaGetLastError());
+  // per refinement, for the whole batch: sample, rollout, particle mean, update.  Problem k's refinement r draws its
+  // population with offset (sample_counter + k) * 1024 + r and rolls out with (offset + k * R + r) * 1024: the values
+  // the k-th of K consecutive single plans takes.
+  for (int r = 0; r < R; ++r) {
+    int rc = launch_mppi_sample_batch(K, N, H, A, mcfg->beta, mean, past, lower, upper, z ? z + (size_t)r * popk : nullptr,
+                                      (long long)R * popk, mcfg->sample_seed, mcfg->sample_counter * 1024 + (unsigned long long)r,
+                                      1024, pop, stream);
+    if (rc) return rc;
+    b200pets_rollout_cfg rc_r = *rcfg;
+    rc_r.offset = (rcfg->offset + (unsigned long long)r) * 1024;
+    rc = eval_rows_batch(model, &rc_r, K, obs0, pop, popk, perms ? perms + (size_t)r * nperm * B : nullptr, (long long)R * nperm * B,
+                         eps ? eps + (size_t)r * H * B * d.out_size : nullptr, (long long)R * H * B * d.out_size, totals, eval_ws,
+                         stream, (unsigned long long)R * 1024);
+    if (rc) return rc;
+    rc = launch_particle_mean(K * N, P, totals, values, stream);  // model_env.py:190-191
+    if (rc) return rc;
+    rc = launch_mppi_update_batch(K, N, dims, mcfg->gamma, pop, values, mean, upd_ws, l.upd_floats, stream);
+    if (rc) return rc;
+    // NB: values_out then holds the values AFTER the reference's in-place NaN rule (trajectory_opt.py:297)
+    if (values_out)  // problem k's values of refinement r -> values_out[k][r]
+      CUDA_TRY(cudaMemcpy2DAsync(values_out + (size_t)r * N, sizeof(float) * R * N, values, sizeof(float) * N, sizeof(float) * N, K,
+                                 cudaMemcpyDeviceToDevice, stream));
+  }
   return B200PETS_OK;
 }
 

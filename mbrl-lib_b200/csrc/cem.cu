@@ -638,12 +638,22 @@ cem_refit_sample_batch_kernel(const SelArgs s0, const float* __restrict__ row_to
 // ------------------------------------------------------------------------------------------------------
 // beta-smoothed noisy actions, sequential over the horizon (trajectory_opt.py:262-287): one thread per (n, action dim).
 // NB the reference overwrites the variance-scaled population with mean + *unscaled* truncated noise; restated as is.
+// blockIdx.y is the problem k of a batch: it reads mean + k*H*A, past + k*A and z + k*z_stride, writes pop + k*n*H*A and
+// draws with offset + k*offset_step, keyed from the unkeyed seed (b200pets_mppi_sample launches one problem).
 __global__ void mppi_sample_kernel(int n, int H, int A, float beta, const float* __restrict__ mean,
                                    const float* __restrict__ past, const float* __restrict__ lb,
-                                   const float* __restrict__ ub, const float* __restrict__ z, unsigned long long seed,
-                                   unsigned long long offset, float* __restrict__ pop) {
+                                   const float* __restrict__ ub, const float* __restrict__ z, long long z_stride,
+                                   unsigned long long seed, unsigned long long offset, unsigned long long offset_step,
+                                   float* __restrict__ pop) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= (long long)n * A) return;
+  const long long k = blockIdx.y;
+  offset += (unsigned long long)k * offset_step;
+  seed = rng_key(seed, offset);
+  mean += k * H * A;
+  past += k * A;
+  pop += k * n * H * A;
+  if (z) z += k * z_stride;
   const int ni = (int)(idx / A), ad = (int)(idx % A);
   float prev = past[ad];
   for (int t = 0; t < H; ++t) {
@@ -670,13 +680,21 @@ __global__ void mppi_sample_kernel(int n, int H, int A, float beta, const float*
   }
 }
 
-// softmax-weighted mean of the population (trajectory_opt.py:296-309): one CTA
+// softmax-weighted mean of the population (trajectory_opt.py:296-309): one CTA per problem.  CTA k of a batch reads
+// pop + k*n*dims and values + k*n, writes mean_out + k*dims and uses the workspace ws + k*ws_stride (weights [n], then
+// per-warp partial sums [32][dims]); the reduction order does not depend on k.
 __global__ void __launch_bounds__(kSelThreads, 1)
 mppi_update_kernel(int n, int dims, float gamma, const float* __restrict__ pop, float* __restrict__ values,
-                   float* __restrict__ mean_out, float* __restrict__ wts, float* __restrict__ partial) {
+                   float* __restrict__ mean_out, float* __restrict__ ws, long long ws_stride) {
   __shared__ float red[32];
   __shared__ float sh_max, sh_norm;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const long long k = blockIdx.x;
+  pop += k * n * dims;
+  values += k * n;
+  mean_out += k * dims;
+  float* __restrict__ wts = ws + k * ws_stride;
+  float* __restrict__ partial = wts + n;
   float vmax = -INFINITY;
   for (int i = tid; i < n; i += kSelThreads) {
     float v = values[i];
@@ -1171,7 +1189,7 @@ int b200pets_mppi_sample(int32_t population, int32_t horizon, int32_t act_dim, f
   if (population <= 0 || horizon <= 0 || act_dim <= 0) return b200pets_set_error(B200PETS_EINVAL, "mppi_sample: empty population");
   long long tot = (long long)population * act_dim;
   mppi_sample_kernel<<<(unsigned)((tot + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
-      population, horizon, act_dim, beta, mean, past_action, lower, upper, z, rng_key(seed, offset), offset, population_out);
+      population, horizon, act_dim, beta, mean, past_action, lower, upper, z, 0, seed, offset, 0, population_out);
   CUDA_TRY(cudaGetLastError());
   return B200PETS_OK;
 }
@@ -1185,9 +1203,8 @@ int b200pets_mppi_update(int32_t population, int32_t dims, float gamma, const fl
   if (population <= 0 || dims <= 0) return b200pets_set_error(B200PETS_EINVAL, "mppi_update: empty population");
   if (workspace_bytes < b200pets_mppi_update_workspace_bytes(population, dims))
     return b200pets_set_error(B200PETS_EINVAL, "mppi_update: workspace too small");
-  float* wts = reinterpret_cast<float*>(workspace);
   mppi_update_kernel<<<1, kSelThreads, 0, (cudaStream_t)stream>>>(population, dims, gamma, population_in, values, mean_out,
-                                                                  wts, wts + population);
+                                                                  reinterpret_cast<float*>(workspace), 0);
   CUDA_TRY(cudaGetLastError());
   return B200PETS_OK;
 }
@@ -1282,6 +1299,28 @@ int launch_cem_refit_sample_batch(int num_problems, int population, int dims, in
   CUDA_TRY(cudaFuncSetAttribute(cem_refit_sample_batch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 150 * 1024));
   CUDA_TRY(launch_pdl(cem_refit_sample_batch_kernel, dim3((unsigned)num_problems * G), dim3(kSelThreads), esm, (cudaStream_t)stream, s,
                       row_totals, particles, q, rb));
+  return B200PETS_OK;
+}
+
+// internal (api.cu, batched MPPI plan): b200pets_mppi_sample for `num_problems` problems (see mppi_sample_kernel); seed is
+// the unkeyed seed
+int launch_mppi_sample_batch(int num_problems, int population, int horizon, int act_dim, float beta, const float* mean,
+                             const float* past, const float* lower, const float* upper, const float* z, long long z_stride,
+                             unsigned long long seed, unsigned long long offset, unsigned long long offset_step, float* pop,
+                             cudaStream_t stream) {
+  const long long tot = (long long)population * act_dim;
+  mppi_sample_kernel<<<dim3((unsigned)((tot + 127) / 128), (unsigned)num_problems), 128, 0, stream>>>(
+      population, horizon, act_dim, beta, mean, past, lower, upper, z, z_stride, seed, offset, offset_step, pop);
+  CUDA_TRY(cudaGetLastError());
+  return B200PETS_OK;
+}
+
+// b200pets_mppi_update for `num_problems` problems, one CTA each; ws_stride_floats >= population + 32 * dims
+int launch_mppi_update_batch(int num_problems, int population, int dims, float gamma, const float* pop, float* values,
+                             float* mean_out, float* workspace, long long ws_stride_floats, cudaStream_t stream) {
+  mppi_update_kernel<<<(unsigned)num_problems, kSelThreads, 0, stream>>>(population, dims, gamma, pop, values, mean_out, workspace,
+                                                                        ws_stride_floats);
+  CUDA_TRY(cudaGetLastError());
   return B200PETS_OK;
 }
 

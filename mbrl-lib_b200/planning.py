@@ -55,11 +55,11 @@ class Optimizer(_RefOptimizer):  # mbrl/planning/trajectory_opt.py:21-40
         raise NotImplementedError
 
     def optimize_batch(self, obj_funs, x0=None, callback=None, **kwargs):
-        """One plan per objective of ``obj_funs`` from the warm starts ``x0 [K, H, A]``.  Only CEMOptimizer keeps no state
-        between calls besides the warm start; an optimiser that does (iCEM's kept elites, MPPI's mean) would have to split
-        it per problem, which is not implemented."""
+        """One plan per objective of ``obj_funs`` from the warm starts ``x0 [K, H, A]``.  CEMOptimizer keeps no state
+        between calls besides the warm start, and MPPIOptimizer keeps one mean per problem; an optimiser with other state
+        (iCEM's kept elites) would have to split it per problem, which is not implemented."""
         raise NotImplementedError(f"{type(self).__name__} does not plan for a batch of observations; "
-                                  "CEMOptimizer is the optimiser that supports act_batch")
+                                  "CEMOptimizer and MPPIOptimizer are the optimisers that support act_batch")
 
 
 class _FusedObjective:
@@ -384,6 +384,10 @@ class MPPIOptimizer(Optimizer):
         self.refinements = num_iterations
         self.lib = _lib.load()
         self._seed = int(torch.initial_seed()) & 0xFFFFFFFFFFFFFFFF
+        self.batch_mean: Optional[torch.Tensor] = None  # [K, H, A] carried means of optimize_batch
+        self._plan_batch_ws = None
+        self.record_values = False
+        self.last_values = None
 
     def optimize(self, obj_fun, x0: Optional[torch.Tensor] = None, callback=None, *, _noise=None, **kwargs) -> torch.Tensor:
         H, A, N = self.planning_horizon, self.action_dimension, self.population_size
@@ -411,6 +415,78 @@ class MPPIOptimizer(Optimizer):
                     callback(pop, values, k)
                 self.mean = new_mean
         return self.mean.clone()
+
+    def optimize_batch(self, obj_funs, x0: Optional[torch.Tensor] = None, callback=None, *, _noise=None, _model_noise=None,
+                       **kwargs) -> torch.Tensor:
+        """K independent plans, one per objective of ``obj_funs`` (a :class:`_FusedBatchObjective` or a list of K
+        objectives); returns ``[K, H, A]``.  Problem k plans as :meth:`optimize` would from its own carried mean
+        ``batch_mean[k]``.  The batch's means start at zeros, as ``mean`` does, and are re-created when K changes;
+        :meth:`optimize` / ``mean`` and the batch never touch each other's state.  ``x0`` is ignored, as in
+        :meth:`optimize`.  The model's objective with no callback and no reward / termination callable runs as one
+        device-resident plan (``b200pets_mppi_plan_batch``) in which problem k takes the counter values of the k-th of K
+        consecutive single plans; anything else runs :meth:`optimize` once per entry, in order.  With ``record_values``
+        the batched plan leaves every refinement's values in ``last_values [K, R, N]``."""
+        K = len(obj_funs.obs) if isinstance(obj_funs, _FusedBatchObjective) else len(obj_funs)
+        H, A = self.planning_horizon, self.action_dimension
+        if self.batch_mean is None or self.batch_mean.shape[0] != K:
+            self.batch_mean = torch.zeros((K, H, A), device=self.device, dtype=torch.float32)
+        self.last_values = None
+        if isinstance(obj_funs, _FusedBatchObjective):
+            if callback is None and not obj_funs.model_env.has_external_callables():
+                return self._optimize_fused_batch(obj_funs, _noise, _model_noise)
+            obj_funs = obj_funs.entries()
+        saved = self.mean
+        try:
+            for k, f in enumerate(obj_funs):
+                self.mean = self.batch_mean[k].clone()
+                self.batch_mean[k] = self.optimize(f, callback=callback, _noise=None if _noise is None else _noise[k])
+        finally:
+            self.mean = saved
+        return self.batch_mean.clone()
+
+    def _optimize_fused_batch(self, obj: _FusedBatchObjective, noise, model_noise) -> torch.Tensor:
+        env = obj.model_env
+        env._fresh()
+        self.batch_mean = self.batch_mean.to(self.device, torch.float32).contiguous()
+        K, H, A = self.batch_mean.shape
+        N, P, R = self.population_size, obj.num_particles, self.refinements
+        obs = np.asarray(obj.obs)
+        if obs.ndim != 2 or obs.shape[0] != K:
+            raise ValueError(f"observations must be [K={K}, obs_dim], got {tuple(obs.shape)}")
+        prop = env._propagation()
+        perms = eps = None
+        if model_noise is not None:
+            perms, eps = model_noise
+        if perms is None and R > 0:
+            # the draws of K consecutive single plans, in their order: problem-major, then refinement
+            per = [env._eval_perms(prop, N, H, P) for _ in range(K * R)]
+            if per[0] is not None:
+                perms = torch.stack(per).view(K, R, *per[0].shape)
+        # problem k takes optimiser counter first + k and environment counters env_first + k * R + r
+        first = _next_seed_offset(self)
+        self._offset += K - 1
+        rcfg = _lib.RolloutCfg(N, H, P, _lib.PREC[env.precision_for(prop)], _lib.PROP[prop],
+                               _lib.TS1_PERMS if perms is not None else _lib.TS1_TILE_SHUFFLE, env._seed, env._offset + 1)
+        env._offset += K * R
+        mcfg = _lib.MppiCfg(R, float(self.gamma), float(self.beta), self._seed, first)
+        need = self.lib.b200pets_mppi_plan_batch_workspace_bytes(env.staged.handle, C.byref(rcfg), C.byref(mcfg), K)
+        if self._plan_batch_ws is None or self._plan_batch_ws.numel() < need:
+            self._plan_batch_ws = torch.empty(max(need, 1), dtype=torch.uint8, device=self.device)
+        obs0 = torch.from_numpy(np.ascontiguousarray(obs, dtype=np.float32)).to(self.device)
+        z = None if noise is None else noise.to(self.device, torch.float32).contiguous()
+        if eps is not None:
+            eps = eps.to(self.device, torch.float32).contiguous()
+        if perms is not None:
+            perms = perms.to(self.device, torch.int64).contiguous()
+        if self.record_values:
+            self.last_values = torch.empty(K, R, N, device=self.device)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.b200pets_mppi_plan_batch(
+                env.staged.handle, C.byref(rcfg), C.byref(mcfg), K, _lib.ptr(obs0), _lib.ptr(self.batch_mean),
+                _lib.ptr(self.lower_bound), _lib.ptr(self.upper_bound), _lib.ptr(z), _lib.ptr(eps), _lib.ptr(perms),
+                _lib.ptr(self.last_values), _lib.ptr(self._plan_batch_ws), self._plan_batch_ws.numel(), _lib.stream_ptr()),
+                "mppi_plan_batch")
+        return self.batch_mean.clone()
 
 
 _KNOWN_TARGETS = {"CEMOptimizer": CEMOptimizer, "ICEMOptimizer": ICEMOptimizer, "MPPIOptimizer": MPPIOptimizer}
@@ -496,7 +572,8 @@ class TrajectoryOptimizer:
         return self._pin_batch.numpy().copy()
 
     def reset_batch(self, indices: Optional[Sequence[int]] = None):
-        """Restore the warm starts of the batch entries ``indices`` (all of them when None)."""
+        """Restore the warm starts of the batch entries ``indices`` (all of them when None).  MPPIOptimizer's carried
+        means are kept, as :meth:`reset` keeps ``MPPIOptimizer.mean``."""
         if indices is None or self.previous_solutions is None:
             self.previous_solutions = None
             return
@@ -596,7 +673,8 @@ class TrajectoryOptimizerAgent(Agent):
 
     def reset_batch(self, indices: Optional[Sequence[int]] = None):
         """Restore the warm starts of the batch entries ``indices`` (every entry when None) and drop the cached actions,
-        so that the next :meth:`act_batch` replans."""
+        so that the next :meth:`act_batch` replans.  With MPPIOptimizer the entries' carried means are not cleared, just
+        as :meth:`reset` leaves ``MPPIOptimizer.mean`` alone in the reference."""
         self.optimizer.reset_batch(indices)
         self._batch_actions = []
 
