@@ -400,6 +400,77 @@ int b200pets_mppi_plan_batch(b200pets_model_t model, const b200pets_rollout_cfg*
                              const float* upper, const float* z, const float* eps, const int64_t* perms,
                              float* values_out, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- Training the dynamics model (mbrl/models/model_trainer.py:70-262) ------------------------------------
+ * OneDTransitionRewardModel(GaussianMLP) trained with torch.optim.Adam, fp32 throughout. */
+
+/* element type of transition arrays */
+#define B200PETS_DTYPE_F32 0
+#define B200PETS_DTYPE_F64 1
+
+/* Raw transitions -> model inputs and targets (one_dim_tr_model.py:103-136), for a whole dataset at once:
+ *   inputs  [dev] float[rows][in_size]  = normalise(cat(obs_process_fn(obs), act)): norm_mode 1 (fp32 statistics, norm_mean /
+ *           norm_std [dev] float[in_size]) or 2 (fp64, [dev] double[in_size], the result rounded to fp32), 0 = none
+ *   targets [dev] float[rows][out_size] = next_obs - obs (next_obs for the no_delta columns, or for all of them when
+ *           target_is_delta == 0), then reward as the last column when learned_rewards
+ *   obs, next_obs [dev] [rows][obs_dim]; act [dev] [rows][act_dim]; reward [dev] [rows] (read only when learned_rewards),
+ *   all of element type `dtype`: B200PETS_DTYPE_F32 (float) or B200PETS_DTYPE_F64 (double).  Float64 transitions are
+ *   processed in double, as numpy processes them in the reference (obs_process_fn, delta, normaliser; fp32 statistics
+ *   promoted to double), and rounded to float at the end;
+ *   no_delta [host] int32[num_no_delta] observation columns, each < obs_dim <= 1024.
+ * in_size = obs_dim (+1 for B200PETS_PROC_CARTPOLE) + act_dim, out_size = obs_dim + learned_rewards.
+ * Refused: NULL pointers, an unknown dtype, obs_process or norm_mode, a no_delta column out of range. */
+typedef struct {
+  int32_t obs_dim, act_dim, obs_process, norm_mode, target_is_delta, learned_rewards;
+  int32_t dtype; /* B200PETS_DTYPE_* of obs, act, next_obs, reward */
+} b200pets_prep_desc;
+int b200pets_train_preprocess(const b200pets_prep_desc* desc, int64_t rows, const void* obs, const void* act,
+                              const void* next_obs, const void* reward, const void* norm_mean, const void* norm_std,
+                              const int32_t* no_delta, int32_t num_no_delta, float* inputs, float* targets, void* stream);
+
+/* A trainer: the caller's GaussianMLP parameters and torch.optim.Adam state (exp_avg, exp_avg_sq), updated in place by
+ * the kernels; nothing is copied and no gradient buffer exists.  Entries of params / exp_avg / exp_avg_sq [host arrays of
+ * dev pointers]: W_0, b_0, ..., W_L, b_L (L = num_hidden; W_l float[E][K_l][N_l], b_l float[E][1][N_l], N_L = out_size or
+ * 2 * out_size), then, unless deterministic, min_logvar and max_logvar (float[1][out_size]); the moments of the bounds are
+ * read only with learn_logvar_bounds (otherwise the bounds are constants, as with requires_grad=False) and may be NULL.
+ * Adam hyper-parameters are torch's (lr, betas, eps, weight_decay as L2 added to the gradient).  Refused: NULL desc /
+ * out / parameter or moment pointers, num_hidden < 1 or num_hidden + 1 > B200PETS_MAX_LAYERS (8), an unknown
+ * activation, non-positive sizes. */
+typedef struct b200pets_trainer_s* b200pets_trainer_t;
+typedef struct {
+  int32_t ensemble_size, in_size, out_size, hid_size, num_hidden;
+  int32_t activation; /* B200PETS_ACT_* */
+  float leaky_slope;
+  int32_t deterministic;
+  int32_t learn_logvar_bounds;
+  double lr, beta1, beta2, eps, weight_decay;
+} b200pets_train_desc;
+int b200pets_trainer_create(const b200pets_train_desc* desc, float* const* params, float* const* exp_avg,
+                            float* const* exp_avg_sq, b200pets_trainer_t* out);
+void b200pets_trainer_destroy(b200pets_trainer_t trainer);
+
+/* One epoch of ModelTrainer.train (model_trainer.py:152-156): `steps` minibatch updates (model.update: loss, backward,
+ * optimizer.step) enqueued on `stream` as one launch, with no host synchronisation.
+ *   inputs / targets [dev] the dataset (b200pets_train_preprocess), rows rows
+ *   indices [dev] int32[E][steps][batch]: rows of member e's minibatch at each step (a bootstrapped minibatch; give every
+ *           member the same rows for a plain TransitionIterator batch); every step has `batch` rows except the last, which
+ *           has last_batch (<= batch) and reads the first last_batch entries of its slice; entries must lie in [0, rows)
+ *   adam_step the optimizer's step count before the epoch (bias correction of step s uses adam_step + s + 1)
+ *   losses [dev] float[steps]: the loss of every step (loss.item() of the reference)
+ * Refused: NULL pointers, steps < 1, batch < 1, last_batch not in [1, batch], a workspace smaller than
+ * b200pets_train_workspace_bytes(trainer, batch). */
+size_t b200pets_train_workspace_bytes(b200pets_trainer_t trainer, int32_t batch);
+int b200pets_train_epoch(b200pets_trainer_t trainer, int64_t rows, const float* inputs, const float* targets,
+                         const int32_t* indices, int32_t steps, int32_t batch, int32_t last_batch, int64_t adam_step,
+                         float* losses, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ModelTrainer.evaluate (model_trainer.py:216-262) over a whole dataset in one launch: scores [dev] float[E], the mean
+ * over rows and output columns of member e's squared error (OneDTransitionRewardModel.eval_score).  Refused: NULL
+ * pointers, rows < 1, a workspace smaller than b200pets_eval_score_workspace_bytes(trainer, rows), layers wider than the
+ * kernel's shared-memory tile (B200PETS_EUNSUPPORTED). */
+size_t b200pets_eval_score_workspace_bytes(b200pets_trainer_t trainer, int64_t rows);
+int b200pets_eval_score(b200pets_trainer_t trainer, int64_t rows, const float* inputs, const float* targets, float* scores,
+                        void* workspace, size_t workspace_bytes, void* stream);
+
 /* Self test of the wgmma building block: D[128][n] = A[128][k] * B[n][k]^T with bf16 operands staged in the
  * no-swizzle canonical layouts, the weight ring and the accumulator fragments the rollout kernel uses.  a, b [dev] float
  * (rounded to bf16 inside), d [dev] float[128][n].  k, n multiples of 16, <= 256.  A negative k writes A as bf16 pairs

@@ -11,7 +11,8 @@ _LAZY = {
     "TrajectoryOptimizer": "planning", "TrajectoryOptimizerAgent": "planning",
     "create_trajectory_optim_agent_for_model": "planning", "complete_agent_cfg": "planning", "rollout_model_env": "planning",
     "GaussianMLP": "models", "OneDTransitionRewardModel": "models", "EnsembleLinearLayer": "models",
-    "Normalizer": "models", "model_from_arrays": "models",
+    "Normalizer": "models", "model_from_arrays": "models", "ModelTrainer": "trainer",
+    "TransitionBatch": "replay", "TransitionIterator": "replay", "BootstrapIterator": "replay",
 }
 
 
@@ -20,6 +21,7 @@ def __getattr__(name):
 
     if name in _LAZY:
         return getattr(importlib.import_module(f"{__name__}.{_LAZY[name]}"), name)
-    if name in ("synthetic", "functions", "planning", "models", "model_env", "staging", "_lib", "build", "dist", "mbpo"):
+    if name in ("synthetic", "functions", "planning", "models", "model_env", "staging", "_lib", "build", "dist", "mbpo",
+                "trainer", "replay"):
         return importlib.import_module(f"{__name__}.{name}")
     raise AttributeError(name)

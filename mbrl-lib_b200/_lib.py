@@ -20,6 +20,7 @@ TERM = {"no_termination": 0, "cartpole": 1, "inverted_pendulum": 2, "hopper": 3,
         "humanoid": 6, "external": 255}
 PROP = {"random_model": 0, "fixed_model": 1, "expectation": 2}
 PREC = {"f32": 0, "bf16_tc": 1}
+DTYPE = {"float32": 0, "float64": 1}
 TS1_PERMS, TS1_TILE_SHUFFLE = 0, 1
 
 
@@ -44,6 +45,17 @@ class CemCfg(C.Structure):
 class MppiCfg(C.Structure):
     _fields_ = [("num_iterations", C.c_int32), ("gamma", C.c_float), ("beta", C.c_float), ("sample_seed", C.c_uint64),
                 ("sample_counter", C.c_uint64)]
+
+
+class PrepDesc(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("obs_dim", "act_dim", "obs_process", "norm_mode", "target_is_delta",
+                                         "learned_rewards", "dtype")]
+
+
+class TrainDesc(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("ensemble_size", "in_size", "out_size", "hid_size", "num_hidden", "activation")] + \
+               [("leaky_slope", C.c_float), ("deterministic", C.c_int32), ("learn_logvar_bounds", C.c_int32)] + \
+               [(n, C.c_double) for n in ("lr", "beta1", "beta2", "eps", "weight_decay")]
 
 
 _P = C.c_void_p
@@ -113,6 +125,15 @@ _SIGNATURES = {
                                             C.c_int32, C.c_uint32, C.POINTER(C.c_void_p), _P, _P, _P, _P, _P, C.c_int32, _P, _P,
                                             C.c_uint64, C.c_uint64, C.c_int32, _P, _P, _P]),
     "b200pets_selftest_wgmma": (C.c_int, [C.c_int32, C.c_int32, _P, _P, _P, _P]),
+    "b200pets_train_preprocess": (C.c_int, [C.POINTER(PrepDesc), C.c_int64, _P, _P, _P, _P, _P, _P, C.POINTER(C.c_int32),
+                                            C.c_int32, _P, _P, _P]),
+    "b200pets_trainer_create": (C.c_int, [C.POINTER(TrainDesc), C.POINTER(_P), C.POINTER(_P), C.POINTER(_P), C.POINTER(_P)]),
+    "b200pets_trainer_destroy": (None, [_P]),
+    "b200pets_train_workspace_bytes": (C.c_size_t, [_P, C.c_int32]),
+    "b200pets_train_epoch": (C.c_int, [_P, C.c_int64, _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int64, _P, _P,
+                                       C.c_size_t, _P]),
+    "b200pets_eval_score_workspace_bytes": (C.c_size_t, [_P, C.c_int64]),
+    "b200pets_eval_score": (C.c_int, [_P, C.c_int64, _P, _P, _P, _P, C.c_size_t, _P]),
 }
 
 _lib = None

@@ -5,9 +5,11 @@
 
 #include <cuda_bf16.h>
 
+#include <new>
 #include <vector>
 
 #include "common.cuh"
+#include "train.cuh"
 
 // launchers defined in the kernel translation units
 int launch_rollout_f32(const ModelDev& m, const RolloutArgs& a, cudaStream_t stream);
@@ -994,6 +996,126 @@ int b200pets_shuffle_member_map(const b200pets_rollout_cfg* cfg, int32_t num_mem
 
 int b200pets_selftest_wgmma(int32_t k, int32_t n, const float* a, const float* b, float* d, void* stream) {
   return launch_wgmma_selftest(k, n, a, b, d, (cudaStream_t)stream);
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// training (train.cu)
+// ---------------------------------------------------------------------------------------------------------
+struct b200pets_trainer_s {
+  TrainDev dev;
+};
+
+int b200pets_train_preprocess(const b200pets_prep_desc* desc, int64_t rows, const void* obs, const void* act,
+                              const void* next_obs, const void* reward, const void* norm_mean, const void* norm_std,
+                              const int32_t* no_delta, int32_t num_no_delta, float* inputs, float* targets, void* stream) {
+  if (!desc || !obs || !act || !next_obs || !inputs || !targets || (desc->learned_rewards && !reward) ||
+      (desc->norm_mode && (!norm_mean || !norm_std)) || (num_no_delta > 0 && !no_delta))
+    return b200pets_set_error(B200PETS_EINVAL, "train_preprocess: NULL pointer");
+  const b200pets_prep_desc& d = *desc;
+  if (rows < 0 || d.obs_dim < 1 || d.act_dim < 0 || d.norm_mode < 0 || d.norm_mode > 2 || num_no_delta < 0)
+    return b200pets_set_error(B200PETS_EINVAL, "train_preprocess: bad sizes");
+  if (d.obs_process < B200PETS_PROC_NONE || d.obs_process > B200PETS_PROC_CARTPOLE)
+    return b200pets_set_error(B200PETS_EUNSUPPORTED, "train_preprocess: unknown obs_process %d", d.obs_process);
+  if (d.dtype != B200PETS_DTYPE_F32 && d.dtype != B200PETS_DTYPE_F64)
+    return b200pets_set_error(B200PETS_EUNSUPPORTED, "train_preprocess: unknown dtype %d", d.dtype);
+  if (d.obs_dim > 1024) return b200pets_set_error(B200PETS_EUNSUPPORTED, "train_preprocess: obs_dim %d > 1024", d.obs_dim);
+  PrepDesc p{};
+  p.D = d.obs_dim; p.A = d.act_dim; p.Dp = d.obs_dim + (d.obs_process == B200PETS_PROC_CARTPOLE ? 1 : 0);
+  p.in = p.Dp + p.A; p.out = d.obs_dim + (d.learned_rewards ? 1 : 0);
+  p.obs_process = d.obs_process; p.norm_mode = d.norm_mode; p.target_is_delta = d.target_is_delta;
+  p.learned_rewards = d.learned_rewards;
+  p.f64 = d.dtype == B200PETS_DTYPE_F64;
+  for (int i = 0; i < num_no_delta; ++i) {
+    const int c = no_delta[i];
+    if (c < 0 || c >= d.obs_dim) return b200pets_set_error(B200PETS_EINVAL, "train_preprocess: no_delta index %d", c);
+    p.no_delta[c >> 5] |= 1u << (c & 31);
+  }
+  return launch_train_preprocess(p, rows, obs, act, next_obs, reward, norm_mean, norm_std, inputs, targets,
+                                 (cudaStream_t)stream);
+}
+
+int b200pets_trainer_create(const b200pets_train_desc* desc, float* const* params, float* const* exp_avg,
+                            float* const* exp_avg_sq, b200pets_trainer_t* out) {
+  if (!desc || !params || !exp_avg || !exp_avg_sq || !out) return b200pets_set_error(B200PETS_EINVAL, "trainer_create: NULL pointer");
+  const b200pets_train_desc& d = *desc;
+  if (d.num_hidden < 1 || d.num_hidden + 1 > B200PETS_MAX_LAYERS)
+    return b200pets_set_error(B200PETS_EUNSUPPORTED, "trainer_create: %d hidden layers (1 .. %d)", d.num_hidden,
+                              B200PETS_MAX_LAYERS - 1);
+  if (d.activation != B200PETS_ACT_RELU && d.activation != B200PETS_ACT_SILU && d.activation != B200PETS_ACT_LEAKY_RELU)
+    return b200pets_set_error(B200PETS_EUNSUPPORTED, "trainer_create: unknown activation %d", d.activation);
+  if (d.ensemble_size < 1 || d.in_size < 1 || d.out_size < 1 || d.hid_size < 1)
+    return b200pets_set_error(B200PETS_EINVAL, "trainer_create: non-positive size");
+  TrainDev v{};
+  v.E = d.ensemble_size; v.in = d.in_size; v.out = d.out_size; v.hid = d.hid_size; v.L = d.num_hidden;
+  v.nout = d.deterministic ? d.out_size : 2 * d.out_size;
+  v.act = d.activation; v.leaky = d.leaky_slope; v.deterministic = d.deterministic ? 1 : 0;
+  v.learn_bounds = !d.deterministic && d.learn_logvar_bounds ? 1 : 0;
+  v.lr = d.lr; v.beta1 = d.beta1; v.beta2 = d.beta2; v.eps = d.eps; v.weight_decay = d.weight_decay;
+  const int layers = d.num_hidden + 1;
+  for (int l = 0; l < layers; ++l) {
+    v.K[l] = l == 0 ? d.in_size : d.hid_size;
+    v.N[l] = l == d.num_hidden ? v.nout : d.hid_size;
+    const int w = 2 * l, b = 2 * l + 1;
+    if (!params[w] || !params[b] || !exp_avg[w] || !exp_avg[b] || !exp_avg_sq[w] || !exp_avg_sq[b])
+      return b200pets_set_error(B200PETS_EINVAL, "trainer_create: NULL parameter or moment of layer %d", l);
+    v.W[l] = params[w]; v.b[l] = params[b];
+    v.mW[l] = exp_avg[w]; v.mb[l] = exp_avg[b];
+    v.vW[l] = exp_avg_sq[w]; v.vb[l] = exp_avg_sq[b];
+  }
+  if (!d.deterministic) {
+    for (int i = 0; i < 2; ++i) {
+      const int k = 2 * layers + i;
+      if (!params[k]) return b200pets_set_error(B200PETS_EINVAL, "trainer_create: NULL logvar bound");
+      v.lv[i] = params[k];
+      if (v.learn_bounds) {
+        if (!exp_avg[k] || !exp_avg_sq[k]) return b200pets_set_error(B200PETS_EINVAL, "trainer_create: NULL logvar-bound moment");
+        v.mlv[i] = exp_avg[k]; v.vlv[i] = exp_avg_sq[k];
+      }
+    }
+  }
+  b200pets_trainer_s* t = new (std::nothrow) b200pets_trainer_s;
+  if (!t) return b200pets_set_error(B200PETS_ENOMEM, "trainer_create: out of host memory");
+  t->dev = v;
+  *out = t;
+  return B200PETS_OK;
+}
+
+void b200pets_trainer_destroy(b200pets_trainer_t trainer) { delete trainer; }
+
+size_t b200pets_train_workspace_bytes(b200pets_trainer_t trainer, int32_t batch) {
+  if (!trainer || batch < 1) return 0;
+  return train_workspace_floats(trainer->dev, batch) * sizeof(float);
+}
+
+int b200pets_train_epoch(b200pets_trainer_t trainer, int64_t rows, const float* inputs, const float* targets,
+                         const int32_t* indices, int32_t steps, int32_t batch, int32_t last_batch, int64_t adam_step,
+                         float* losses, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!trainer || !inputs || !targets || !indices || !losses || !workspace)
+    return b200pets_set_error(B200PETS_EINVAL, "train_epoch: NULL pointer");
+  if (rows < 1 || steps < 1 || batch < 1 || last_batch < 1 || last_batch > batch || adam_step < 0)
+    return b200pets_set_error(B200PETS_EINVAL, "train_epoch: bad sizes (rows %lld, steps %d, batch %d, last_batch %d)",
+                              (long long)rows, steps, batch, last_batch);
+  const size_t need = b200pets_train_workspace_bytes(trainer, batch);
+  if (workspace_bytes < need)
+    return b200pets_set_error(B200PETS_EINVAL, "train_epoch: workspace of %zu bytes, %zu needed", workspace_bytes, need);
+  return launch_train_epoch(trainer->dev, rows, inputs, targets, indices, steps, batch, last_batch, adam_step, losses,
+                            (float*)workspace, (cudaStream_t)stream);
+}
+
+size_t b200pets_eval_score_workspace_bytes(b200pets_trainer_t trainer, int64_t rows) {
+  if (!trainer || rows < 1) return 0;
+  return eval_score_workspace_bytes(trainer->dev, rows);
+}
+
+int b200pets_eval_score(b200pets_trainer_t trainer, int64_t rows, const float* inputs, const float* targets, float* scores,
+                        void* workspace, size_t workspace_bytes, void* stream) {
+  if (!trainer || !inputs || !targets || !scores || !workspace)
+    return b200pets_set_error(B200PETS_EINVAL, "eval_score: NULL pointer");
+  if (rows < 1) return b200pets_set_error(B200PETS_EINVAL, "eval_score: rows %lld < 1", (long long)rows);
+  const size_t need = b200pets_eval_score_workspace_bytes(trainer, rows);
+  if (workspace_bytes < need)
+    return b200pets_set_error(B200PETS_EINVAL, "eval_score: workspace of %zu bytes, %zu needed", workspace_bytes, need);
+  return launch_eval_score(trainer->dev, rows, inputs, targets, scores, workspace, (cudaStream_t)stream);
 }
 
 }  // extern "C"

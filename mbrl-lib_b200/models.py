@@ -5,8 +5,9 @@ The drop-in use case hands *mbrl-lib's own* ``OneDTransitionRewardModel(Gaussian
 These classes exist so that tests, ``bench.py`` and users without mbrl-lib installed can build the same
 structure: ``.model.hidden_layers[i][0].{weight[E,K,N], bias[E,1,N]}``, ``.model.mean_and_logvar``,
 ``.model.{min,max}_logvar``, ``.model.elite_models``, ``.input_normalizer.{mean,std}`` ...
-(mbrl/models/gaussian_mlp.py:86-127, mbrl/models/one_dim_tr_model.py:84-101).  They hold parameters only;
-training stays in mbrl-lib / PyTorch (out of scope, SURVEY.md section 2 row 9).
+(mbrl/models/gaussian_mlp.py:86-127, mbrl/models/one_dim_tr_model.py:84-101).  They also carry the reference's
+PyTorch training interface (``loss`` / ``update`` / ``eval_score`` without propagation, ``_process_batch``): the loop
+:class:`mbrl_lib_b200.ModelTrainer` falls back to, and the yardstick its device path is tested against.
 """
 from __future__ import annotations
 
@@ -14,6 +15,7 @@ from typing import Callable, List, Optional, Sequence
 
 import numpy as np
 import torch
+import torch.nn.functional as F
 from torch import nn
 
 _ACT = {"relu": nn.ReLU, "silu": nn.SiLU, "leaky_relu": lambda: nn.LeakyReLU(0.01)}
@@ -27,6 +29,9 @@ class EnsembleLinearLayer(nn.Module):
         self.num_members, self.in_size, self.out_size = num_members, in_size, out_size
         self.weight = nn.Parameter(torch.zeros(num_members, in_size, out_size))
         self.bias = nn.Parameter(torch.zeros(num_members, 1, out_size))
+
+    def forward(self, x):  # every member (no elite selection): [E or 1, B, in] -> [E, B, out]
+        return x.matmul(self.weight) + self.bias
 
 
 class GaussianMLP(nn.Module):
@@ -59,6 +64,47 @@ class GaussianMLP(nn.Module):
     def set_propagation_method(self, propagation_method: Optional[str] = None):
         self.propagation_method = propagation_method
 
+    # ---- PyTorch training interface (gaussian_mlp.py:140-154, 283-361; model.py:129-167) --------------------------
+    def forward(self, x, use_propagation: bool = False):
+        """Every member's mean and (soft-bounded) logvar: [E, B, in] or [B, in] -> [E, B, out] each.  Only the
+        ``use_propagation=False`` form of the reference, the one training and evaluation use."""
+        ml = self.mean_and_logvar(self.hidden_layers(x))
+        if self.deterministic:
+            return ml, None
+        mean, logvar = ml[..., :self.out_size], ml[..., self.out_size:]
+        logvar = self.max_logvar - F.softplus(self.max_logvar - logvar)
+        logvar = self.min_logvar + F.softplus(logvar - self.min_logvar)
+        return mean, logvar
+
+    def loss(self, model_in, target):
+        if model_in.ndim == 2:
+            model_in, target = model_in.unsqueeze(0), target.unsqueeze(0)
+        mean, logvar = self.forward(model_in)
+        if self.deterministic:  # _mse_loss: summed squared error
+            return F.mse_loss(mean, target, reduction="none").sum((1, 2)).sum(), {}
+        if target.shape[0] != self.num_members:
+            target = target.repeat(self.num_members, 1, 1)
+        # gaussian_nll(reduce=False) averaged per member, summed over members, plus the bound penalty (_nll_loss)
+        nll = F.mse_loss(mean, target, reduction="none") * (-logvar).exp() + logvar
+        loss = nll.mean((1, 2)).sum()
+        return loss + 0.01 * (self.max_logvar.sum() - self.min_logvar.sum()), {}
+
+    def update(self, model_in, optimizer, target=None):
+        self.train()
+        optimizer.zero_grad()
+        loss, meta = self.loss(model_in, target)
+        loss.backward()
+        with torch.no_grad():  # the reference logs the gradient norm of every update
+            meta["grad_norm"] = sum(p.grad.norm(2).item() ** 2 for p in self.parameters() if p.grad is not None)
+        optimizer.step()
+        return loss.item(), meta
+
+    def eval_score(self, model_in, target):
+        """Squared error per member, row and output column: [E, B, out]."""
+        with torch.no_grad():
+            mean, _ = self.forward(model_in)
+            return F.mse_loss(mean, target.repeat((self.num_members, 1, 1)), reduction="none"), {}
+
 
 class Normalizer:
     """mean / std of the model input, [1, in]   (mbrl/util/math.py:95-143)."""
@@ -75,6 +121,11 @@ class Normalizer:
         self.mean = data.mean(0, keepdim=True)
         self.std = data.std(0, keepdim=True)
         self.std[self.std < self.eps] = 1.0
+
+    def normalize(self, val):
+        if isinstance(val, np.ndarray):
+            val = torch.from_numpy(val).to(self.device)
+        return (val - self.mean) / self.std
 
 
 class OneDTransitionRewardModel:
@@ -102,6 +153,52 @@ class OneDTransitionRewardModel:
 
     def __len__(self):
         return len(self.model)
+
+    # ---- PyTorch training interface (one_dim_tr_model.py:103-223) -------------------------------------------------
+    def parameters(self):
+        return self.model.parameters()
+
+    def state_dict(self):
+        return {f"model.{k}": v for k, v in self.model.state_dict().items()}
+
+    def load_state_dict(self, state_dict):
+        return self.model.load_state_dict({k[len("model."):]: v for k, v in state_dict.items()})
+
+    def update_normalizer(self, batch):
+        if self.input_normalizer is None:
+            return
+        obs, act = torch.as_tensor(batch.obs), torch.as_tensor(batch.act)
+        if obs.ndim == 1:
+            obs, act = obs[None], act[None]
+        if self.obs_process_fn:
+            obs = self.obs_process_fn(obs)
+        self.input_normalizer.update_stats(torch.cat([obs, act], dim=obs.ndim - 1).numpy())
+
+    def _process_batch(self, batch):
+        """Model input and target of a transition batch ([B, ...] or [E, B, ...] numpy arrays)."""
+        obs, act, next_obs, reward = (torch.as_tensor(x).to(self.device) for x in
+                                      (batch.obs, batch.act, batch.next_obs, batch.rewards))
+        target = next_obs
+        if self.target_is_delta:
+            target = next_obs - obs
+            for dim in self.no_delta_list:
+                target[..., dim] = next_obs[..., dim]
+        proc = self.obs_process_fn(obs) if self.obs_process_fn else obs
+        model_in = torch.cat([proc, act], dim=obs.ndim - 1)
+        if self.input_normalizer:
+            model_in = self.input_normalizer.normalize(model_in).float()
+        if self.learned_rewards:
+            target = torch.cat([target, reward.unsqueeze(reward.ndim)], dim=obs.ndim - 1)
+        return model_in.float(), target.float()
+
+    def update(self, batch, optimizer, target=None):
+        model_in, target = self._process_batch(batch)
+        return self.model.update(model_in, optimizer, target=target)
+
+    def eval_score(self, batch, target=None):
+        with torch.no_grad():
+            model_in, target = self._process_batch(batch)
+            return self.model.eval_score(model_in, target=target)
 
 
 def model_from_arrays(spec, arrays, device) -> OneDTransitionRewardModel:

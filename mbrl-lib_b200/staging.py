@@ -17,6 +17,12 @@ import torch
 from . import _lib, functions
 
 
+def mark_trained(mlp):
+    """Record that kernels rewrote ``mlp``'s parameters in place: their writes bypass torch's ``_version`` counters, so
+    :class:`mbrl_lib_b200.ModelTrainer` bumps this count, which every staged copy's signature includes."""
+    mlp._b200pets_trained = getattr(mlp, "_b200pets_trained", 0) + 1
+
+
 def _activation_of(module) -> tuple:
     name = type(module).__name__
     if name == "ReLU":
@@ -101,6 +107,7 @@ class StagedModel:
         if norm is not None:
             sig.append((id(norm.mean), norm.mean.data_ptr(), norm.mean._version, id(norm.std), norm.std._version))
         sig.append(tuple(self.members()))
+        sig.append(getattr(self.mlp, "_b200pets_trained", 0))
         return tuple(sig)
 
     # ---- staging ---------------------------------------------------------------------------------------
