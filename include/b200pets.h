@@ -447,6 +447,10 @@ typedef struct {
 int b200pets_trainer_create(const b200pets_train_desc* desc, float* const* params, float* const* exp_avg,
                             float* const* exp_avg_sq, b200pets_trainer_t* out);
 void b200pets_trainer_destroy(b200pets_trainer_t trainer);
+/* Whether the training kernels cover a model, asked before any tensor exists: 0 when b200pets_trainer_create accepts
+ * desc (pointers aside) and b200pets_eval_score can evaluate its layers on the current device; otherwise the code and
+ * b200pets_last_error() that the first of the two refusals gives (num_hidden > 7, or layers about 890 columns wide). */
+int b200pets_trainer_supported(const b200pets_train_desc* desc);
 
 /* One epoch of ModelTrainer.train (model_trainer.py:152-156): `steps` minibatch updates (model.update: loss, backward,
  * optimizer.step) enqueued on `stream` as one launch, with no host synchronisation.

@@ -129,6 +129,7 @@ _SIGNATURES = {
                                             C.c_int32, _P, _P, _P]),
     "b200pets_trainer_create": (C.c_int, [C.POINTER(TrainDesc), C.POINTER(_P), C.POINTER(_P), C.POINTER(_P), C.POINTER(_P)]),
     "b200pets_trainer_destroy": (None, [_P]),
+    "b200pets_trainer_supported": (C.c_int, [C.POINTER(TrainDesc)]),
     "b200pets_train_workspace_bytes": (C.c_size_t, [_P, C.c_int32]),
     "b200pets_train_epoch": (C.c_int, [_P, C.c_int64, _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int64, _P, _P,
                                        C.c_size_t, _P]),

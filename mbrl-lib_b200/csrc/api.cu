@@ -1034,27 +1034,44 @@ int b200pets_train_preprocess(const b200pets_prep_desc* desc, int64_t rows, cons
                                  (cudaStream_t)stream);
 }
 
-int b200pets_trainer_create(const b200pets_train_desc* desc, float* const* params, float* const* exp_avg,
-                            float* const* exp_avg_sq, b200pets_trainer_t* out) {
-  if (!desc || !params || !exp_avg || !exp_avg_sq || !out) return b200pets_set_error(B200PETS_EINVAL, "trainer_create: NULL pointer");
-  const b200pets_train_desc& d = *desc;
+// The descriptor checks of b200pets_trainer_create, and the sizes and hyper-parameters of its TrainDev (no pointers).
+static int train_desc_to_dev(const b200pets_train_desc& d, const char* who, TrainDev* out) {
   if (d.num_hidden < 1 || d.num_hidden + 1 > B200PETS_MAX_LAYERS)
-    return b200pets_set_error(B200PETS_EUNSUPPORTED, "trainer_create: %d hidden layers (1 .. %d)", d.num_hidden,
+    return b200pets_set_error(B200PETS_EUNSUPPORTED, "%s: %d hidden layers (1 .. %d)", who, d.num_hidden,
                               B200PETS_MAX_LAYERS - 1);
   if (d.activation != B200PETS_ACT_RELU && d.activation != B200PETS_ACT_SILU && d.activation != B200PETS_ACT_LEAKY_RELU)
-    return b200pets_set_error(B200PETS_EUNSUPPORTED, "trainer_create: unknown activation %d", d.activation);
+    return b200pets_set_error(B200PETS_EUNSUPPORTED, "%s: unknown activation %d", who, d.activation);
   if (d.ensemble_size < 1 || d.in_size < 1 || d.out_size < 1 || d.hid_size < 1)
-    return b200pets_set_error(B200PETS_EINVAL, "trainer_create: non-positive size");
+    return b200pets_set_error(B200PETS_EINVAL, "%s: non-positive size", who);
   TrainDev v{};
   v.E = d.ensemble_size; v.in = d.in_size; v.out = d.out_size; v.hid = d.hid_size; v.L = d.num_hidden;
   v.nout = d.deterministic ? d.out_size : 2 * d.out_size;
   v.act = d.activation; v.leaky = d.leaky_slope; v.deterministic = d.deterministic ? 1 : 0;
   v.learn_bounds = !d.deterministic && d.learn_logvar_bounds ? 1 : 0;
   v.lr = d.lr; v.beta1 = d.beta1; v.beta2 = d.beta2; v.eps = d.eps; v.weight_decay = d.weight_decay;
-  const int layers = d.num_hidden + 1;
-  for (int l = 0; l < layers; ++l) {
+  for (int l = 0; l <= d.num_hidden; ++l) {
     v.K[l] = l == 0 ? d.in_size : d.hid_size;
     v.N[l] = l == d.num_hidden ? v.nout : d.hid_size;
+  }
+  *out = v;
+  return B200PETS_OK;
+}
+
+int b200pets_trainer_supported(const b200pets_train_desc* desc) {
+  if (!desc) return b200pets_set_error(B200PETS_EINVAL, "trainer_supported: NULL pointer");
+  TrainDev v;
+  if (const int rc = train_desc_to_dev(*desc, "trainer_supported", &v)) return rc;
+  return eval_score_fits(v);
+}
+
+int b200pets_trainer_create(const b200pets_train_desc* desc, float* const* params, float* const* exp_avg,
+                            float* const* exp_avg_sq, b200pets_trainer_t* out) {
+  if (!desc || !params || !exp_avg || !exp_avg_sq || !out) return b200pets_set_error(B200PETS_EINVAL, "trainer_create: NULL pointer");
+  const b200pets_train_desc& d = *desc;
+  TrainDev v;
+  if (const int rc = train_desc_to_dev(d, "trainer_create", &v)) return rc;
+  const int layers = d.num_hidden + 1;
+  for (int l = 0; l < layers; ++l) {
     const int w = 2 * l, b = 2 * l + 1;
     if (!params[w] || !params[b] || !exp_avg[w] || !exp_avg[b] || !exp_avg_sq[w] || !exp_avg_sq[b])
       return b200pets_set_error(B200PETS_EINVAL, "trainer_create: NULL parameter or moment of layer %d", l);

@@ -589,10 +589,7 @@ int launch_train_epoch(const TrainDev& m, long long rows, const float* X, const 
   return 0;
 }
 
-int launch_eval_score(const TrainDev& m, long long rows, const float* X, const float* Y, float* scores, void* ws,
-                      cudaStream_t stream) {
-  const long long tiles = (rows + kEvalRows - 1) / kEvalRows;
-  if (tiles > 0x7fffffff) return b200pets_set_error(B200PETS_EINVAL, "eval_score: too many rows");
+int eval_score_fits(const TrainDev& m) {
   const int LD = eval_ld(m);
   const size_t smem = 2 * (size_t)kEvalRows * LD * sizeof(float);
   int dev, max_smem;
@@ -602,6 +599,16 @@ int launch_eval_score(const TrainDev& m, long long rows, const float* X, const f
   CUDA_TRY(cudaFuncGetAttributes(&fa, train_eval_kernel));
   if (smem + fa.sharedSizeBytes > (size_t)max_smem)  // dynamic activations + the kernel's static reduction buffers
     return b200pets_set_error(B200PETS_EUNSUPPORTED, "eval_score: layers of %d columns do not fit in shared memory", LD);
+  return 0;
+}
+
+int launch_eval_score(const TrainDev& m, long long rows, const float* X, const float* Y, float* scores, void* ws,
+                      cudaStream_t stream) {
+  const long long tiles = (rows + kEvalRows - 1) / kEvalRows;
+  if (tiles > 0x7fffffff) return b200pets_set_error(B200PETS_EINVAL, "eval_score: too many rows");
+  if (const int rc = eval_score_fits(m)) return rc;
+  const int LD = eval_ld(m);
+  const size_t smem = 2 * (size_t)kEvalRows * LD * sizeof(float);
   CUDA_TRY(cudaFuncSetAttribute(train_eval_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   unsigned int* counter = (unsigned int*)ws;
   float* partial = (float*)((char*)ws + 256);

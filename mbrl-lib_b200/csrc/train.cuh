@@ -30,6 +30,9 @@ int launch_train_epoch(const TrainDev& m, long long rows, const float* X, const 
                        int last_batch, long long adam_step, float* losses, float* ws, cudaStream_t stream);
 int launch_eval_score(const TrainDev& m, long long rows, const float* X, const float* Y, float* scores, void* ws,
                       cudaStream_t stream);
+// 0 when train_eval_kernel holds every layer's activations in shared memory on the current device, else the refusal
+// (B200PETS_EUNSUPPORTED) launch_eval_score returns.  Reads only the sizes of m.
+int eval_score_fits(const TrainDev& m);
 
 struct PrepDesc {
   int D, A, Dp, in, out, obs_process, norm_mode, target_is_delta, learned_rewards;

@@ -18,9 +18,10 @@ What runs where:
     other iterable of transition batches takes one fused Adam step per yielded batch.  Transitions may be float32 or
     float64 (mbrl-lib's PETS / MBPO replay buffers are float64 with ``normalize_double_precision``); float64 ones are
     processed in double, as the reference's numpy / torch code processes them, and rounded to float32 at the end;
-  * otherwise (a ``batch_callback``, which needs every batch's loss as it happens, another model, or transitions of
-    another element type) the reference's PyTorch loop runs unchanged: ``model.update(batch, optimizer)`` /
-    ``model.eval_score(batch)``.
+  * otherwise (a ``batch_callback``, which needs every batch's loss as it happens, another model, a model the kernels
+    refuse -- more than 7 hidden layers, or layers too wide for the evaluation kernel's shared memory -- or transitions
+    of another element type) the reference's PyTorch loop runs unchanged: ``model.update(batch, optimizer)`` /
+    ``model.eval_score(batch)``.  A refused model runs the whole ``train()`` / ``evaluate()`` call that way.
 """
 from __future__ import annotations
 
@@ -93,14 +94,7 @@ class _DeviceModel:
         P = (C.c_void_p * n)(*[p.data_ptr() for p in allp])
         M = (C.c_void_p * n)(*[optimizer.state[p]["exp_avg"].data_ptr() if p in optimizer.state else None for p in allp])
         V = (C.c_void_p * n)(*[optimizer.state[p]["exp_avg_sq"].data_ptr() if p in optimizer.state else None for p in allp])
-        act, slope = staging._activation_of(mlp.hidden_layers[0][1])
-        d = _lib.TrainDesc()
-        d.ensemble_size = int(self.layers[0].weight.shape[0])
-        d.in_size, d.out_size = int(mlp.in_size), int(mlp.out_size)
-        d.hid_size, d.num_hidden = int(self.layers[0].weight.shape[2]), len(self.layers) - 1
-        d.activation, d.leaky_slope = act, slope
-        d.deterministic, d.learn_logvar_bounds = int(bool(mlp.deterministic)), int(self.learn_bounds)
-        d.lr, (d.beta1, d.beta2), d.eps, d.weight_decay = group["lr"], group["betas"], group["eps"], group["weight_decay"]
+        d = train_desc(mlp, group)
         self.E = d.ensemble_size
         h = C.c_void_p()
         _lib.check(self.lib.b200pets_trainer_create(C.byref(d), P, M, V, C.byref(h)), "trainer_create")
@@ -128,6 +122,7 @@ class _DeviceModel:
         if dtype is None:
             raise TypeError("the training kernels read float32 or float64 transitions; got "
                             f"{[str(getattr(x, 'dtype', type(x))) for x in (batch.obs, batch.act, batch.next_obs, batch.rewards)]}")
+        check_model_sizes(w, int(np.shape(batch.obs)[-1]), int(np.shape(batch.act)[-1]))
         obs, act, next_obs, reward = (torch.as_tensor(x).to(dev, dtype).contiguous()
                                       for x in (batch.obs, batch.act, batch.next_obs, batch.rewards))
         rows = int(obs.shape[0])
@@ -198,6 +193,37 @@ class _DeviceModel:
             pass
 
 
+def train_desc(mlp, group) -> _lib.TrainDesc:
+    """The C descriptor of a GaussianMLP trained with the Adam hyper-parameters of ``group``."""
+    layers = [seq[0] for seq in mlp.hidden_layers] + [mlp.mean_and_logvar]
+    act, slope = staging._activation_of(mlp.hidden_layers[0][1])
+    learn_bounds = not mlp.deterministic and mlp.min_logvar.requires_grad and mlp.max_logvar.requires_grad
+    d = _lib.TrainDesc()
+    d.ensemble_size = int(layers[0].weight.shape[0])
+    d.in_size, d.out_size = int(mlp.in_size), int(mlp.out_size)
+    d.hid_size, d.num_hidden = int(layers[0].weight.shape[2]), len(layers) - 1
+    d.activation, d.leaky_slope = act, slope
+    d.deterministic, d.learn_logvar_bounds = int(bool(mlp.deterministic)), int(learn_bounds)
+    d.lr, (d.beta1, d.beta2), d.eps, d.weight_decay = group["lr"], group["betas"], group["eps"], group["weight_decay"]
+    return d
+
+
+def check_model_sizes(model, obs_dim: int, act_dim: int):
+    """Raise ValueError unless the model's ``in_size`` / ``out_size`` are the widths ``_process_batch`` makes of
+    transitions with ``obs_dim`` / ``act_dim`` columns: ``obs_process_fn``'s output plus the action, and the observation
+    plus the reward when it is learned.  The preprocessing kernel writes those widths whatever the model says, so a model
+    built for other data (the cartpole ``obs_process_fn`` adds a column) would have it write past the staged arrays; the
+    reference raises a shape error there too."""
+    proc = functions.resolve_obs_process(getattr(model, "obs_process_fn", None))
+    want_in = obs_dim + (1 if proc == _lib.PROC["cartpole"] else 0) + act_dim
+    want_out = obs_dim + int(bool(model.learned_rewards))
+    mlp = model.model
+    if (int(mlp.in_size), int(mlp.out_size)) != (want_in, want_out):
+        raise ValueError(f"transitions with {obs_dim} observation and {act_dim} action columns make model inputs of "
+                         f"{want_in} and targets of {want_out} columns; the model has in_size {mlp.in_size} and "
+                         f"out_size {mlp.out_size}")
+
+
 def transition_dtype(batch) -> Optional[torch.dtype]:
     """The precision the reference's ``_process_batch`` computes a batch in: float64 when obs, act or next_obs is float64
     (numpy / torch promote the others), float32 when all are float32 (the reward column is rounded to float32 either way:
@@ -263,7 +289,12 @@ class ModelTrainer:
         if g.get("amsgrad") or g.get("maximize") or g.get("capturable") or g.get("differentiable") or g.get("fused") or \
                 g.get("decoupled_weight_decay") or isinstance(g["lr"], torch.Tensor):
             return False
-        return {id(p) for p in g["params"]} == {id(p) for p in params}
+        if {id(p) for p in g["params"]} != {id(p) for p in params}:
+            return False
+        # the kernels' own limits (more than 7 hidden layers; layers too wide for the evaluation kernel's shared memory),
+        # asked before anything is touched, so that the reference loop runs from the same state
+        with torch.cuda.device(dev):
+            return _lib.load().b200pets_trainer_supported(C.byref(train_desc(mlp, g))) == 0
 
     @staticmethod
     def _store_supported(ds) -> bool:

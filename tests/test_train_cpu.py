@@ -218,3 +218,37 @@ def test_container_loss_is_the_reference_formula():
             + 0.01 * (model.max_logvar.sum() - model.min_logvar.sum()))
     got, _ = model.loss(x, y)
     assert abs(got.item() - want.item()) < 1e-10
+
+
+def test_stage_refuses_a_model_the_transitions_do_not_fit():
+    """pets_cartpole_paper_version without dynamics_model.in_size=6: the cartpole obs_process_fn makes 4 + 1 observation
+    columns and the action one more, so a model of in_size 5 would have the preprocessing kernel write past its staged
+    inputs.  The check runs on the host, before anything is copied or launched."""
+    from mbrl_lib_b200 import functions
+
+    mlp = models.GaussianMLP(5, 5, "cpu", num_layers=2, ensemble_size=2, hid_size=8)
+    model = models.OneDTransitionRewardModel(mlp, obs_process_fn=functions.OBS_PROCESS_FNS["cartpole"])
+    store = _store(n=16, D=4, A=1)
+    with pytest.raises(ValueError, match="in_size 5"):
+        tr.check_model_sizes(model, 4, 1)
+    dm = tr._DeviceModel(model, tr.ModelTrainer(model).optimizer)  # a handle only: nothing runs on a CPU model
+    try:
+        with pytest.raises(ValueError, match="in_size 5"):
+            dm.stage(store)
+    finally:
+        dm.close()
+    # the sizes that do fit, and the reward column
+    tr.check_model_sizes(models.OneDTransitionRewardModel(models.GaussianMLP(6, 5, "cpu", num_layers=1, hid_size=8),
+                                                          obs_process_fn=functions.OBS_PROCESS_FNS["cartpole"]), 4, 1)
+    with pytest.raises(ValueError, match="out_size 5"):
+        tr.check_model_sizes(models.OneDTransitionRewardModel(models.GaussianMLP(5, 5, "cpu", num_layers=1, hid_size=8),
+                                                              learned_rewards=False), 4, 1)
+
+
+def test_trainer_supported_refuses_what_trainer_create_refuses():
+    lib = _lib.load()
+    assert lib.b200pets_trainer_supported(None) == -1
+    assert lib.b200pets_trainer_supported(C.byref(_desc(num_hidden=8))) == -2
+    assert b"trainer_supported" in lib.b200pets_last_error() and b"hidden layers" in lib.b200pets_last_error()
+    assert lib.b200pets_trainer_supported(C.byref(_desc(activation=7))) == -2
+    assert lib.b200pets_trainer_supported(C.byref(_desc(hid_size=0))) == -1
