@@ -55,6 +55,7 @@ template <int NWG>
 constexpr int threads_of() { return 128 * NWG + 32; }
 constexpr int kSliceK16 = 4;       // longest ring slot in K steps (16 rows of the weight image each)
 constexpr int kMaxStages = 16;
+constexpr int kActRegs = 8;  // models with up to this many actions load a step's action words in one round trip
 
 __device__ __forceinline__ float tanh_approx(float x) {
   float y;
@@ -392,12 +393,23 @@ __device__ __forceinline__ void rollout_tc_body(const ModelDev& m, const Rollout
       float tot = 0.f;
       int dead = 0;
       const float* act_row = a.act + prob_off<BATCH>(bt, kp, &BatchArgs::act) + (rid / a.act_div) * a.act_row_stride;
-      // this step's actions from the action tensor into the row's action words
+      // this step's actions from the action tensor into the row's action words.  Up to kActRegs words are loaded into
+      // registers first, so that the loads are in flight together (the word-by-word loop waits for each load before
+      // it issues the next: one L2 round trip per word).
       auto load_actions = [&](int t) {
         if (owner) {
           const float* ap = act_row + (long long)t * a.act_t_stride;
+          if (m.A <= kActRegs) {
+            float v[kActRegs];
+#pragma unroll
+            for (int j = 0; j < kActRegs; ++j) v[j] = (j < m.A && valid) ? ap[j] : 0.f;
+#pragma unroll
+            for (int j = 0; j < kActRegs; ++j)
+              if (j < m.A) my_act[j] = v[j];
+          } else {
 #pragma unroll 1
-          for (int j = 0; j < m.A; ++j) my_act[j] = valid ? ap[j] : 0.f;
+            for (int j = 0; j < m.A; ++j) my_act[j] = valid ? ap[j] : 0.f;
+          }
         }
       };
       wg_bar(wg);  // previous tile fully consumed before its row state is overwritten
@@ -524,7 +536,7 @@ __device__ __forceinline__ void rollout_tc_body(const ModelDev& m, const Rollout
           tot += rew;
         }
         if (t + 1 < a.t1) {
-          wg_bar(wg);  // the score has read this step's actions
+          // the owner overwrites the action words its own score has just read: no barrier before
           load_actions(t + 1);
           wg_bar(wg);  // both threads of a row build the next operand from the action words one of them wrote
         }
