@@ -159,7 +159,7 @@ class ShardedCEMOptimizer:
         return self._peer
 
     def _close_peers(self):
-        if self._peer is None:
+        if getattr(self, "_peer", None) is None:  # (also a constructor that refused its arguments: __del__ still runs)
             return
         try:
             with torch.cuda.device(self.device):

@@ -6,7 +6,8 @@ on ONE GPU, so that the single-GPU suite covers them (tests/test_gpu_multi.py ne
 * world = 2 emulated in one process: two "ranks" with their own buffers, kernels on two streams (they wait for each other's
   flags, so they must be co-resident: two single-CTA selects + sampling CTAs fit an H100 many times over); both must end
   with the refit of the UNION population and draw their own shard of the next one.
-NaNs, ties at the selection threshold and a -inf are in the values on purpose.
+NaNs, ties at the selection threshold and a -inf are in the values on purpose; the world-1 case also runs on the hazard
+values of the refit tests (+inf among the elites, the k-th value inside a run of zeros of both signs).
 """
 import ctypes as C
 import os
@@ -40,6 +41,23 @@ def _problem(n, dims, seed=0):
     return pop, values, mu, disp, lb, ub
 
 
+def _hazard_problem(n, dims, k, seed=0):
+    """_problem with the values of tests/test_gpu_scale.py::_refit_values: k // 2 values above the rest with two +inf among
+    them, then a run of k exact zeros of both signs in which the k-th largest falls, NaNs and three -inf below."""
+    pop, values, mu, disp, lb, ub = _problem(n, dims, seed)
+    g = torch.Generator().manual_seed(seed + 1)
+    order = torch.randperm(n, generator=g)
+    hi, zeros, rest = order[:k // 2], order[k // 2:k // 2 + k], order[k // 2 + k:]
+    values = torch.randn(n, generator=g)
+    values[hi] = values[hi].abs() + 1.0
+    values[hi[:2]] = float("inf")
+    values[zeros] = torch.where(torch.rand(zeros.numel(), generator=g) < 0.5, 0.0, -0.0)
+    values[rest] = -values[rest].abs() - 1e-3
+    values[rest[:3]] = float("nan")
+    values[rest[-3:]] = float("-inf")
+    return pop, values, mu, disp, lb, ub
+
+
 def _single_gpu_reference(lib, pop, values, mu, disp, lb, ub, k, alpha, seed, offset, first, n_next):
     """b200pets_cem_update on the whole population, then the next population shard [first, first + n_next)."""
     n, dims = pop.shape
@@ -67,8 +85,20 @@ def _alloc(lib, world, n_loc, dims, k):
 
 @pytest.mark.parametrize("n,dims,k", [(500, 180, 50), (96, 12, 7), (3000, 30, 300)])
 def test_peer_exchange_world1_equals_single_gpu_refit(n, dims, k):
+    _check_world1(n, dims, k, _problem(n, dims))
+
+
+@pytest.mark.parametrize("n,dims,k", [(500, 180, 50), (96, 12, 7), (3000, 30, 300)])
+def test_peer_exchange_world1_on_hazard_values_equals_single_gpu_refit(n, dims, k):
+    """World 1 only: the kernel waits on no other kernel, so the hazards cost no co-residency."""
+    problem = _hazard_problem(n, dims, k)
+    assert problem[1].isnan().any() and problem[1].isposinf().any() and problem[1].isneginf().any()
+    _check_world1(n, dims, k, problem)
+
+
+def _check_world1(n, dims, k, problem):
     lib = _lib.load()
-    pop, values, mu, disp, lb, ub = _problem(n, dims)
+    pop, values, mu, disp, lb, ub = problem
     alpha, seed, offset = 0.1, 1234, 77
     want = _single_gpu_reference(lib, pop, values, mu, disp, lb, ub, k, alpha, seed, offset, 0, n)
     buf = _alloc(lib, 1, n, dims, k)
