@@ -400,6 +400,78 @@ int b200pets_mppi_plan_batch(b200pets_model_t model, const b200pets_rollout_cfg*
                              const float* upper, const float* z, const float* eps, const int64_t* perms,
                              float* values_out, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- PlaNet's latent model (mbrl/models/planet.py, mbrl/algorithms/planet.py) --------------------------------
+ * The prior transition and reward models PlaNet plans with, PlaNetModel.sample (planet.py:531-581), in fp32:
+ *   e = relu(W_e [s, a] + b_e);  h' = GRUCell(e, h);  p = W_p2 relu(W_p1 h' + b_p1) + b_p2;
+ *   s' = p[:L] + (softplus(p[L:]) + min_std) * eps  (s' = p[:L] when deterministic);
+ *   reward = W_r3 relu(W_r2 relu(W_r1 [h', s'] + b_r1) + b_r2) + b_r3.
+ * The encoder, the posterior and the decoder (update_posterior, training) stay with the caller. */
+typedef struct b200pets_latent_model_s* b200pets_latent_model_t;
+typedef struct {
+  int32_t action_size;  /* A */
+  int32_t latent_size;  /* L, latent_state_size */
+  int32_t belief_size;  /* Hb */
+  int32_t hidden_size;  /* Hf, hidden_size_fcs */
+  float min_std;
+} b200pets_latent_model_desc;
+
+/* params [host] array of B200PETS_LATENT_NUM_PARAMS device pointers to contiguous fp32 tensors in torch's layout:
+ *    0 W_e [Hb][L+A], 1 b_e [Hb]                                belief_model.embedding_layer[0]
+ *    2 weight_ih [3Hb][Hb], 3 weight_hh [3Hb][Hb], 4 bias_ih [3Hb], 5 bias_hh [3Hb]   belief_model.rnn (gates r, z, n)
+ *    6 W_p1 [Hf][Hb], 7 b_p1 [Hf]                               prior_transition_model[0]
+ *    8 W_p2 [2L][Hf], 9 b_p2 [2L]                               prior_transition_model[2]
+ *   10 W_r1 [Hf][Hb+L], 11 b_r1 [Hf]                            reward_model[0] (input: belief, then latent)
+ *   12 W_r2 [Hf][Hf], 13 b_r2 [Hf]                              reward_model[2]
+ *   14 W_r3 [1][Hf], 15 b_r3 [1]                                reward_model[4]
+ * Staging packs transposed copies on `stream` (no host round trip); refresh re-packs them after the weights changed.
+ * Refused (B200PETS_EUNSUPPORTED): a model whose per-row state needs more than an eighth of the device's opt-in shared
+ * memory per CTA (29 056 bytes on an H100: about belief = hidden = 1200 at L 30, A 6); b200pets_latent_plan_info
+ * reports the bytes per row. */
+#define B200PETS_LATENT_NUM_PARAMS 16
+int b200pets_latent_model_create(const b200pets_latent_model_desc* desc, const float* const* params, void* stream,
+                                 b200pets_latent_model_t* out);
+int b200pets_latent_model_refresh(b200pets_latent_model_t model, const float* const* params, void* stream);
+void b200pets_latent_model_destroy(b200pets_latent_model_t model);
+/* The rollout kernel's launch for `rows` rows on the current device:
+ *   info[0] rows per CTA (1, 2, 4, 8, 16 or 32: enough CTAs to cover the SMs once, at most 32 rows)
+ *   info[1] CTAs;  info[2] dynamic shared memory of one CTA in bytes;  info[3] shared memory bytes of one row */
+int b200pets_latent_plan_info(b200pets_latent_model_t model, int64_t rows, int32_t info[4]);
+
+/* ModelEnv.step over PlaNetModel.sample (model_env.py:87-140) for `batch` independent states, one launch:
+ *   latent [dev] float[B][L], belief [dev] float[B][Hb], act [dev] float[B][A]
+ *   eps [dev] float[B][L] injected N(0,1) draws or NULL = Philox (RNG_STREAM_LATENT, step 0, key seed / offset);
+ *   sample == 0 returns the prior's mean (deterministic=True) and reads no draw
+ *   next_latent [dev] float[B][L], next_belief [dev] float[B][Hb], reward [dev] float[B] (each may be NULL) */
+int b200pets_latent_step(b200pets_latent_model_t model, int64_t batch, const float* latent, const float* belief,
+                         const float* act, const float* eps, uint64_t seed, uint64_t offset, int32_t sample,
+                         float* next_latent, float* next_belief, float* reward, void* stream);
+
+/* ModelEnv.evaluate_action_sequences over PlaNetModel with no_termination (model_env.py:145-191): every row starts at
+ * the posterior, row r = n * P + p follows sequence n, draws every step (sample=True), sums the rewards; returns the
+ * particle mean.  One launch for the whole horizon, plus the particle mean.
+ * The latent entry points read population, horizon, particles, seed and offset of b200pets_rollout_cfg; precision must
+ * be B200PETS_PREC_F32, first_sequence 0 and global_population 0 or population (no sharding); propagation and ts1_mode
+ * are not read.
+ *   latent0 [dev] float[L], belief0 [dev] float[Hb]: the posterior (PlaNetModel.reset repeats it)
+ *   actions [dev] float[N][H][A]; eps [dev] float[H][B][L] or NULL = Philox (row r, step t as in b200pets_latent_step)
+ *   returns [dev] float[N]; row_returns [dev] float[B] or NULL */
+size_t b200pets_latent_eval_workspace_bytes(b200pets_latent_model_t model, const b200pets_rollout_cfg* cfg);
+int b200pets_latent_eval_sequences(b200pets_latent_model_t model, const b200pets_rollout_cfg* cfg, const float* latent0,
+                                   const float* belief0, const float* actions, const float* eps, float* returns,
+                                   float* row_returns, void* workspace, size_t workspace_bytes, void* stream);
+
+/* CEMOptimizer.optimize over the latent model's evaluate_action_sequences as one call: the structure, Philox offsets
+ * (offset * 1024 + iteration for the population and the rollout) and values_out of b200pets_cem_plan, with the latent
+ * rollout in place of the ensemble's.  b200pets_cem_cfg is read whole.  z [dev] float[it][N][H*A] or NULL,
+ * eps [dev] float[it][H][B][L] or NULL; x0, lower, upper, solution [dev] float[H*A]; values_out [dev] float[it][N] or
+ * NULL. */
+size_t b200pets_latent_cem_plan_workspace_bytes(b200pets_latent_model_t model, const b200pets_rollout_cfg* rcfg,
+                                                const b200pets_cem_cfg* ccfg);
+int b200pets_latent_cem_plan(b200pets_latent_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg,
+                             const float* latent0, const float* belief0, const float* x0, const float* lower,
+                             const float* upper, const float* z, const float* eps, float* solution, float* values_out,
+                             void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- Training the dynamics model (mbrl/models/model_trainer.py:70-262) ------------------------------------
  * OneDTransitionRewardModel(GaussianMLP) trained with torch.optim.Adam, fp32 throughout. */
 

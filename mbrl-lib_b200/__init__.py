@@ -6,12 +6,12 @@ without the CUDA library; every compute entry point fails loudly when ``libb200p
 __version__ = "0.1.0"
 
 _LAZY = {
-    "ModelEnv": "model_env", "StagedModel": "staging",
+    "ModelEnv": "model_env", "StagedModel": "staging", "LatentModelEnv": "latent", "StagedLatentModel": "latent",
     "Agent": "planning", "Optimizer": "planning", "CEMOptimizer": "planning", "ICEMOptimizer": "planning", "MPPIOptimizer": "planning",
     "TrajectoryOptimizer": "planning", "TrajectoryOptimizerAgent": "planning",
     "create_trajectory_optim_agent_for_model": "planning", "complete_agent_cfg": "planning", "rollout_model_env": "planning",
     "GaussianMLP": "models", "OneDTransitionRewardModel": "models", "EnsembleLinearLayer": "models",
-    "Normalizer": "models", "model_from_arrays": "models", "ModelTrainer": "trainer",
+    "Normalizer": "models", "model_from_arrays": "models", "PlaNetModel": "models", "ModelTrainer": "trainer",
     "TransitionBatch": "replay", "TransitionIterator": "replay", "BootstrapIterator": "replay",
 }
 
@@ -22,6 +22,6 @@ def __getattr__(name):
     if name in _LAZY:
         return getattr(importlib.import_module(f"{__name__}.{_LAZY[name]}"), name)
     if name in ("synthetic", "functions", "planning", "models", "model_env", "staging", "_lib", "build", "dist", "mbpo",
-                "trainer", "replay"):
+                "trainer", "replay", "latent"):
         return importlib.import_module(f"{__name__}.{name}")
     raise AttributeError(name)

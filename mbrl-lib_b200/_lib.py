@@ -47,6 +47,14 @@ class MppiCfg(C.Structure):
                 ("sample_counter", C.c_uint64)]
 
 
+class LatentDesc(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("action_size", "latent_size", "belief_size", "hidden_size")] + \
+               [("min_std", C.c_float)]
+
+
+LATENT_NUM_PARAMS = 16
+
+
 class PrepDesc(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("obs_dim", "act_dim", "obs_process", "norm_mode", "target_is_delta",
                                          "learned_rewards", "dtype")]
@@ -125,6 +133,16 @@ _SIGNATURES = {
                                             C.c_int32, C.c_uint32, C.POINTER(C.c_void_p), _P, _P, _P, _P, _P, C.c_int32, _P, _P,
                                             C.c_uint64, C.c_uint64, C.c_int32, _P, _P, _P]),
     "b200pets_selftest_wgmma": (C.c_int, [C.c_int32, C.c_int32, _P, _P, _P, _P]),
+    "b200pets_latent_model_create": (C.c_int, [C.POINTER(LatentDesc), C.POINTER(_P), _P, C.POINTER(_P)]),
+    "b200pets_latent_model_refresh": (C.c_int, [_P, C.POINTER(_P), _P]),
+    "b200pets_latent_model_destroy": (None, [_P]),
+    "b200pets_latent_plan_info": (C.c_int, [_P, C.c_int64, C.POINTER(C.c_int32)]),
+    "b200pets_latent_step": (C.c_int, [_P, C.c_int64, _P, _P, _P, _P, C.c_uint64, C.c_uint64, C.c_int32, _P, _P, _P, _P]),
+    "b200pets_latent_eval_workspace_bytes": (C.c_size_t, [_P, C.POINTER(RolloutCfg)]),
+    "b200pets_latent_eval_sequences": (C.c_int, [_P, C.POINTER(RolloutCfg), _P, _P, _P, _P, _P, _P, _P, C.c_size_t, _P]),
+    "b200pets_latent_cem_plan_workspace_bytes": (C.c_size_t, [_P, C.POINTER(RolloutCfg), C.POINTER(CemCfg)]),
+    "b200pets_latent_cem_plan": (C.c_int, [_P, C.POINTER(RolloutCfg), C.POINTER(CemCfg), _P, _P, _P, _P, _P, _P, _P, _P, _P,
+                                           _P, C.c_size_t, _P]),
     "b200pets_train_preprocess": (C.c_int, [C.POINTER(PrepDesc), C.c_int64, _P, _P, _P, _P, _P, _P, C.POINTER(C.c_int32),
                                             C.c_int32, _P, _P, _P]),
     "b200pets_trainer_create": (C.c_int, [C.POINTER(TrainDesc), C.POINTER(_P), C.POINTER(_P), C.POINTER(_P), C.POINTER(_P)]),

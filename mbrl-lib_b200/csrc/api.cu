@@ -9,6 +9,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "latent.cuh"
 #include "train.cuh"
 
 // launchers defined in the kernel translation units
@@ -1133,6 +1134,225 @@ int b200pets_eval_score(b200pets_trainer_t trainer, int64_t rows, const float* i
   if (workspace_bytes < need)
     return b200pets_set_error(B200PETS_EINVAL, "eval_score: workspace of %zu bytes, %zu needed", workspace_bytes, need);
   return launch_eval_score(trainer->dev, rows, inputs, targets, scores, workspace, (cudaStream_t)stream);
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// PlaNet's latent model (latent.cu)
+// ---------------------------------------------------------------------------------------------------------
+}  // extern "C"
+
+struct b200pets_latent_model_s {
+  b200pets_latent_model_desc desc;
+  LatentDev dev;
+  float* blob = nullptr;
+};
+
+static int latent_check_params(const float* const* params, const char* who) {
+  if (!params) return b200pets_set_error(B200PETS_EINVAL, "%s: null params", who);
+  for (int i = 0; i < B200PETS_LATENT_NUM_PARAMS; ++i)
+    if (!params[i]) return b200pets_set_error(B200PETS_EINVAL, "%s: parameter %d is NULL", who, i);
+  return B200PETS_OK;
+}
+
+// checks of the latent evaluation and plan entry points: the fields of b200pets_rollout_cfg they read or constrain
+static int latent_check_cfg(const b200pets_rollout_cfg* cfg, const char* who) {
+  if (cfg->population <= 0 || cfg->horizon <= 0 || cfg->particles <= 0)
+    return b200pets_set_error(B200PETS_EINVAL, "%s: population, horizon, particles must be positive", who);
+  if (cfg->precision != B200PETS_PREC_F32)
+    return b200pets_set_error(B200PETS_EUNSUPPORTED, "%s: the latent model runs in fp32 only (precision %d)", who, cfg->precision);
+  if (cfg->first_sequence != 0 || (cfg->global_population != 0 && cfg->global_population != cfg->population))
+    return b200pets_set_error(B200PETS_EUNSUPPORTED, "%s: the latent model's population cannot be sharded (first_sequence %d, "
+                                                     "global_population %d)", who, cfg->first_sequence, cfg->global_population);
+  return B200PETS_OK;
+}
+
+static void latent_rollout_args(const b200pets_rollout_cfg* cfg, unsigned long long offset, const float* latent0,
+                                const float* belief0, const float* actions, const float* eps, float* totals, LatentArgs* a) {
+  *a = LatentArgs{};
+  a->B = (long long)cfg->population * cfg->particles;
+  a->H = cfg->horizon;
+  a->P = cfg->particles;
+  a->latent0 = latent0;
+  a->belief0 = belief0;
+  a->act = actions;
+  a->eps = eps;
+  a->sample = 1;  // evaluate_action_sequences steps with sample=True (model_env.py:182-184)
+  a->seed = rng_key(cfg->seed, offset);
+  a->offset = offset;
+  a->totals = totals;
+}
+
+extern "C" {
+
+int b200pets_latent_model_create(const b200pets_latent_model_desc* desc, const float* const* params, void* stream,
+                                 b200pets_latent_model_t* out) {
+  if (!desc || !out) return b200pets_set_error(B200PETS_EINVAL, "latent_model_create: null argument");
+  { int rc = latent_check_params(params, "latent_model_create"); if (rc) return rc; }
+  const b200pets_latent_model_desc& d = *desc;
+  if (d.action_size < 1 || d.latent_size < 1 || d.belief_size < 1 || d.hidden_size < 1)
+    return b200pets_set_error(B200PETS_EINVAL, "latent_model_create: sizes must be positive (action %d, latent %d, belief %d, "
+                                               "hidden %d)", d.action_size, d.latent_size, d.belief_size, d.hidden_size);
+  LatentDev v{};
+  v.A = d.action_size; v.L = d.latent_size; v.Hb = d.belief_size; v.Hf = d.hidden_size;
+  v.A4 = round_up(v.A, 4); v.L4 = round_up(v.L, 4); v.Hb4 = round_up(v.Hb, 4); v.Hf4 = round_up(v.Hf, 4);
+  v.min_std = d.min_std;
+  LatentPlan plan;
+  { int rc = latent_plan(v, 1, &plan); if (rc) return rc; }
+  b200pets_latent_model_s* mdl = new (std::nothrow) b200pets_latent_model_s;
+  if (!mdl) return b200pets_set_error(B200PETS_ENOMEM, "latent_model_create: out of host memory");
+  mdl->desc = d;
+  const size_t bytes = latent_blob_floats(v) * sizeof(float);
+  cudaError_t e = cudaMalloc(&mdl->blob, bytes);
+  if (e != cudaSuccess) {
+    delete mdl;
+    return b200pets_set_error(B200PETS_ECUDA, "cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e));
+  }
+  latent_bind(&v, mdl->blob);
+  mdl->dev = v;
+  int rc = latent_stage(mdl->dev, params, (cudaStream_t)stream);
+  if (rc) {
+    cudaFree(mdl->blob);
+    delete mdl;
+    return rc;
+  }
+  *out = mdl;
+  return B200PETS_OK;
+}
+
+int b200pets_latent_model_refresh(b200pets_latent_model_t model, const float* const* params, void* stream) {
+  if (!model) return b200pets_set_error(B200PETS_EINVAL, "latent_model_refresh: null model");
+  { int rc = latent_check_params(params, "latent_model_refresh"); if (rc) return rc; }
+  return latent_stage(model->dev, params, (cudaStream_t)stream);
+}
+
+void b200pets_latent_model_destroy(b200pets_latent_model_t model) {
+  if (!model) return;
+  cudaFree(model->blob);
+  delete model;
+}
+
+int b200pets_latent_plan_info(b200pets_latent_model_t model, int64_t rows, int32_t info[4]) {
+  if (!model || !info) return b200pets_set_error(B200PETS_EINVAL, "latent_plan_info: null argument");
+  if (rows < 1) return b200pets_set_error(B200PETS_EINVAL, "latent_plan_info: rows %lld < 1", (long long)rows);
+  LatentPlan p;
+  { int rc = latent_plan(model->dev, rows, &p); if (rc) return rc; }
+  info[0] = p.rows;
+  info[1] = (int32_t)p.ctas;
+  info[2] = (int32_t)p.smem;
+  info[3] = (int32_t)p.row_bytes;
+  return B200PETS_OK;
+}
+
+int b200pets_latent_step(b200pets_latent_model_t model, int64_t batch, const float* latent, const float* belief,
+                         const float* act, const float* eps, uint64_t seed, uint64_t offset, int32_t sample,
+                         float* next_latent, float* next_belief, float* reward, void* stream) {
+  if (!model || !latent || !belief || !act) return b200pets_set_error(B200PETS_EINVAL, "latent_step: null argument");
+  if (batch < 1) return b200pets_set_error(B200PETS_EINVAL, "latent_step: empty batch");
+  LatentArgs a{};
+  a.B = batch; a.H = 1; a.P = 1;
+  a.latent_in = latent; a.belief_in = belief; a.act = act;
+  a.eps = eps; a.sample = sample ? 1 : 0;
+  a.seed = rng_key(seed, offset); a.offset = offset;
+  a.latent_out = next_latent; a.belief_out = next_belief; a.reward_out = reward;
+  return launch_latent_rollout(model->dev, a, (cudaStream_t)stream);
+}
+
+size_t b200pets_latent_eval_workspace_bytes(b200pets_latent_model_t model, const b200pets_rollout_cfg* cfg) {
+  if (!model || !cfg) return 0;
+  return al256((size_t)cfg->population * cfg->particles * sizeof(float));
+}
+
+int b200pets_latent_eval_sequences(b200pets_latent_model_t model, const b200pets_rollout_cfg* cfg, const float* latent0,
+                                   const float* belief0, const float* actions, const float* eps, float* returns,
+                                   float* row_returns, void* workspace, size_t workspace_bytes, void* stream_) {
+  if (!model || !cfg || !latent0 || !belief0 || !actions || !returns || !workspace)
+    return b200pets_set_error(B200PETS_EINVAL, "latent_eval_sequences: null argument");
+  { int rc = latent_check_cfg(cfg, "latent_eval_sequences"); if (rc) return rc; }
+  if (workspace_bytes < b200pets_latent_eval_workspace_bytes(model, cfg))
+    return b200pets_set_error(B200PETS_EINVAL, "latent_eval_sequences: workspace too small");
+  cudaStream_t stream = (cudaStream_t)stream_;
+  float* totals = row_returns ? row_returns : reinterpret_cast<float*>(workspace);
+  LatentArgs a;
+  latent_rollout_args(cfg, cfg->offset, latent0, belief0, actions, eps, totals, &a);
+  int rc = launch_latent_rollout(model->dev, a, stream);
+  if (rc) return rc;
+  return launch_particle_mean(cfg->population, cfg->particles, totals, returns, stream);  // model_env.py:190-191
+}
+
+size_t b200pets_latent_cem_plan_workspace_bytes(b200pets_latent_model_t model, const b200pets_rollout_cfg* rcfg,
+                                                const b200pets_cem_cfg* ccfg) {
+  if (!model || !rcfg || !ccfg) return 0;
+  const size_t N = rcfg->population, dims = (size_t)rcfg->horizon * model->desc.action_size;
+  return al256(N * dims * 4) + al256(N * 4) + 3 * al256(dims * 4) + 256 +
+         al256(b200pets_cem_update_workspace_bytes((int)N, (int)dims, ccfg->elite_num)) +
+         b200pets_latent_eval_workspace_bytes(model, rcfg);
+}
+
+// b200pets_cem_plan with the latent rollout: the same launches, offsets and buffers around a different model
+int b200pets_latent_cem_plan(b200pets_latent_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg,
+                             const float* latent0, const float* belief0, const float* x0, const float* lower,
+                             const float* upper, const float* z, const float* eps, float* solution, float* values_out,
+                             void* workspace, size_t workspace_bytes, void* stream_) {
+  if (!model || !rcfg || !ccfg || !latent0 || !belief0 || !x0 || !lower || !upper || !solution || !workspace)
+    return b200pets_set_error(B200PETS_EINVAL, "latent_cem_plan: null argument");
+  { int rc = latent_check_cfg(rcfg, "latent_cem_plan"); if (rc) return rc; }
+  if (ccfg->num_iterations < 0 || ccfg->elite_num < 1 || ccfg->elite_num > rcfg->population)
+    return b200pets_set_error(B200PETS_EINVAL, "latent_cem_plan: %d iterations, %d elites of %d", ccfg->num_iterations,
+                              ccfg->elite_num, rcfg->population);
+  if (workspace_bytes < b200pets_latent_cem_plan_workspace_bytes(model, rcfg, ccfg))
+    return b200pets_set_error(B200PETS_EINVAL, "latent_cem_plan: workspace too small");
+  cudaStream_t stream = (cudaStream_t)stream_;
+  const int N = rcfg->population, H = rcfg->horizon, P = rcfg->particles, L = model->desc.latent_size;
+  const int dims = H * model->desc.action_size;
+  const long long B = (long long)N * P;
+  unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
+  float* pop = reinterpret_cast<float*>(ws); ws += al256((size_t)N * dims * 4);
+  float* values = reinterpret_cast<float*>(ws); ws += al256((size_t)N * 4);
+  float* mu = reinterpret_cast<float*>(ws); ws += al256((size_t)dims * 4);
+  float* disp = reinterpret_cast<float*>(ws); ws += al256((size_t)dims * 4);
+  float* best_sol = reinterpret_cast<float*>(ws); ws += al256((size_t)dims * 4);
+  float* best_val = reinterpret_cast<float*>(ws); ws += 256;
+  void* upd_ws = ws; const size_t upd_bytes = al256(b200pets_cem_update_workspace_bytes(N, dims, ccfg->elite_num)); ws += upd_bytes;
+  float* totals = reinterpret_cast<float*>(ws);
+
+  cem_init_kernel<<<(dims + 255) / 256, 256, 0, stream>>>(dims, x0, lower, upper, ccfg->clipped_normal, mu, disp, best_val);
+  CUDA_TRY(cudaGetLastError());
+  const bool merged = cem_refit_sample_supported(N, dims, ccfg->elite_num);
+  unsigned int* refit_flag = reinterpret_cast<unsigned int*>(best_val + 2);
+  auto next_pop = [&](int it_next, int refit, const float* rows) -> int {  // refit of it_next - 1 (if any) + population of it_next
+    const int sample = it_next < ccfg->num_iterations;
+    const unsigned long long off = rcfg->offset * 1024 + (unsigned long long)it_next;
+    return launch_cem_refit_sample(N, dims, ccfg->elite_num, ccfg->alpha, ccfg->clipped_normal, rows, P, values, mu, disp,
+                                   best_val, best_sol, upd_ws, upd_bytes, refit, sample, lower, upper,
+                                   (z && sample) ? z + (size_t)it_next * N * dims : nullptr, rng_key(rcfg->seed, off), off,
+                                   ccfg->clipped_normal, 0, refit_flag, (unsigned int)it_next, pop, stream);
+  };
+  if (merged) {
+    int rc0 = next_pop(0, 0, nullptr);
+    if (rc0) return rc0;
+  }
+  for (int it = 0; it < ccfg->num_iterations; ++it) {
+    const unsigned long long off = rcfg->offset * 1024 + it;
+    if (!merged) {
+      int rcs = b200pets_cem_sample_shard(N, 0, dims, mu, disp, lower, upper, z ? z + (size_t)it * N * dims : nullptr,
+                                          rcfg->seed, off, ccfg->clipped_normal, pop, stream);
+      if (rcs) return rcs;
+    }
+    LatentArgs a;
+    latent_rollout_args(rcfg, off, latent0, belief0, pop, eps ? eps + (size_t)it * H * B * L : nullptr, totals, &a);
+    int rc = launch_latent_rollout(model->dev, a, stream);
+    if (rc) return rc;
+    if (merged)
+      rc = next_pop(it + 1, 1, totals);
+    else  // particle mean + NaN rule + top-k + refit in one kernel
+      rc = launch_cem_update_rows(N, dims, ccfg->elite_num, ccfg->alpha, 1, ccfg->clipped_normal, pop, totals, P, values, mu,
+                                  disp, best_val, best_sol, upd_ws, upd_bytes, stream);
+    if (rc) return rc;
+    // values_out holds the values after the reference's in-place NaN rule (trajectory_opt.py:178), as b200pets_cem_plan's
+    if (values_out) CUDA_TRY(cudaMemcpyAsync(values_out + (size_t)it * N, values, sizeof(float) * N, cudaMemcpyDeviceToDevice, stream));
+  }
+  CUDA_TRY(cudaMemcpyAsync(solution, ccfg->return_mean_elites ? mu : best_sol, sizeof(float) * dims, cudaMemcpyDeviceToDevice, stream));
+  return B200PETS_OK;
 }
 
 }  // extern "C"

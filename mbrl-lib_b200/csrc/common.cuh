@@ -147,6 +147,9 @@ __device__ __forceinline__ void philox_normal4(uint32_t c0, uint32_t c1, uint32_
 #define RNG_STREAM_CEM 0x30000u
 #define RNG_STREAM_ICEM 0x40000u
 #define RNG_STREAM_PERM 0x50000u
+// latent.cu, the prior's draw of latent element j of row r at step t: philox_normal4(r, t, RNG_STREAM_LATENT | (j >> 2),
+// offset, rng_key(seed, offset)), lane j & 3 (r: row of the call, n * P + p; t: step of the call, 0 for one step)
+#define RNG_STREAM_LATENT 0x60000u
 
 // ------------------------------------------------------------------------------------------------------
 // small math

@@ -3,6 +3,7 @@
 Drop-in: same constructor ``(env, model, termination_fn, reward_fn=None, generator=None)``, same
 ``reset`` / ``step`` / ``evaluate_action_sequences`` signatures, shapes, return types and error behaviour.
 Extra keyword-only knobs choose the arithmetic (``precision``) and how TS1 draws members (``ts1``).
+Constructed over a PlaNet latent model, it returns the latent environment of :mod:`mbrl_lib_b200.latent`.
 """
 from __future__ import annotations
 
@@ -17,6 +18,16 @@ from .staging import StagedModel
 
 
 class ModelEnv:
+    def __new__(cls, env=None, model=None, *args, **kwargs):
+        """A PlaNet latent model (``belief_model``, ``prior_transition_model``, ``reward_model``) gets the latent
+        environment, :class:`mbrl_lib_b200.latent.LatentModelEnv`; every other model this class."""
+        if cls is ModelEnv and model is not None:
+            from .latent import LatentModelEnv, is_latent_model
+
+            if is_latent_model(model):
+                return super().__new__(LatentModelEnv)
+        return super().__new__(cls)
+
     def __init__(self, env, model, termination_fn, reward_fn=None, generator: Optional[torch.Generator] = None, *,
                  precision: str = "auto", ts1: str = "tile_shuffle"):
         self.dynamics_model = model

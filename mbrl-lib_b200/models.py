@@ -228,3 +228,55 @@ def model_from_arrays(spec, arrays, device) -> OneDTransitionRewardModel:
     if spec.elites is not None:
         wrapper.set_elite(list(spec.elites))
     return wrapper
+
+
+class _BeliefModel(nn.Module):  # mbrl/models/planet.py:82-101
+    def __init__(self, latent_state_size: int, action_size: int, belief_size: int):
+        super().__init__()
+        self.embedding_layer = nn.Sequential(nn.Linear(latent_state_size + action_size, belief_size), nn.ReLU())
+        self.rnn = nn.GRUCell(belief_size, belief_size)
+
+
+class PlaNetModel(nn.Module):
+    """The planning half of mbrl-lib's ``PlaNetModel`` (planet.py:121-306) with its attribute layout:
+    ``belief_model.{embedding_layer, rnn}``, ``prior_transition_model[0, 2]``, ``reward_model[0, 2, 4]``, ``min_std``
+    and the posterior ``_current_posterior_sample [1, L]`` / ``_current_belief [1, Hb]`` that planning starts from.
+    The conv encoder / decoder and the posterior model are not here: :meth:`set_posterior` stands in for
+    ``update_posterior``.  Weights start as torch's default initialisation unless ``seed`` is given, in which case
+    every parameter is drawn from N(0, scale^2) with that numpy seed, in the order of ``latent.latent_params``."""
+
+    def __init__(self, action_size: int, latent_state_size: int = 30, belief_size: int = 200, hidden_size_fcs: int = 200,
+                 device="cpu", min_std: float = 0.1, seed: Optional[int] = None, scale: float = 0.1):
+        super().__init__()
+        self.action_size, self.latent_state_size, self.belief_size = action_size, latent_state_size, belief_size
+        self.min_std = min_std
+        self.device = torch.device(device)
+        self.belief_model = _BeliefModel(latent_state_size, action_size, belief_size)
+        self.prior_transition_model = nn.Sequential(nn.Linear(belief_size, hidden_size_fcs), nn.ReLU(),
+                                                    nn.Linear(hidden_size_fcs, 2 * latent_state_size))
+        self.reward_model = nn.Sequential(nn.Linear(belief_size + latent_state_size, hidden_size_fcs), nn.ReLU(),
+                                          nn.Linear(hidden_size_fcs, hidden_size_fcs), nn.ReLU(),
+                                          nn.Linear(hidden_size_fcs, 1))
+        if seed is not None:
+            from .latent import latent_params
+
+            rng = np.random.default_rng(seed)
+            with torch.no_grad():
+                for p in latent_params(self):
+                    p.copy_(torch.from_numpy(rng.normal(0.0, scale, tuple(p.shape)).astype(np.float32)))
+        self._current_posterior_sample: Optional[torch.Tensor] = None
+        self._current_belief: Optional[torch.Tensor] = None
+        self.to(self.device)
+
+    def set_posterior(self, latent, belief):
+        """Set the state planning starts from: ``latent [L]`` / ``belief [Hb]`` (or ``[1, .]``)."""
+        self._current_posterior_sample = torch.as_tensor(latent, dtype=torch.float32).reshape(1, -1).to(self.device)
+        self._current_belief = torch.as_tensor(belief, dtype=torch.float32).reshape(1, -1).to(self.device)
+
+    def reset_posterior(self):
+        self._current_posterior_sample = None
+        self._current_belief = None
+
+    def reset(self, obs, rng=None):  # planet.py:662-677
+        return {"latent": self._current_posterior_sample.repeat(obs.shape[0], 1),
+                "belief": self._current_belief.repeat(obs.shape[0], 1)}

@@ -10,6 +10,8 @@
   C call (``b200pets_cem_plan``): every iteration's sample -> rollout -> refit is enqueued back to back.
   With a reward or termination callable the kernels do not know it runs the per-iteration loop instead, the
   objective applying the callable to windows of the rollout (``ModelEnv.evaluate_action_sequences``).
+* Over PlaNet's latent model (:class:`mbrl_lib_b200.latent.LatentModelEnv`) the fused plan is one
+  ``b200pets_latent_cem_plan`` call; iCEM and MPPI evaluate through its ``evaluate_action_sequences``.
 * ``TrajectoryOptimizer`` / ``TrajectoryOptimizerAgent`` / ``create_trajectory_optim_agent_for_model``:
   reference semantics (warm-start shift, action cache, RuntimeError when the eval fn is unset).
 """
@@ -226,6 +228,8 @@ class CEMOptimizer(Optimizer):
 
     def _optimize_fused(self, obj: _FusedObjective, x0, noise, model_noise) -> torch.Tensor:
         env = obj.model_env
+        if getattr(env, "is_latent", False):  # PlaNet's latent model: b200pets_latent_cem_plan, model noise = eps only
+            return env.cem_plan(self, x0, obj.num_particles, noise, None if model_noise is None else model_noise[1])
         env._fresh()
         H, A = x0.shape
         prop = env._propagation()
@@ -652,6 +656,9 @@ class TrajectoryOptimizerAgent(Agent):
         :meth:`reset_batch` restores them."""
         if self.trajectory_eval_fn is None:
             raise RuntimeError("Please call `set_trajectory_eval_fn()` before using TrajectoryOptimizerAgent")
+        if getattr(self._fused_env, "is_latent", False):
+            raise NotImplementedError("act_batch plans for K observations, but a latent model holds one posterior: call "
+                                      "act once per observation after update_posterior")
         obs = np.asarray(obs)
         K = obs.shape[0]
         if self._batch_actions and self._batch_actions[0].shape[0] != K:
