@@ -547,6 +547,54 @@ size_t b200pets_eval_score_workspace_bytes(b200pets_trainer_t trainer, int64_t r
 int b200pets_eval_score(b200pets_trainer_t trainer, int64_t rows, const float* inputs, const float* targets, float* scores,
                         void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- Training MBPO's SAC agent (mbrl/third_party/pytorch_sac_pranz24/sac.py) ----------------------------------------
+ * An agent: the caller's live tensors, updated in place by b200pets_sac_update; nothing is copied.
+ *   params      [host array of 20 dev pointers] the critic's 12 parameters in QNetwork.parameters() order (linear1.weight,
+ *               linear1.bias, .., linear6.bias), then the policy's 8 in GaussianPolicy.parameters() order (linear1,
+ *               linear2, mean_linear, log_std_linear; weight, bias).  Weights are nn.Linear's float[out][in].
+ *   target_params [12] critic_target's parameters, in the critic's order
+ *   exp_avg, exp_avg_sq [20] the Adam moments of params, same order (critic_optim's, then policy_optim's)
+ *   log_alpha, log_alpha_exp_avg, log_alpha_exp_avg_sq [dev] float[1]: read only with automatic_entropy_tuning (may be
+ *               NULL otherwise)
+ * Refused: NULL pointers, non-positive sizes, act_dim > 32 (the policy heads' row-wise phase holds a row's actions in
+ * one 32-column tile: B200PETS_EUNSUPPORTED), target_update_interval < 1. */
+#define B200PETS_SAC_MAX_ACTIONS 32
+#define B200PETS_SAC_NUM_PARAMS 20
+#define B200PETS_SAC_NUM_CRITIC_PARAMS 12
+typedef struct b200pets_sac_s* b200pets_sac_t;
+typedef struct {
+  int32_t obs_dim, act_dim, hidden;
+  float action_scale[B200PETS_SAC_MAX_ACTIONS], action_bias[B200PETS_SAC_MAX_ACTIONS]; /* first act_dim entries */
+  double gamma, tau, lr, beta1, beta2, eps; /* one lr and one set of betas for the three optimizers, no weight decay */
+  int32_t automatic_entropy_tuning;
+  float target_entropy;
+  int32_t target_update_interval;
+} b200pets_sac_desc;
+int b200pets_sac_supported(const b200pets_sac_desc* desc);
+int b200pets_sac_create(const b200pets_sac_desc* desc, float* const* params, float* const* target_params,
+                        float* const* exp_avg, float* const* exp_avg_sq, float* log_alpha, float* log_alpha_exp_avg,
+                        float* log_alpha_exp_avg_sq, b200pets_sac_t* out);
+void b200pets_sac_destroy(b200pets_sac_t sac);
+
+/* One SAC.update_parameters (sac.py:76-173) after its memory.sample, enqueued on `stream` as one launch, with no host
+ * synchronisation: the critic step, the policy step against the updated critic, the temperature step (with
+ * automatic_entropy_tuning) and, when updates % target_update_interval == 0, the soft target update.
+ *   updates       the reference's `updates` argument (>= 0)
+ *   reverse_mask  nonzero: the target's mask is 1 - terminated (as MBPO calls it), else terminated
+ *   adam_steps    [host] int64[3]: the step counts of critic_optim, policy_optim and alpha_optim before this update
+ *   transitions   [dev] float[batch][2 * obs_dim + act_dim + 2]: s, a, s', r, terminated (0 or 1)
+ *   eps           [dev] float[2][batch][act_dim]: the reparameterisation draws on s' and on s, or NULL for the in-kernel
+ *                 Philox draws keyed by (seed, offset) (RNG_STREAM_SAC in csrc/common.cuh)
+ *   alpha         [dev] float[1]: the temperature this update uses; written with exp(log_alpha) when tuning
+ *   stats         [dev] float[8]: qf1 loss, qf2 loss, policy loss, alpha loss, alpha after the update, the batch's mean
+ *                 reward, -mean(log pi), 0
+ * Refused: NULL pointers, batch < 1, updates < 0, a workspace smaller than b200pets_sac_workspace_bytes(sac, batch). */
+size_t b200pets_sac_workspace_bytes(b200pets_sac_t sac, int32_t batch);
+int b200pets_sac_update(b200pets_sac_t sac, int32_t batch, int64_t updates, int32_t reverse_mask,
+                        const int64_t* adam_steps, const float* transitions, const float* eps, uint64_t seed,
+                        uint64_t offset, float* alpha, float* stats, void* workspace, size_t workspace_bytes,
+                        void* stream);
+
 /* Self test of the wgmma building block: D[128][n] = A[128][k] * B[n][k]^T with bf16 operands staged in the
  * no-swizzle canonical layouts, the weight ring and the accumulator fragments the rollout kernel uses.  a, b [dev] float
  * (rounded to bf16 inside), d [dev] float[128][n].  k, n multiples of 16, <= 256.  A negative k writes A as bf16 pairs

@@ -12,7 +12,7 @@ _LAZY = {
     "create_trajectory_optim_agent_for_model": "planning", "complete_agent_cfg": "planning", "rollout_model_env": "planning",
     "GaussianMLP": "models", "OneDTransitionRewardModel": "models", "EnsembleLinearLayer": "models",
     "Normalizer": "models", "model_from_arrays": "models", "PlaNetModel": "models", "ModelTrainer": "trainer",
-    "TransitionBatch": "replay", "TransitionIterator": "replay", "BootstrapIterator": "replay",
+    "TransitionBatch": "replay", "TransitionIterator": "replay", "BootstrapIterator": "replay", "SAC": "sac",
 }
 
 
@@ -22,6 +22,6 @@ def __getattr__(name):
     if name in _LAZY:
         return getattr(importlib.import_module(f"{__name__}.{_LAZY[name]}"), name)
     if name in ("synthetic", "functions", "planning", "models", "model_env", "staging", "_lib", "build", "dist", "mbpo",
-                "trainer", "replay", "latent"):
+                "trainer", "replay", "latent", "sac"):
         return importlib.import_module(f"{__name__}.{name}")
     raise AttributeError(name)

@@ -66,6 +66,18 @@ class TrainDesc(C.Structure):
                [(n, C.c_double) for n in ("lr", "beta1", "beta2", "eps", "weight_decay")]
 
 
+SAC_MAX_ACTIONS = 32
+SAC_NUM_PARAMS, SAC_NUM_CRITIC_PARAMS = 20, 12
+
+
+class SacDesc(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("obs_dim", "act_dim", "hidden")] + \
+               [("action_scale", C.c_float * SAC_MAX_ACTIONS), ("action_bias", C.c_float * SAC_MAX_ACTIONS)] + \
+               [(n, C.c_double) for n in ("gamma", "tau", "lr", "beta1", "beta2", "eps")] + \
+               [("automatic_entropy_tuning", C.c_int32), ("target_entropy", C.c_float),
+                ("target_update_interval", C.c_int32)]
+
+
 _P = C.c_void_p
 _SIGNATURES = {
     "b200pets_version": (C.c_int, []),
@@ -153,6 +165,13 @@ _SIGNATURES = {
                                        C.c_size_t, _P]),
     "b200pets_eval_score_workspace_bytes": (C.c_size_t, [_P, C.c_int64]),
     "b200pets_eval_score": (C.c_int, [_P, C.c_int64, _P, _P, _P, _P, C.c_size_t, _P]),
+    "b200pets_sac_supported": (C.c_int, [C.POINTER(SacDesc)]),
+    "b200pets_sac_create": (C.c_int, [C.POINTER(SacDesc), C.POINTER(_P), C.POINTER(_P), C.POINTER(_P), C.POINTER(_P), _P, _P,
+                                      _P, C.POINTER(_P)]),
+    "b200pets_sac_destroy": (None, [_P]),
+    "b200pets_sac_workspace_bytes": (C.c_size_t, [_P, C.c_int32]),
+    "b200pets_sac_update": (C.c_int, [_P, C.c_int32, C.c_int64, C.c_int32, C.POINTER(C.c_int64), _P, _P, C.c_uint64,
+                                      C.c_uint64, _P, _P, _P, C.c_size_t, _P]),
 }
 
 _lib = None

@@ -10,6 +10,7 @@
 
 #include "common.cuh"
 #include "latent.cuh"
+#include "sac.cuh"
 #include "train.cuh"
 
 // launchers defined in the kernel translation units
@@ -1134,6 +1135,108 @@ int b200pets_eval_score(b200pets_trainer_t trainer, int64_t rows, const float* i
   if (workspace_bytes < need)
     return b200pets_set_error(B200PETS_EINVAL, "eval_score: workspace of %zu bytes, %zu needed", workspace_bytes, need);
   return launch_eval_score(trainer->dev, rows, inputs, targets, scores, workspace, (cudaStream_t)stream);
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// MBPO's SAC agent (sac.cu)
+// ---------------------------------------------------------------------------------------------------------
+struct b200pets_sac_s {
+  SacDev dev;
+  int interval;
+};
+
+// The descriptor checks of b200pets_sac_create, and the sizes and hyper-parameters of its SacDev (no pointers).
+static int sac_desc_to_dev(const b200pets_sac_desc& d, const char* who, SacDev* out) {
+  if (d.obs_dim < 1 || d.act_dim < 1 || d.hidden < 1)
+    return b200pets_set_error(B200PETS_EINVAL, "%s: non-positive size (obs_dim %d, act_dim %d, hidden %d)", who, d.obs_dim,
+                              d.act_dim, d.hidden);
+  if (d.act_dim > SAC_MAX_ACTIONS)
+    return b200pets_set_error(B200PETS_EUNSUPPORTED,
+                              "%s: act_dim %d > %d (the policy heads' row-wise phase holds a row's actions in one tile)", who,
+                              d.act_dim, SAC_MAX_ACTIONS);
+  if (d.target_update_interval < 1)
+    return b200pets_set_error(B200PETS_EINVAL, "%s: target_update_interval %d < 1", who, d.target_update_interval);
+  SacDev v{};
+  v.D = d.obs_dim; v.A = d.act_dim; v.H = d.hidden;
+  for (int j = 0; j < d.act_dim; ++j) { v.scale[j] = d.action_scale[j]; v.bias[j] = d.action_bias[j]; }
+  v.gamma = (float)d.gamma;
+  v.one_minus_tau = (float)(1.0 - d.tau);
+  v.tau = (float)d.tau;
+  v.target_entropy = d.target_entropy;
+  v.tuning = d.automatic_entropy_tuning ? 1 : 0;
+  v.lr = d.lr; v.beta1 = d.beta1; v.beta2 = d.beta2; v.eps = d.eps;
+  *out = v;
+  return B200PETS_OK;
+}
+
+int b200pets_sac_supported(const b200pets_sac_desc* desc) {
+  if (!desc) return b200pets_set_error(B200PETS_EINVAL, "sac_supported: NULL pointer");
+  SacDev v;
+  return sac_desc_to_dev(*desc, "sac_supported", &v);
+}
+
+int b200pets_sac_create(const b200pets_sac_desc* desc, float* const* params, float* const* target_params,
+                        float* const* exp_avg, float* const* exp_avg_sq, float* log_alpha, float* log_alpha_exp_avg,
+                        float* log_alpha_exp_avg_sq, b200pets_sac_t* out) {
+  if (!desc || !params || !target_params || !exp_avg || !exp_avg_sq || !out)
+    return b200pets_set_error(B200PETS_EINVAL, "sac_create: NULL pointer");
+  SacDev v;
+  if (const int rc = sac_desc_to_dev(*desc, "sac_create", &v)) return rc;
+  for (int i = 0; i < B200PETS_SAC_NUM_PARAMS; ++i)
+    if (!params[i] || !exp_avg[i] || !exp_avg_sq[i])
+      return b200pets_set_error(B200PETS_EINVAL, "sac_create: NULL parameter or moment %d", i);
+  for (int i = 0; i < SAC_CRITIC_PARAMS; ++i) {
+    if (!target_params[i]) return b200pets_set_error(B200PETS_EINVAL, "sac_create: NULL target parameter %d", i);
+    v.cp[i] = params[i]; v.cm[i] = exp_avg[i]; v.cv[i] = exp_avg_sq[i]; v.ct[i] = target_params[i];
+  }
+  for (int i = 0; i < SAC_POLICY_PARAMS; ++i) {
+    const int k = SAC_CRITIC_PARAMS + i;
+    v.pp[i] = params[k]; v.pm[i] = exp_avg[k]; v.pv[i] = exp_avg_sq[k];
+  }
+  if (v.tuning) {
+    if (!log_alpha || !log_alpha_exp_avg || !log_alpha_exp_avg_sq)
+      return b200pets_set_error(B200PETS_EINVAL, "sac_create: NULL log_alpha or moment with automatic entropy tuning");
+    v.log_alpha = log_alpha; v.la_m = log_alpha_exp_avg; v.la_v = log_alpha_exp_avg_sq;
+  }
+  b200pets_sac_s* s = new (std::nothrow) b200pets_sac_s;
+  if (!s) return b200pets_set_error(B200PETS_ENOMEM, "sac_create: out of host memory");
+  s->dev = v;
+  s->interval = desc->target_update_interval;
+  *out = s;
+  return B200PETS_OK;
+}
+
+void b200pets_sac_destroy(b200pets_sac_t sac) { delete sac; }
+
+size_t b200pets_sac_workspace_bytes(b200pets_sac_t sac, int32_t batch) {
+  if (!sac || batch < 1) return 0;
+  return sac_workspace_floats(sac->dev, batch) * sizeof(float);
+}
+
+int b200pets_sac_update(b200pets_sac_t sac, int32_t batch, int64_t updates, int32_t reverse_mask,
+                        const int64_t* adam_steps, const float* transitions, const float* eps, uint64_t seed,
+                        uint64_t offset, float* alpha, float* stats, void* workspace, size_t workspace_bytes,
+                        void* stream) {
+  if (!sac || !adam_steps || !transitions || !alpha || !stats || !workspace)
+    return b200pets_set_error(B200PETS_EINVAL, "sac_update: NULL pointer");
+  if (batch < 1 || updates < 0 || adam_steps[0] < 0 || adam_steps[1] < 0 || adam_steps[2] < 0)
+    return b200pets_set_error(B200PETS_EINVAL, "sac_update: bad sizes (batch %d, updates %lld)", batch, (long long)updates);
+  const size_t need = b200pets_sac_workspace_bytes(sac, batch);
+  if (workspace_bytes < need)
+    return b200pets_set_error(B200PETS_EINVAL, "sac_update: workspace of %zu bytes, %zu needed", workspace_bytes, need);
+  SacArgs a{};
+  a.B = batch;
+  a.reverse_mask = reverse_mask ? 1 : 0;
+  a.soft_update = updates % sac->interval == 0 ? 1 : 0;
+  a.trans = transitions;
+  a.eps = eps;
+  a.seed = rng_key(seed, offset);
+  a.offset = offset;
+  a.step_c = adam_steps[0]; a.step_p = adam_steps[1]; a.step_a = adam_steps[2];
+  a.alpha = alpha;
+  a.stats = stats;
+  a.ws = (float*)workspace;
+  return launch_sac_update(sac->dev, a, (cudaStream_t)stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------

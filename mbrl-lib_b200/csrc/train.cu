@@ -40,6 +40,7 @@
 //   p  = p + (-(lr / (1 - beta1^t))) * (m / (sqrt(v) / sqrt(1 - beta2^t) + eps))
 #include <cooperative_groups.h>
 
+#include "adam.cuh"
 #include "train.cuh"
 
 namespace cg = cooperative_groups;
@@ -129,35 +130,8 @@ __device__ __forceinline__ float activation_grad(float g, float z, int act, floa
   return z > 0.0f ? g : g * slope;
 }
 
-struct AdamStep {
-  float wd, omb1, b2, omb2, eps, bc2_sqrt, step_size;
-};
-
 __device__ __forceinline__ AdamStep adam_scalars(const TrainDev& m, long long t) {
-  AdamStep s;
-  s.wd = (float)m.weight_decay;
-  s.omb1 = (float)(1.0 - m.beta1);
-  s.b2 = (float)m.beta2;
-  s.omb2 = (float)(1.0 - m.beta2);
-  s.eps = (float)m.eps;
-  const double bc1 = 1.0 - pow(m.beta1, (double)t), bc2 = 1.0 - pow(m.beta2, (double)t);
-  s.step_size = (float)(-(m.lr / bc1));
-  s.bc2_sqrt = (float)sqrt(bc2);
-  return s;
-}
-
-__device__ __forceinline__ void adam_update(float* p, float* mo, float* vo, float g, const AdamStep& s) {
-  float pv = *p;
-  if (s.wd != 0.0f) g = g + s.wd * pv;
-  float mv = *mo;
-  mv = mv + s.omb1 * (g - mv);
-  float vv = *vo * s.b2;
-  vv = vv + s.omb2 * g * g;
-  const float den = sqrtf(vv) / s.bc2_sqrt + s.eps;
-  pv = pv + s.step_size * (mv / den);
-  *p = pv;
-  *mo = mv;
-  *vo = vv;
+  return ::adam_scalars(m.lr, m.beta1, m.beta2, m.weight_decay, m.eps, t);
 }
 
 // Workspace of train_adam_kernel, offsets in floats.  Hidden layer l owns three consecutive [E][Bm][hid] blocks (Z, A,
