@@ -472,6 +472,73 @@ int b200pets_latent_cem_plan(b200pets_latent_model_t model, const b200pets_rollo
                              const float* upper, const float* z, const float* eps, float* solution, float* values_out,
                              void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- Training PlaNet's latent model: the recurrence of PlaNetModel.forward (planet.py:354-404) ------------------
+ * The belief GRU, the posterior and the prior over T steps from s0 = 0, h0 = 0 (planet.py:364-367), in fp32 FFMA:
+ *   e = relu(W_e [s, a_t] + b_e);  h = GRUCell(e, h);
+ *   q = W_q2 relu(W_q1[:, :Hb] h + P_t) + b_q2;  s = q[:L] + (softplus(q[L:]) + min_std) * eps_q;
+ *   p = W_p2 relu(W_p1 h + b_p1) + b_p2;        s_prior = p[:L] + (softplus(p[L:]) + min_std) * eps_p.
+ * P_t = W_q1[:, Hb:] enc_t + b_q1 (the posterior's encoding half) comes in precomputed for every (b, t); the encoder,
+ * the decoder, the reward model and the losses stay with the caller.  The backward pass runs t = T-1 .. 0 and writes
+ * dP and every layer's pre-activation gradient for all (b, t) into the tape: the weight gradients are products of
+ * those with the stored layer inputs over all B x T rows, which the caller forms.  Sums run in a fixed order, so both
+ * calls are bit-identical from run to run. */
+typedef struct {
+  int32_t action_size;    /* A */
+  int32_t latent_size;    /* L */
+  int32_t belief_size;    /* Hb */
+  int32_t hidden_size;    /* Hf */
+  int32_t encoding_size;  /* E, obs_encoding_size */
+  float min_std;
+} b200pets_latent_train_desc;
+
+/* params [host] array of B200PETS_LATENT_TRAIN_NUM_PARAMS device pointers to contiguous fp32 tensors in torch's layout:
+ *    0 W_e [Hb][L+A], 1 b_e [Hb]                                belief_model.embedding_layer[0]
+ *    2 weight_ih [3Hb][Hb], 3 weight_hh [3Hb][Hb], 4 bias_ih [3Hb], 5 bias_hh [3Hb]   belief_model.rnn (gates r, z, n)
+ *    6 W_q1 [Hf][Hb+E] (only the belief columns are read)       posterior_transition_model[0] (input: belief, encoding)
+ *    7 W_q2 [2L][Hf], 8 b_q2 [2L]                               posterior_transition_model[2]
+ *    9 W_p1 [Hf][Hb], 10 b_p1 [Hf]                              prior_transition_model[0]
+ *   11 W_p2 [2L][Hf], 12 b_p2 [2L]                              prior_transition_model[2] */
+#define B200PETS_LATENT_TRAIN_NUM_PARAMS 13
+
+/* What the backward pass needs from the forward pass, and the pre-activation gradients it writes: caller-owned device
+ * arrays, each [B][T][width] fp32 (row b * T + t).  Forward: e [Hb] (the embedding after its ReLU), gates [4Hb]
+ * (r, z, n, W_hn h + b_hn), q1 [Hf] and p1 [Hf] (the posterior's and the prior's hidden layer after its ReLU), pre_std
+ * [2L] (q[L:], then p[L:]), eps [2L] (the posterior's draws, then the prior's).  Backward: de [Hb] (embedding
+ * pre-activation), dgi [3Hb] (GRU input-side pre-activations r, z, n), dghn [Hb] (W_hn h + b_hn), dq [2L] (posterior
+ * layer 2), dv [Hf] (prior layer 1), dp [2L] (prior layer 2).  The hidden-side gradients of r and z equal dgi's, and
+ * the posterior's layer-1 pre-activation gradient is dP. */
+typedef struct {
+  float *e, *gates, *q1, *p1, *pre_std, *eps;
+  float *de, *dgi, *dghn, *dq, *dv, *dp;
+} b200pets_latent_tape;
+
+/* 0 when the kernels cover `desc`, asked before anything is touched.  B200PETS_EINVAL for sizes below 1 or min_std
+ * below 0; B200PETS_EUNSUPPORTED when a row of the forward or the backward kernel needs more than an eighth of the
+ * device's opt-in shared memory per CTA (PlaNet's A 6, L 30, Hb = Hf = 200 needs 7 808 bytes; the limit is 29 056 on an
+ * H100, which admits Hb = Hf up to 788 at A 6, L 30). */
+int b200pets_latent_train_supported(const b200pets_latent_train_desc* desc);
+/* Bytes of the workspace b200pets_latent_seq_forward re-packs the weights into (0 for bad arguments). */
+size_t b200pets_latent_train_workspace_bytes(const b200pets_latent_train_desc* desc, int32_t batch, int32_t steps);
+/* The forward pass (planet.py:370-402 without the decoder and the reward model), one re-pack and one launch:
+ *   P [dev] float[B][T][Hf]; act [dev] float[B][T][A] (action[:, :-1]);
+ *   eps_q, eps_p [dev] float[T][B][L] injected N(0,1) draws (both or neither), or NULL = Philox on RNG_STREAM_LATENT_TRAIN
+ *   with key (seed, offset);
+ *   beliefs [dev] float[B][T][Hb], post_params / prior_params [dev] float[B][T][2L] (mean, then std), post_samples /
+ *   prior_samples [dev] float[B][T][L]: the five stacked outputs of PlaNetModel.forward;
+ *   tape: every forward field set, or NULL when no backward pass follows (no_grad). */
+int b200pets_latent_seq_forward(const b200pets_latent_train_desc* desc, const float* const* params, int32_t batch,
+                                int32_t steps, const float* P, const float* act, const float* eps_q, const float* eps_p,
+                                uint64_t seed, uint64_t offset, float* beliefs, float* post_params, float* post_samples,
+                                float* prior_params, float* prior_samples, const b200pets_latent_tape* tape,
+                                void* workspace, size_t workspace_bytes, void* stream);
+/* The backward pass of the same call, after it on the same weights: the upstream gradients of the five outputs (each
+ * may be NULL = zero), beliefs [dev] as the forward pass wrote them, the tape (every field set) in; dP [dev]
+ * float[B][T][Hf] and the tape's backward fields out.  Reads torch's tensors directly: no workspace. */
+int b200pets_latent_seq_backward(const b200pets_latent_train_desc* desc, const float* const* params, int32_t batch,
+                                 int32_t steps, const float* beliefs, const float* g_beliefs, const float* g_post_params,
+                                 const float* g_post_samples, const float* g_prior_params, const float* g_prior_samples,
+                                 const b200pets_latent_tape* tape, float* dP, void* stream);
+
 /* ---- Training the dynamics model (mbrl/models/model_trainer.py:70-262) ------------------------------------
  * OneDTransitionRewardModel(GaussianMLP) trained with torch.optim.Adam, fp32 throughout. */
 

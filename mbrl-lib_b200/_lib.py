@@ -55,6 +55,18 @@ class LatentDesc(C.Structure):
 LATENT_NUM_PARAMS = 16
 
 
+class LatentTrainDesc(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("action_size", "latent_size", "belief_size", "hidden_size", "encoding_size")] + \
+               [("min_std", C.c_float)]
+
+
+class LatentTape(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("e", "gates", "q1", "p1", "pre_std", "eps", "de", "dgi", "dghn", "dq", "dv", "dp")]
+
+
+LATENT_TRAIN_NUM_PARAMS = 13
+
+
 class PrepDesc(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("obs_dim", "act_dim", "obs_process", "norm_mode", "target_is_delta",
                                          "learned_rewards", "dtype")]
@@ -155,6 +167,13 @@ _SIGNATURES = {
     "b200pets_latent_cem_plan_workspace_bytes": (C.c_size_t, [_P, C.POINTER(RolloutCfg), C.POINTER(CemCfg)]),
     "b200pets_latent_cem_plan": (C.c_int, [_P, C.POINTER(RolloutCfg), C.POINTER(CemCfg), _P, _P, _P, _P, _P, _P, _P, _P, _P,
                                            _P, C.c_size_t, _P]),
+    "b200pets_latent_train_supported": (C.c_int, [C.POINTER(LatentTrainDesc)]),
+    "b200pets_latent_train_workspace_bytes": (C.c_size_t, [C.POINTER(LatentTrainDesc), C.c_int32, C.c_int32]),
+    "b200pets_latent_seq_forward": (C.c_int, [C.POINTER(LatentTrainDesc), C.POINTER(_P), C.c_int32, C.c_int32, _P, _P, _P, _P,
+                                              C.c_uint64, C.c_uint64, _P, _P, _P, _P, _P, C.POINTER(LatentTape), _P,
+                                              C.c_size_t, _P]),
+    "b200pets_latent_seq_backward": (C.c_int, [C.POINTER(LatentTrainDesc), C.POINTER(_P), C.c_int32, C.c_int32, _P, _P, _P,
+                                               _P, _P, _P, C.POINTER(LatentTape), _P, _P]),
     "b200pets_train_preprocess": (C.c_int, [C.POINTER(PrepDesc), C.c_int64, _P, _P, _P, _P, _P, _P, C.POINTER(C.c_int32),
                                             C.c_int32, _P, _P, _P]),
     "b200pets_trainer_create": (C.c_int, [C.POINTER(TrainDesc), C.POINTER(_P), C.POINTER(_P), C.POINTER(_P), C.POINTER(_P)]),

@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200pets.so")
-SOURCES = ["api.cu", "rollout_f32.cu", "rollout_tc.cu", "cem.cu", "mbpo.cu", "train.cu", "latent.cu", "sac.cu"]
+SOURCES = ["api.cu", "rollout_f32.cu", "rollout_tc.cu", "cem.cu", "mbpo.cu", "train.cu", "latent.cu", "sac.cu", "latent_train.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 

@@ -1458,4 +1458,93 @@ int b200pets_latent_cem_plan(b200pets_latent_model_t model, const b200pets_rollo
   return B200PETS_OK;
 }
 
+// ---------------------------------------------------------------------------------------------------------
+// Training PlaNet's latent model: the recurrence's forward and backward passes (latent_train.cu)
+// ---------------------------------------------------------------------------------------------------------
+}  // extern "C"
+
+static LatentTrainDev latent_train_dev(const b200pets_latent_train_desc& d, const float* const* params) {
+  LatentTrainDev v{};
+  v.m.A = d.action_size; v.m.L = d.latent_size; v.m.Hb = d.belief_size; v.m.Hf = d.hidden_size;
+  v.m.A4 = round_up(v.m.A, 4); v.m.L4 = round_up(v.m.L, 4); v.m.Hb4 = round_up(v.m.Hb, 4); v.m.Hf4 = round_up(v.m.Hf, 4);
+  v.m.min_std = d.min_std;
+  v.E = d.encoding_size;
+  if (params)
+    for (int i = 0; i < B200PETS_LATENT_TRAIN_NUM_PARAMS; ++i) v.src[i] = params[i];
+  return v;
+}
+
+static int latent_train_args(const b200pets_latent_train_desc* desc, const float* const* params, int32_t batch,
+                             int32_t steps, const b200pets_latent_tape* tape, bool backward, const char* who) {
+  if (!desc || !params) return b200pets_set_error(B200PETS_EINVAL, "%s: null argument", who);
+  for (int i = 0; i < B200PETS_LATENT_TRAIN_NUM_PARAMS; ++i)
+    if (!params[i]) return b200pets_set_error(B200PETS_EINVAL, "%s: parameter %d is NULL", who, i);
+  if (batch < 1 || steps < 1)
+    return b200pets_set_error(B200PETS_EINVAL, "%s: batch %d and steps %d must be positive", who, batch, steps);
+  if (tape) {
+    const float* f[6] = {tape->e, tape->gates, tape->q1, tape->p1, tape->pre_std, tape->eps};
+    const float* g[6] = {tape->de, tape->dgi, tape->dghn, tape->dq, tape->dv, tape->dp};
+    for (int i = 0; i < 6; ++i)
+      if (!f[i] || (backward && !g[i])) return b200pets_set_error(B200PETS_EINVAL, "%s: a tape field is NULL", who);
+  } else if (backward) {
+    return b200pets_set_error(B200PETS_EINVAL, "%s: the backward pass needs the forward pass's tape", who);
+  }
+  return B200PETS_OK;
+}
+
+extern "C" {
+
+int b200pets_latent_train_supported(const b200pets_latent_train_desc* desc) {
+  if (!desc) return b200pets_set_error(B200PETS_EINVAL, "latent_train_supported: null argument");
+  return latent_train_check(latent_train_dev(*desc, nullptr), "latent_train_supported");
+}
+
+size_t b200pets_latent_train_workspace_bytes(const b200pets_latent_train_desc* desc, int32_t batch, int32_t steps) {
+  if (!desc || batch < 1 || steps < 1) return 0;
+  return latent_train_blob_floats(latent_train_dev(*desc, nullptr)) * sizeof(float);
+}
+
+int b200pets_latent_seq_forward(const b200pets_latent_train_desc* desc, const float* const* params, int32_t batch,
+                                int32_t steps, const float* P, const float* act, const float* eps_q, const float* eps_p,
+                                uint64_t seed, uint64_t offset, float* beliefs, float* post_params, float* post_samples,
+                                float* prior_params, float* prior_samples, const b200pets_latent_tape* tape,
+                                void* workspace, size_t workspace_bytes, void* stream) {
+  if (int rc = latent_train_args(desc, params, batch, steps, tape, false, "latent_seq_forward")) return rc;
+  if (!P || !act || !beliefs || !post_params || !post_samples || !prior_params || !prior_samples || !workspace)
+    return b200pets_set_error(B200PETS_EINVAL, "latent_seq_forward: null argument");
+  if (!eps_q != !eps_p)
+    return b200pets_set_error(B200PETS_EINVAL, "latent_seq_forward: inject both eps_q and eps_p or neither");
+  LatentTrainDev d = latent_train_dev(*desc, params);
+  if (int rc = latent_train_check(d, "latent_seq_forward")) return rc;
+  const size_t need = b200pets_latent_train_workspace_bytes(desc, batch, steps);
+  if (workspace_bytes < need)
+    return b200pets_set_error(B200PETS_EINVAL, "latent_seq_forward: workspace of %zu bytes, %zu needed", workspace_bytes, need);
+  if (int rc = latent_train_stage(&d, (float*)workspace, (cudaStream_t)stream)) return rc;
+  LatentSeqArgs a{};
+  a.B = batch; a.T = steps;
+  a.P = P; a.act = act; a.eps_q = eps_q; a.eps_p = eps_p;
+  a.seed = rng_key(seed, offset); a.offset = offset;
+  a.beliefs = beliefs; a.post_params = post_params; a.post_samples = post_samples;
+  a.prior_params = prior_params; a.prior_samples = prior_samples;
+  if (tape) a.tape = *tape;
+  return launch_latent_seq_forward(d, a, (cudaStream_t)stream);
+}
+
+int b200pets_latent_seq_backward(const b200pets_latent_train_desc* desc, const float* const* params, int32_t batch,
+                                 int32_t steps, const float* beliefs, const float* g_beliefs, const float* g_post_params,
+                                 const float* g_post_samples, const float* g_prior_params, const float* g_prior_samples,
+                                 const b200pets_latent_tape* tape, float* dP, void* stream) {
+  if (int rc = latent_train_args(desc, params, batch, steps, tape, true, "latent_seq_backward")) return rc;
+  if (!beliefs || !dP) return b200pets_set_error(B200PETS_EINVAL, "latent_seq_backward: null argument");
+  const LatentTrainDev d = latent_train_dev(*desc, params);
+  LatentSeqArgs a{};
+  a.B = batch; a.T = steps;
+  a.beliefs = const_cast<float*>(beliefs);
+  a.g_beliefs = g_beliefs; a.g_post_params = g_post_params; a.g_post_samples = g_post_samples;
+  a.g_prior_params = g_prior_params; a.g_prior_samples = g_prior_samples;
+  a.dP = dP;
+  a.tape = *tape;
+  return launch_latent_seq_backward(d, a, (cudaStream_t)stream);
+}
+
 }  // extern "C"

@@ -150,6 +150,10 @@ __device__ __forceinline__ void philox_normal4(uint32_t c0, uint32_t c1, uint32_
 // latent.cu, the prior's draw of latent element j of row r at step t: philox_normal4(r, t, RNG_STREAM_LATENT | (j >> 2),
 // offset, rng_key(seed, offset)), lane j & 3 (r: row of the call, n * P + p; t: step of the call, 0 for one step)
 #define RNG_STREAM_LATENT 0x60000u
+// latent_train.cu, the draw of latent element j of row b at step t of a training sequence, kind 0 for the posterior and
+// 1 for the prior: philox_normal4(b, t, RNG_STREAM_LATENT_TRAIN | (kind << 15) | (j >> 2), offset, rng_key(seed, offset)),
+// lane j & 3 (offset: the model's update counter)
+#define RNG_STREAM_LATENT_TRAIN 0x80000u
 // sac.cu, the reparameterisation draw of action j of row r in sample s (0: the policy on s', 1: on s) of one update:
 // philox_normal4(r, s, RNG_STREAM_SAC | (j >> 2), offset, rng_key(seed, offset)), lane j & 3 (offset: the agent's update
 // counter)

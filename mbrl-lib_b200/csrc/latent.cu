@@ -10,66 +10,6 @@
 
 namespace {
 
-constexpr int kLatentThreads = 256;
-
-__host__ __device__ inline int pad4(int x) { return (x + 3) & ~3; }
-
-// per-row shared memory (floats): V = [embedding | belief | latent | action], G = gates / hidden activations, total
-__host__ __device__ inline int latent_v_stride(const LatentDev& m) { return 2 * m.Hb4 + m.L4 + m.A4; }
-__host__ __device__ inline int latent_g_stride(const LatentDev& m) {
-  return pad4(max(4 * m.Hb, max(m.Hf4 + 2 * m.L, 2 * m.Hf4)));
-}
-
-// acc[r] += sum_k in[r][k] * W[k][n] over k < Kp (a multiple of 4); in rows are ld floats apart
-template <int R>
-__device__ __forceinline__ void dense_col(const float* __restrict__ W, int N, int Kp, const float* in, int ld, int n,
-                                          float (&acc)[R]) {
-  const float* w = W + n;
-#pragma unroll 2
-  for (int k = 0; k < Kp; k += 4) {
-    const float w0 = __ldg(w), w1 = __ldg(w + N), w2 = __ldg(w + 2 * N), w3 = __ldg(w + 3 * N);
-    w += 4 * (size_t)N;
-#pragma unroll
-    for (int r = 0; r < R; ++r) {
-      const float4 x = *reinterpret_cast<const float4*>(in + r * ld + k);
-      acc[r] = fmaf(x.x, w0, acc[r]);
-      acc[r] = fmaf(x.y, w1, acc[r]);
-      acc[r] = fmaf(x.z, w2, acc[r]);
-      acc[r] = fmaf(x.w, w3, acc[r]);
-    }
-  }
-}
-
-// out[r][n] = act(W[:, n] . in[r] + b[n]) for n < N4 (columns N .. N4-1 are written as zeros: they are the padding the
-// next layer reads)
-template <int R, bool RELU>
-__device__ __forceinline__ void dense(const float* __restrict__ W, const float* __restrict__ b, int N, int N4, int Kp,
-                                      const float* in, int ld_in, float* out, int ld_out) {
-  for (int n = threadIdx.x; n < N4; n += kLatentThreads) {
-    float acc[R];
-    const float bn = n < N ? __ldg(b + n) : 0.f;
-#pragma unroll
-    for (int r = 0; r < R; ++r) acc[r] = bn;
-    if (n < N) dense_col<R>(W, N, Kp, in, ld_in, n, acc);
-#pragma unroll
-    for (int r = 0; r < R; ++r) out[r * ld_out + n] = n < N ? (RELU ? fmaxf(acc[r], 0.f) : acc[r]) : 0.f;
-  }
-}
-
-__device__ __forceinline__ float sigmoid_f(float x) { return 1.0f / (1.0f + expf(-x)); }
-
-// Lane j & 3 of philox_normal4v at the RNG_STREAM_LATENT counter (common.cuh), computed inline: only the Box-Muller
-// pair the lane belongs to, with the same operations, so the value is that of philox_normal4v
-__device__ __forceinline__ float latent_draw(uint32_t row, uint32_t t, int j, uint32_t offset, unsigned long long key) {
-  const U4 q = philox4x32_10(row, t, RNG_STREAM_LATENT | (uint32_t)(j >> 2), offset, (uint32_t)key, (uint32_t)(key >> 32));
-  const int lane = j & 3;
-  const float ur = u32_to_unit(lane < 2 ? q.x : q.z), ua = u32_to_unit(lane < 2 ? q.y : q.w);
-  const float rad = sqrtf(-2.0f * __logf(ur));
-  float sn, cs;
-  __sincosf(6.283185307179586f * ua, &sn, &cs);
-  return rad * ((lane & 1) ? sn : cs);
-}
-
 template <int R>
 __global__ void __launch_bounds__(kLatentThreads, 1) latent_rollout_kernel(const LatentDev m, const LatentArgs a) {
   extern __shared__ float4 smem4[];
@@ -157,7 +97,7 @@ __global__ void __launch_bounds__(kLatentThreads, 1) latent_rollout_kernel(const
         if (a.eps) {
           e = a.eps[((long long)t * a.B + row) * L + j];
         } else {
-          e = latent_draw((uint32_t)row, (uint32_t)t, j, (uint32_t)a.offset, a.seed);
+          e = latent_draw((uint32_t)row, (uint32_t)t, RNG_STREAM_LATENT, j, (uint32_t)a.offset, a.seed);
         }
         const float sd = softplus_f(p[L + j]) + m.min_std;
         s = s + sd * e;
@@ -264,17 +204,26 @@ void latent_bind(LatentDev* m, float* blob) {
   }
 }
 
+void latent_pack(float* dst, int Kp, int N, const float* src0, int ld0, int coff0, int n0, const float* src1, int ld1,
+                 int coff1, int n1, int row1, int row_off, cudaStream_t stream) {
+  const long long tot = (long long)Kp * N;
+  latent_pack_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, stream>>>(dst, Kp, N, src0, ld0, coff0, n0, src1, ld1, coff1,
+                                                                       n1, row1, row_off);
+}
+
+void latent_pack_bias(float* dst, int N, const float* b0, const float* b1, int off, cudaStream_t stream) {
+  latent_bias_kernel<<<(N + 255) / 256, 256, 0, stream>>>(dst, N, b0, b1, off);
+}
+
 // params: the B200PETS_LATENT_NUM_PARAMS torch tensors in the order of include/b200pets.h
 int latent_stage(const LatentDev& m, const float* const* params, cudaStream_t stream) {
   const int L = m.L, A = m.A, Hb = m.Hb, Hf = m.Hf;
   auto pack = [&](const float* dst, int Kp, int N, const float* s0, int ld0, int c0, int n0, const float* s1, int ld1, int c1,
                   int n1, int row1, int row_off) {
-    const long long tot = (long long)Kp * N;
-    latent_pack_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, stream>>>(const_cast<float*>(dst), Kp, N, s0, ld0, c0, n0, s1,
-                                                                         ld1, c1, n1, row1, row_off);
+    latent_pack(const_cast<float*>(dst), Kp, N, s0, ld0, c0, n0, s1, ld1, c1, n1, row1, row_off, stream);
   };
   auto bias = [&](const float* dst, int N, const float* b0, const float* b1, int off) {
-    latent_bias_kernel<<<(N + 255) / 256, 256, 0, stream>>>(const_cast<float*>(dst), N, b0, b1, off);
+    latent_pack_bias(const_cast<float*>(dst), N, b0, b1, off, stream);
   };
   const float *We = params[0], *be = params[1], *Wih = params[2], *Whh = params[3], *bih = params[4], *bhh = params[5];
   pack(m.We, m.L4 + m.A4, Hb, We, L + A, 0, L, We, L + A, L, A, m.L4, 0);

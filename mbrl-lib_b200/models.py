@@ -237,16 +237,75 @@ class _BeliefModel(nn.Module):  # mbrl/models/planet.py:82-101
         self.rnn = nn.GRUCell(belief_size, belief_size)
 
 
+class _Conv2dEncoder(nn.Module):  # mbrl/models/util.py:101-157
+    def __init__(self, layers_config, image_shape, encoding_size: int):
+        super().__init__()
+        self.convs = nn.ModuleList([nn.Sequential(nn.Conv2d(c[0], c[1], c[2], stride=c[3]), nn.ReLU())
+                                    for c in layers_config])
+        with torch.no_grad():
+            out = self.convs_forward(torch.zeros(1, layers_config[0][0], *image_shape))
+        cnn_out_size = int(np.prod(out.shape[1:]))
+        self.fc = nn.Identity() if cnn_out_size == encoding_size else nn.Linear(cnn_out_size, encoding_size)
+
+    def convs_forward(self, obs):
+        for conv in self.convs:
+            obs = conv(obs)
+        return obs
+
+    def forward(self, obs):
+        conv = self.convs_forward(obs)
+        return self.fc(conv.view(conv.size(0), -1))
+
+
+class _Conv2dDecoder(nn.Module):  # mbrl/models/util.py:162-212
+    def __init__(self, encoding_size: int, deconv_input_shape, layers_config):
+        super().__init__()
+        self.encoding_size = encoding_size
+        self.deconv_input_shape = tuple(deconv_input_shape)
+        self.fc = nn.Linear(encoding_size, int(np.prod(self.deconv_input_shape)))
+        mods = []
+        for i, c in enumerate(layers_config):
+            layer = nn.ConvTranspose2d(c[0], c[1], c[2], stride=c[3])
+            mods.append(layer if i == len(layers_config) - 1 else nn.Sequential(layer, nn.ReLU()))
+        self.deconvs = nn.ModuleList(mods)
+
+    def forward(self, x):
+        deconv = self.fc(x).view(-1, *self.deconv_input_shape)
+        for layer in self.deconvs:
+            deconv = layer(deconv)
+        return deconv
+
+
+class _MeanStdCat(nn.Module):  # mbrl/models/planet.py:103-114
+    def __init__(self, latent_state_size: int, min_std: float):
+        super().__init__()
+        self.min_std = min_std
+        self.latent_state_size = latent_state_size
+
+    def forward(self, params):
+        mean = params[:, : self.latent_state_size]
+        std = F.softplus(params[:, self.latent_state_size:]) + self.min_std
+        return torch.cat([mean, std], dim=1)
+
+
 class PlaNetModel(nn.Module):
-    """The planning half of mbrl-lib's ``PlaNetModel`` (planet.py:121-306) with its attribute layout:
-    ``belief_model.{embedding_layer, rnn}``, ``prior_transition_model[0, 2]``, ``reward_model[0, 2, 4]``, ``min_std``
-    and the posterior ``_current_posterior_sample [1, L]`` / ``_current_belief [1, Hb]`` that planning starts from.
-    The conv encoder / decoder and the posterior model are not here: :meth:`set_posterior` stands in for
-    ``update_posterior``.  Weights start as torch's default initialisation unless ``seed`` is given, in which case
-    every parameter is drawn from N(0, scale^2) with that numpy seed, in the order of ``latent.latent_params``."""
+    """mbrl-lib's ``PlaNetModel`` (planet.py:121-306) with its attribute layout: ``belief_model.{embedding_layer, rnn}``,
+    ``prior_transition_model[0, 2]``, ``reward_model[0, 2, 4]``, ``min_std`` and the posterior
+    ``_current_posterior_sample [1, L]`` / ``_current_belief [1, Hb]`` that planning starts from.
+
+    Without ``obs_shape`` it is the planning half only: no encoder, decoder or posterior model, and :meth:`set_posterior`
+    stands in for ``update_posterior``.  With ``obs_shape``, ``obs_encoding_size``, ``encoder_config`` and
+    ``decoder_config`` it also has ``encoder``, ``posterior_transition_model`` and ``decoder`` with the reference's
+    layout and ``state_dict`` keys, and ``free_nats``, ``kl_scale``, ``grad_clip_norm`` and ``rng``: what
+    :mod:`mbrl_lib_b200.latent_train` trains.  Weights start as torch's default initialisation unless ``seed`` is
+    given, in which case every parameter is drawn from N(0, scale^2) with that numpy seed, in the order of
+    ``latent.latent_params`` and then of the encoder, the posterior and the decoder."""
 
     def __init__(self, action_size: int, latent_state_size: int = 30, belief_size: int = 200, hidden_size_fcs: int = 200,
-                 device="cpu", min_std: float = 0.1, seed: Optional[int] = None, scale: float = 0.1):
+                 device="cpu", min_std: float = 0.1, seed: Optional[int] = None, scale: float = 0.1, *,
+                 obs_shape=None, obs_encoding_size: Optional[int] = None, encoder_config=None, decoder_config=None,
+                 free_nats: float = 3, kl_scale: float = 1.0, grad_clip_norm: float = 1000.0,
+                 rng: Optional[torch.Generator] = None):
         super().__init__()
         self.action_size, self.latent_state_size, self.belief_size = action_size, latent_state_size, belief_size
         self.min_std = min_std
@@ -254,16 +313,30 @@ class PlaNetModel(nn.Module):
         self.belief_model = _BeliefModel(latent_state_size, action_size, belief_size)
         self.prior_transition_model = nn.Sequential(nn.Linear(belief_size, hidden_size_fcs), nn.ReLU(),
                                                     nn.Linear(hidden_size_fcs, 2 * latent_state_size))
+        if obs_shape is not None:  # the reference's module order (planet.py:227-265)
+            self.obs_shape = tuple(obs_shape)
+            self.free_nats = free_nats * torch.ones(1).to(device)
+            self.kl_scale = kl_scale
+            self.grad_clip_norm = grad_clip_norm
+            self.rng = torch.Generator(device=self.device) if rng is None else rng
+            self.encoder = _Conv2dEncoder(encoder_config, self.obs_shape[1:], obs_encoding_size)
+            self.posterior_transition_model = nn.Sequential(
+                nn.Linear(obs_encoding_size + belief_size, hidden_size_fcs), nn.ReLU(),
+                nn.Linear(hidden_size_fcs, 2 * latent_state_size), _MeanStdCat(latent_state_size, min_std))
+            self.decoder = _Conv2dDecoder(latent_state_size + belief_size, decoder_config[0], decoder_config[1])
         self.reward_model = nn.Sequential(nn.Linear(belief_size + latent_state_size, hidden_size_fcs), nn.ReLU(),
                                           nn.Linear(hidden_size_fcs, hidden_size_fcs), nn.ReLU(),
                                           nn.Linear(hidden_size_fcs, 1))
         if seed is not None:
             from .latent import latent_params
 
-            rng = np.random.default_rng(seed)
+            rng_np = np.random.default_rng(seed)
+            first = latent_params(self)
+            rest = [] if obs_shape is None else \
+                [p for mod in (self.encoder, self.posterior_transition_model, self.decoder) for p in mod.parameters()]
             with torch.no_grad():
-                for p in latent_params(self):
-                    p.copy_(torch.from_numpy(rng.normal(0.0, scale, tuple(p.shape)).astype(np.float32)))
+                for p in first + rest:
+                    p.copy_(torch.from_numpy(rng_np.normal(0.0, scale, tuple(p.shape)).astype(np.float32)))
         self._current_posterior_sample: Optional[torch.Tensor] = None
         self._current_belief: Optional[torch.Tensor] = None
         self.to(self.device)

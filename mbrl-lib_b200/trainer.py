@@ -18,10 +18,15 @@ What runs where:
     other iterable of transition batches takes one fused Adam step per yielded batch.  Transitions may be float32 or
     float64 (mbrl-lib's PETS / MBPO replay buffers are float64 with ``normalize_double_precision``); float64 ones are
     processed in double, as the reference's numpy / torch code processes them, and rounded to float32 at the end;
-  * otherwise (a ``batch_callback``, which needs every batch's loss as it happens, another model, a model the kernels
-    refuse -- more than 7 hidden layers, or layers too wide for the evaluation kernel's shared memory -- or transitions
-    of another element type) the reference's PyTorch loop runs unchanged: ``model.update(batch, optimizer)`` /
-    ``model.eval_score(batch)``.  A refused model runs the whole ``train()`` / ``evaluate()`` call that way.
+  * the latent path: a ``PlaNetModel`` (mbrl-lib's or :mod:`models`' with the encoder and decoder) whose recurrence
+    ``b200pets_latent_train_supported`` accepts, with fp32 CUDA parameters and one Adam param group over
+    ``model.parameters()``: the reference's loop below, with each batch through :func:`latent_train.update` and each
+    evaluation batch through :func:`latent_train.eval_score` in place of the model's own methods.  ``batch_callback`` is
+    called per batch with the reference's arguments, as ``mbrl/algorithms/planet.py`` needs;
+  * otherwise (a ``batch_callback`` on a GaussianMLP, which needs every batch's loss as it happens, another model, a
+    model the kernels refuse -- more than 7 hidden layers, or layers too wide for the evaluation kernel's shared memory
+    -- or transitions of another element type) the reference's PyTorch loop runs unchanged: ``model.update(batch,
+    optimizer)`` / ``model.eval_score(batch)``.  A refused model runs the whole ``train()`` / ``evaluate()`` call that way.
 """
 from __future__ import annotations
 
@@ -34,7 +39,7 @@ from typing import Callable, Dict, List, Optional, Tuple
 import numpy as np
 import torch
 
-from . import _lib, functions, staging
+from . import _lib, functions, latent_train, staging
 
 MODEL_LOG_FORMAT = [
     ("train_iteration", "I", "int"),
@@ -265,6 +270,7 @@ class ModelTrainer:
             self.logger.register_group(self._LOG_GROUP_NAME, MODEL_LOG_FORMAT, color="blue", dump_frequency=1)
         self.optimizer = torch.optim.Adam(self.model.parameters(), lr=optim_lr, weight_decay=weight_decay, eps=optim_eps)
         self._dev: Optional[_DeviceModel] = None
+        self._latent = False
 
     # ---- which path ----------------------------------------------------------------------------------------------
     def _device_supported(self) -> bool:
@@ -296,6 +302,24 @@ class ModelTrainer:
         with torch.cuda.device(dev):
             return _lib.load().b200pets_trainer_supported(C.byref(train_desc(mlp, g))) == 0
 
+    def _latent_supported(self) -> bool:
+        """The latent path (see the module docstring), asked before anything is touched."""
+        if not latent_train.is_trainable_latent_model(self.model) or len(self.optimizer.param_groups) != 1:
+            return False
+        if {id(p) for p in self.optimizer.param_groups[0]["params"]} != {id(p) for p in self.model.parameters()}:
+            return False
+        return latent_train.supported(self.model)
+
+    def _model_update(self, batch):
+        if self._latent:
+            return latent_train.update(self.model, batch, self.optimizer)
+        return self.model.update(batch, self.optimizer)
+
+    def _model_eval_score(self, batch):
+        if self._latent:
+            return latent_train.eval_score(self.model, batch)
+        return self.model.eval_score(batch)
+
     @staticmethod
     def _store_supported(ds) -> bool:
         return transition_dtype(ds.transitions) is not None
@@ -313,7 +337,8 @@ class ModelTrainer:
         """Trains the model for some number of epochs (model_trainer.py:70-214): returns the per-epoch mean training
         losses and evaluation scores; keeps the weights of the best evaluation score (relative improvement of any member
         above ``improvement_threshold``), stops after ``patience`` epochs without one and sets the elite members."""
-        device = batch_callback is None and self._device_supported()
+        self._latent = self._latent_supported()
+        device = not self._latent and batch_callback is None and self._device_supported()
         self._dev = None
         try:
             return self._train(dataset_train, dataset_val, num_epochs, patience, improvement_threshold, callback,
@@ -338,7 +363,7 @@ class ModelTrainer:
             else:
                 batch_losses = []
                 for batch in dataset_train:
-                    loss, meta = self.model.update(batch, self.optimizer)
+                    loss, meta = self._model_update(batch)
                     batch_losses.append(loss)
                     if batch_callback_epoch:
                         batch_callback_epoch(loss, meta, "train")
@@ -418,6 +443,8 @@ class ModelTrainer:
 
     def evaluate(self, dataset, batch_callback: Optional[Callable] = None) -> torch.Tensor:
         """Mean score of the model over the dataset, per ensemble member (model_trainer.py:216-262)."""
+        if self._dev is None:
+            self._latent = self._latent_supported()
         if batch_callback is None and self._dev is None and self._device_supported():
             try:
                 return self._evaluate(dataset, None, True)
@@ -433,7 +460,7 @@ class ModelTrainer:
             dataset.toggle_bootstrap()
         batch_scores_list = []
         for batch in dataset:
-            batch_score, meta = self.model.eval_score(batch)
+            batch_score, meta = self._model_eval_score(batch)
             batch_scores_list.append(batch_score)
             if batch_callback:
                 batch_callback(batch_score.mean(), meta, "eval")
