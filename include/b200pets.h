@@ -519,6 +519,13 @@ typedef struct {
 int b200pets_latent_train_supported(const b200pets_latent_train_desc* desc);
 /* Bytes of the workspace b200pets_latent_seq_forward re-packs the weights into (0 for bad arguments). */
 size_t b200pets_latent_train_workspace_bytes(const b200pets_latent_train_desc* desc, int32_t batch, int32_t steps);
+/* The launch of b200pets_latent_seq_forward (backward == 0) or b200pets_latent_seq_backward for `batch` rows on the
+ * current device, by the rule and in the layout of b200pets_latent_plan_info: info[0] rows per CTA, info[1] CTAs,
+ * info[2] dynamic shared memory of one CTA, info[3] shared memory bytes of one row.  The backward kernel's row is the
+ * larger, so at the same batch its tile can be half the forward's.  Refused as b200pets_latent_train_supported, and
+ * B200PETS_EINVAL for a NULL argument or batch < 1. */
+int b200pets_latent_train_plan_info(const b200pets_latent_train_desc* desc, int32_t batch, int32_t backward,
+                                    int32_t info[4]);
 /* The forward pass (planet.py:370-402 without the decoder and the reward model), one re-pack and one launch:
  *   P [dev] float[B][T][Hf]; act [dev] float[B][T][A] (action[:, :-1]);
  *   eps_q, eps_p [dev] float[T][B][L] injected N(0,1) draws (both or neither), or NULL = Philox on RNG_STREAM_LATENT_TRAIN

@@ -169,6 +169,8 @@ _SIGNATURES = {
                                            _P, C.c_size_t, _P]),
     "b200pets_latent_train_supported": (C.c_int, [C.POINTER(LatentTrainDesc)]),
     "b200pets_latent_train_workspace_bytes": (C.c_size_t, [C.POINTER(LatentTrainDesc), C.c_int32, C.c_int32]),
+    "b200pets_latent_train_plan_info": (C.c_int, [C.POINTER(LatentTrainDesc), C.c_int32, C.c_int32,
+                                                  C.POINTER(C.c_int32)]),
     "b200pets_latent_seq_forward": (C.c_int, [C.POINTER(LatentTrainDesc), C.POINTER(_P), C.c_int32, C.c_int32, _P, _P, _P, _P,
                                               C.c_uint64, C.c_uint64, _P, _P, _P, _P, _P, C.POINTER(LatentTape), _P,
                                               C.c_size_t, _P]),

@@ -1504,6 +1504,19 @@ size_t b200pets_latent_train_workspace_bytes(const b200pets_latent_train_desc* d
   return latent_train_blob_floats(latent_train_dev(*desc, nullptr)) * sizeof(float);
 }
 
+int b200pets_latent_train_plan_info(const b200pets_latent_train_desc* desc, int32_t batch, int32_t backward,
+                                    int32_t info[4]) {
+  if (!desc || !info) return b200pets_set_error(B200PETS_EINVAL, "latent_train_plan_info: null argument");
+  if (batch < 1) return b200pets_set_error(B200PETS_EINVAL, "latent_train_plan_info: batch %d < 1", batch);
+  LatentPlan p;
+  if (int rc = latent_train_plan(latent_train_dev(*desc, nullptr), batch, !backward, "latent_train_plan_info", &p)) return rc;
+  info[0] = p.rows;
+  info[1] = (int32_t)p.ctas;
+  info[2] = (int32_t)p.smem;
+  info[3] = (int32_t)p.row_bytes;
+  return B200PETS_OK;
+}
+
 int b200pets_latent_seq_forward(const b200pets_latent_train_desc* desc, const float* const* params, int32_t batch,
                                 int32_t steps, const float* P, const float* act, const float* eps_q, const float* eps_p,
                                 uint64_t seed, uint64_t offset, float* beliefs, float* post_params, float* post_samples,

@@ -249,28 +249,32 @@ int latent_stage(const LatentDev& m, const float* const* params, cudaStream_t st
   return B200PETS_OK;
 }
 
-// Rows per CTA: enough CTAs to cover the SMs once (the smallest power of two >= rows / SMs, at most 32), halved while
-// the tile does not fit in shared memory.  A model is refused when a row needs more than an eighth of the opt-in shared
-// memory, so that the 8-row tile a 1000-row population takes on an H100 always fits.
-int latent_plan(const LatentDev& m, long long rows, LatentPlan* p) {
+int latent_tile(size_t row_bytes, long long rows, LatentPlan* p) {
   int dev = 0, max_smem = 0, sms = 0;
   CUDA_TRY(cudaGetDevice(&dev));
   CUDA_TRY(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
   CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  p->row_bytes = (size_t)(latent_v_stride(m) + latent_g_stride(m) + 1) * sizeof(float);
-  p->row_limit = (size_t)max_smem / 8;
-  if (p->row_bytes > p->row_limit)
-    return b200pets_set_error(B200PETS_EUNSUPPORTED,
-                              "latent model: one row needs %zu bytes of shared memory (belief %d, hidden %d, latent %d, action "
-                              "%d); the limit is %zu bytes, an eighth of the %d bytes a CTA can have",
-                              p->row_bytes, m.Hb, m.Hf, m.L, m.A, p->row_limit, max_smem);
   const long long want = rows > 0 ? (rows + sms - 1) / sms : 1;
   int R = 1;
   while (R < want && R < 32) R *= 2;
-  while (R > 1 && (size_t)R * p->row_bytes > (size_t)max_smem) R /= 2;
+  while (R > 1 && (size_t)R * row_bytes > (size_t)max_smem) R /= 2;
   p->rows = R;
   p->ctas = rows > 0 ? (rows + R - 1) / R : 0;
-  p->smem = ((size_t)R * p->row_bytes + 15) & ~(size_t)15;
+  p->smem = ((size_t)R * row_bytes + 15) & ~(size_t)15;
+  p->row_bytes = row_bytes;
+  p->row_limit = (size_t)max_smem / 8;
+  return B200PETS_OK;
+}
+
+// The rollout's tile.  A model is refused when a row needs more than an eighth of the opt-in shared memory, so that the
+// 8-row tile a 1000-row population takes on an H100 always fits.
+int latent_plan(const LatentDev& m, long long rows, LatentPlan* p) {
+  if (int rc = latent_tile((size_t)(latent_v_stride(m) + latent_g_stride(m) + 1) * sizeof(float), rows, p)) return rc;
+  if (p->row_bytes > p->row_limit)
+    return b200pets_set_error(B200PETS_EUNSUPPORTED,
+                              "latent model: one row needs %zu bytes of shared memory (belief %d, hidden %d, latent %d, action "
+                              "%d); the limit is %zu bytes, an eighth of the shared memory a CTA can have",
+                              p->row_bytes, m.Hb, m.Hf, m.L, m.A, p->row_limit);
   return B200PETS_OK;
 }
 

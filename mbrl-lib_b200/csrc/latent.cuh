@@ -123,6 +123,11 @@ int latent_stage(const LatentDev& m, const float* const* params, cudaStream_t st
 void latent_pack(float* dst, int Kp, int N, const float* src0, int ld0, int coff0, int n0, const float* src1, int ld1,
                  int coff1, int n1, int row1, int row_off, cudaStream_t stream);
 void latent_pack_bias(float* dst, int N, const float* b0, const float* b1, int off, cudaStream_t stream);
+// The tile rule of every latent kernel (the rollout's and training's two): for `rows` rows of `row_bytes` bytes of
+// shared memory each on the current device, enough CTAs to cover the SMs once (the smallest power of two >= rows / SMs,
+// at most 32 rows), halved while the tile does not fit in the opt-in shared memory.  Sets every field of *p; rows < 1
+// gives one row per CTA and no CTAs.
+int latent_tile(size_t row_bytes, long long rows, LatentPlan* p);
 int latent_plan(const LatentDev& m, long long rows, LatentPlan* p);
 int launch_latent_rollout(const LatentDev& m, const LatentArgs& a, cudaStream_t stream);
 
@@ -152,5 +157,7 @@ struct LatentSeqArgs {
 int latent_train_check(const LatentTrainDev& d, const char* who);
 size_t latent_train_blob_floats(const LatentTrainDev& d);
 int latent_train_stage(LatentTrainDev* d, float* blob, cudaStream_t stream);  // binds the packed fields into blob
+// The launch of the forward (or the backward) kernel for `batch` rows: latent_train_check, then latent_tile
+int latent_train_plan(const LatentTrainDev& d, int batch, bool forward, const char* who, LatentPlan* p);
 int launch_latent_seq_forward(const LatentTrainDev& d, const LatentSeqArgs& a, cudaStream_t stream);
 int launch_latent_seq_backward(const LatentTrainDev& d, const LatentSeqArgs& a, cudaStream_t stream);

@@ -421,29 +421,23 @@ static int launch_seq(const LatentTrainDev& d, const LatentSeqArgs& a, size_t sm
   return B200PETS_OK;
 }
 
-// Rows per CTA as latent_plan picks them: enough CTAs to cover the SMs once (at most 32 rows), halved while the tile
-// does not fit in shared memory
+int latent_train_plan(const LatentTrainDev& d, int batch, bool forward, const char* who, LatentPlan* p) {
+  if (int rc = latent_train_check(d, who)) return rc;
+  return latent_tile((size_t)(forward ? fwd_row_floats(d.m) : bwd_row_floats(d.m)) * sizeof(float), batch, p);
+}
+
 template <bool FWD>
 static int launch(const LatentTrainDev& d, const LatentSeqArgs& a, cudaStream_t stream) {
-  if (int rc = latent_train_check(d, FWD ? "latent_seq_forward" : "latent_seq_backward")) return rc;
-  int dev = 0, max_smem = 0, sms = 0;
-  CUDA_TRY(cudaGetDevice(&dev));
-  CUDA_TRY(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-  CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  const size_t row_bytes = (size_t)(FWD ? fwd_row_floats(d.m) : bwd_row_floats(d.m)) * sizeof(float);
-  const int want = (a.B + sms - 1) / sms;
-  int R = 1;
-  while (R < want && R < 32) R *= 2;
-  while (R > 1 && (size_t)R * row_bytes > (size_t)max_smem) R /= 2;
-  const int ctas = (a.B + R - 1) / R;
-  const size_t smem = ((size_t)R * row_bytes + 15) & ~(size_t)15;
-  switch (R) {
-    case 1: return launch_seq<1, FWD>(d, a, smem, ctas, stream);
-    case 2: return launch_seq<2, FWD>(d, a, smem, ctas, stream);
-    case 4: return launch_seq<4, FWD>(d, a, smem, ctas, stream);
-    case 8: return launch_seq<8, FWD>(d, a, smem, ctas, stream);
-    case 16: return launch_seq<16, FWD>(d, a, smem, ctas, stream);
-    default: return launch_seq<32, FWD>(d, a, smem, ctas, stream);
+  LatentPlan p;
+  if (int rc = latent_train_plan(d, a.B, FWD, FWD ? "latent_seq_forward" : "latent_seq_backward", &p)) return rc;
+  const int ctas = (int)p.ctas;
+  switch (p.rows) {
+    case 1: return launch_seq<1, FWD>(d, a, p.smem, ctas, stream);
+    case 2: return launch_seq<2, FWD>(d, a, p.smem, ctas, stream);
+    case 4: return launch_seq<4, FWD>(d, a, p.smem, ctas, stream);
+    case 8: return launch_seq<8, FWD>(d, a, p.smem, ctas, stream);
+    case 16: return launch_seq<16, FWD>(d, a, p.smem, ctas, stream);
+    default: return launch_seq<32, FWD>(d, a, p.smem, ctas, stream);
   }
 }
 
