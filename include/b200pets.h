@@ -546,12 +546,40 @@ int b200pets_latent_seq_backward(const b200pets_latent_train_desc* desc, const f
                                  const float* g_post_samples, const float* g_prior_params, const float* g_prior_samples,
                                  const b200pets_latent_tape* tape, float* dP, void* stream);
 
+/* ---- PlaNet's sequence batches from a device-resident replay buffer (mbrl_lib_b200/replay.py) -------------------
+ * The mirror holds a replay buffer's observations in chunks of 2^chunk_shift rows (separate allocations, found through
+ * a device table of chunk pointers) and its actions and rewards as float arrays of all rows. */
+typedef struct {
+  int64_t frame_elems;  /* elements of one observation (3 x 64 x 64 = 12288 for PlaNet's frames) */
+  int64_t rows;         /* rows held: sequences must lie in [0, rows) */
+  int32_t action_size;  /* A */
+  int32_t dtype;        /* storage type of the frames: B200PETS_DTYPE_U8 or B200PETS_DTYPE_F32 */
+  int32_t chunk_shift;  /* log2 of the rows per chunk, in [0, B200PETS_REPLAY_MAX_CHUNK_SHIFT] */
+} b200pets_replay_desc;
+#define B200PETS_REPLAY_MAX_CHUNK_SHIFT 30
+
+/* The batch PlaNetModel's loss reads from B sequences of T rows starting at starts[b] (_sequence_getitem_impl, then
+ * _process_batch and the loss's shifts, planet.py:274-287, 429-434), as one launch:
+ *   obs_chunks [dev] array of device pointers, chunk c holding rows [c << chunk_shift, (c + 1) << chunk_shift), each
+ *              row frame_elems contiguous elements of the storage type
+ *   act [dev] float[rows][A]; rew [dev] float[rows]; starts [dev] int64[B], each in [0, rows - T]
+ *   obs_out [dev] float[B][T-1][frame_elems]: frames t = 1 .. T-1 as x / 256 - 0.5 (bit-identical to torch's
+ *           obs.float() / 256.0 - 0.5)
+ *   act_out [dev] float[B][T-1][A], rew_out [dev] float[B][T-1]: rows t = 0 .. T-2
+ * A sequence whose start lies outside [0, rows - T] is skipped (its outputs are left as they were): the caller checks
+ * the starts.  Refused: NULL pointers, B < 1, T < 2, an unknown dtype, a chunk_shift out of range, frame_elems or A
+ * below 1, rows < T. */
+int b200pets_sequence_gather(const b200pets_replay_desc* desc, const void* const* obs_chunks, const float* act,
+                             const float* rew, const int64_t* starts, int32_t batch, int32_t steps, float* obs_out,
+                             float* act_out, float* rew_out, void* stream);
+
 /* ---- Training the dynamics model (mbrl/models/model_trainer.py:70-262) ------------------------------------
  * OneDTransitionRewardModel(GaussianMLP) trained with torch.optim.Adam, fp32 throughout. */
 
 /* element type of transition arrays */
 #define B200PETS_DTYPE_F32 0
 #define B200PETS_DTYPE_F64 1
+#define B200PETS_DTYPE_U8 2 /* frames of a replay mirror (b200pets_sequence_gather) */
 
 /* Raw transitions -> model inputs and targets (one_dim_tr_model.py:103-136), for a whole dataset at once:
  *   inputs  [dev] float[rows][in_size]  = normalise(cat(obs_process_fn(obs), act)): norm_mode 1 (fp32 statistics, norm_mean /

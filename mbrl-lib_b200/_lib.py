@@ -20,7 +20,7 @@ TERM = {"no_termination": 0, "cartpole": 1, "inverted_pendulum": 2, "hopper": 3,
         "humanoid": 6, "external": 255}
 PROP = {"random_model": 0, "fixed_model": 1, "expectation": 2}
 PREC = {"f32": 0, "bf16_tc": 1}
-DTYPE = {"float32": 0, "float64": 1}
+DTYPE = {"float32": 0, "float64": 1, "uint8": 2}
 TS1_PERMS, TS1_TILE_SHUFFLE = 0, 1
 
 
@@ -78,6 +78,12 @@ class TrainDesc(C.Structure):
                [(n, C.c_double) for n in ("lr", "beta1", "beta2", "eps", "weight_decay")]
 
 
+class ReplayDesc(C.Structure):
+    _fields_ = [("frame_elems", C.c_int64), ("rows", C.c_int64), ("action_size", C.c_int32), ("dtype", C.c_int32),
+                ("chunk_shift", C.c_int32)]
+
+
+REPLAY_MAX_CHUNK_SHIFT = 30
 SAC_MAX_ACTIONS = 32
 SAC_NUM_PARAMS, SAC_NUM_CRITIC_PARAMS = 20, 12
 
@@ -176,6 +182,7 @@ _SIGNATURES = {
                                               C.c_size_t, _P]),
     "b200pets_latent_seq_backward": (C.c_int, [C.POINTER(LatentTrainDesc), C.POINTER(_P), C.c_int32, C.c_int32, _P, _P, _P,
                                                _P, _P, _P, C.POINTER(LatentTape), _P, _P]),
+    "b200pets_sequence_gather": (C.c_int, [C.POINTER(ReplayDesc), _P, _P, _P, _P, C.c_int32, C.c_int32, _P, _P, _P, _P]),
     "b200pets_train_preprocess": (C.c_int, [C.POINTER(PrepDesc), C.c_int64, _P, _P, _P, _P, _P, _P, C.POINTER(C.c_int32),
                                             C.c_int32, _P, _P, _P]),
     "b200pets_trainer_create": (C.c_int, [C.POINTER(TrainDesc), C.POINTER(_P), C.POINTER(_P), C.POINTER(_P), C.POINTER(_P)]),

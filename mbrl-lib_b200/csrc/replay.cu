@@ -1,0 +1,163 @@
+// Sequence batches gathered from a device-resident mirror of a replay buffer (mbrl_lib_b200/replay.py): what
+//   mbrl/util/replay_buffer.py:183-195  _sequence_getitem_impl          (rows start .. start + T - 1 of each sequence)
+//   mbrl/models/planet.py:274-287       PlaNetModel._process_batch     (obs.float() / 256 - 0.5)
+//   mbrl/models/planet.py:429-434       the loss's obs[:, 1:], action[:, :-1], rewards[:, :-1]
+// compute on the host and copy over PCIe, as one launch that reads the mirror in HBM and writes only what the loss reads.
+//
+// The mirror keeps frames in chunks of 2^chunk_shift rows, each its own allocation, found through a device table of
+// chunk pointers; actions and rewards are one float array each.  Pure byte movement: every CTA walks whole frames
+// (grid-stride), its threads moving consecutive 16-byte pieces of a frame, so reads and writes coalesce.
+#include "common.cuh"
+
+namespace {
+
+constexpr int kThreads = 256;
+constexpr int kCtasPerSm = 8;  // 8 x 256 threads fill an SM; at B x (T-1) = 2450 frames each CTA walks 2 to 3 frames
+
+struct GatherArgs {
+  long long frame_elems, rows;
+  int action_size, chunk_shift, batch, steps;  // steps = T: each sequence yields T - 1 frames
+  const void* const* chunks;
+  const float* act;
+  const float* rew;
+  const long long* starts;
+  float *obs_out, *act_out, *rew_out;
+};
+
+// x / 256 - 0.5 in fp32, each operation rounded on its own: the division by a power of two is exact, so this is
+// bit-identical to torch's `obs.float() / 256.0 - 0.5` whatever the compiler's contraction settings.
+__device__ __forceinline__ float normalise(float x) { return __fsub_rn(__fmul_rn(x, 0x1p-8f), 0.5f); }
+
+__device__ __forceinline__ float4 normalise4(float a, float b, float c, float d) {
+  return make_float4(normalise(a), normalise(b), normalise(c), normalise(d));
+}
+
+// four uint8 pixels of a 32-bit word, lowest address first
+__device__ __forceinline__ float4 normalise_bytes(uint32_t w) {
+  return normalise4((float)(w & 0xff), (float)((w >> 8) & 0xff), (float)((w >> 16) & 0xff), (float)(w >> 24));
+}
+
+// one frame: 16-byte loads (16 uint8 pixels or 4 floats) and float4 stores.  A warp loads 32 consecutive 16-byte
+// pieces (512 pixels) and stores their 128 float4 in 4 rounds of 32 consecutive float4: float4 o of the warp's span
+// comes from 32-bit word o, held by lane o / 4 as component o % 4, and reaches its storing lane by a shuffle.  The
+// loop bounds are the same for the whole warp (the caller runs this for the whole CTA), so every shuffle has all lanes.
+__device__ __forceinline__ void frame_vec(const uint8_t* __restrict__ src, float* __restrict__ dst, long long n) {
+  const uint4* s = reinterpret_cast<const uint4*>(src);
+  float4* d = reinterpret_cast<float4*>(dst);
+  const long long nv = n / 16, nout = n / 4;
+  const int lane = threadIdx.x & 31, c = lane & 3;
+  for (long long base = (threadIdx.x >> 5) * 32LL; base < nv; base += kThreads) {
+    const long long i = base + lane;
+    const uint4 v = i < nv ? __ldg(s + i) : make_uint4(0u, 0u, 0u, 0u);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int from = 8 * k + (lane >> 2);
+      const uint32_t x = __shfl_sync(0xffffffffu, v.x, from), y = __shfl_sync(0xffffffffu, v.y, from),
+                     z = __shfl_sync(0xffffffffu, v.z, from), w = __shfl_sync(0xffffffffu, v.w, from);
+      const long long o = 4 * base + 32 * k + lane;
+      if (o < nout) d[o] = normalise_bytes(c == 0 ? x : c == 1 ? y : c == 2 ? z : w);
+    }
+  }
+}
+
+__device__ __forceinline__ void frame_vec(const float* __restrict__ src, float* __restrict__ dst, long long n) {
+  const float4* s = reinterpret_cast<const float4*>(src);
+  float4* d = reinterpret_cast<float4*>(dst);
+  const long long nv = n / 4;
+#pragma unroll 4
+  for (long long i = threadIdx.x; i < nv; i += kThreads) {
+    const float4 v = __ldg(s + i);
+    d[i] = normalise4(v.x, v.y, v.z, v.w);
+  }
+}
+
+template <typename S>
+__device__ __forceinline__ void frame_scalar(const S* __restrict__ src, float* __restrict__ dst, long long n) {
+  for (long long i = threadIdx.x; i < n; i += kThreads) dst[i] = normalise((float)src[i]);
+}
+
+template <typename S>
+__global__ void __launch_bounds__(kThreads) sequence_gather_kernel(const GatherArgs a) {
+  constexpr long long kVec = 16 / sizeof(S);  // elements per 16-byte load
+  const int per_seq = a.steps - 1;
+  const int frames = a.batch * per_seq;  // below 2^31: the entry point refuses more
+  const long long mask = (1LL << a.chunk_shift) - 1;
+  // the 16-byte path needs whole 16-byte pieces per frame on both sides; chunk bases are checked per frame below
+  const bool vec_rows = a.frame_elems % kVec == 0 && a.frame_elems % 4 == 0 &&
+                        (reinterpret_cast<uintptr_t>(a.obs_out) & 15) == 0;
+  for (int f = blockIdx.x; f < frames; f += gridDim.x) {
+    const int b = f / per_seq, t = f - b * per_seq;
+    const long long start = a.starts[b];
+    if (start < 0 || start + a.steps > a.rows) continue;  // the host refuses these before upload; never read past the store
+    // frame t + 1 of the sequence (the loss's obs[:, 1:]); action and reward t (action[:, :-1], rewards[:, :-1])
+    const long long row = start + t + 1;
+    const S* src = reinterpret_cast<const S*>(a.chunks[row >> a.chunk_shift]) + (row & mask) * a.frame_elems;
+    float* dst = a.obs_out + (long long)f * a.frame_elems;
+    if (vec_rows && (reinterpret_cast<uintptr_t>(src) & 15) == 0)
+      frame_vec(src, dst, a.frame_elems);
+    else
+      frame_scalar(src, dst, a.frame_elems);
+    const long long r = start + t;
+    for (int j = threadIdx.x; j < a.action_size; j += kThreads)
+      a.act_out[(long long)f * a.action_size + j] = a.act[r * a.action_size + j];
+    if (threadIdx.x == 0) a.rew_out[f] = a.rew[r];
+  }
+}
+
+int g_sms[64];  // SM count per device ordinal, read once
+
+}  // namespace
+
+extern "C" {
+
+int b200pets_sequence_gather(const b200pets_replay_desc* desc, const void* const* obs_chunks, const float* act,
+                             const float* rew, const int64_t* starts, int32_t batch, int32_t steps, float* obs_out,
+                             float* act_out, float* rew_out, void* stream) {
+  if (!desc || !obs_chunks || !act || !rew || !starts || !obs_out || !act_out || !rew_out)
+    return b200pets_set_error(B200PETS_EINVAL, "sequence_gather: NULL argument");
+  if (batch < 1 || steps < 2)
+    return b200pets_set_error(B200PETS_EINVAL, "sequence_gather: needs batch >= 1 and steps >= 2 (batch %d, steps %d)",
+                              batch, steps);
+  if (desc->dtype != B200PETS_DTYPE_U8 && desc->dtype != B200PETS_DTYPE_F32)
+    return b200pets_set_error(B200PETS_EINVAL, "sequence_gather: unknown storage dtype %d", desc->dtype);
+  if (desc->chunk_shift < 0 || desc->chunk_shift > B200PETS_REPLAY_MAX_CHUNK_SHIFT)
+    return b200pets_set_error(B200PETS_EINVAL, "sequence_gather: chunk_shift %d outside [0, %d]", desc->chunk_shift,
+                              B200PETS_REPLAY_MAX_CHUNK_SHIFT);
+  if (desc->frame_elems < 1 || desc->action_size < 1 || desc->rows < steps)
+    return b200pets_set_error(B200PETS_EINVAL,
+                              "sequence_gather: frame_elems %lld and action_size %d must be positive and rows %lld at "
+                              "least steps %d", (long long)desc->frame_elems, desc->action_size, (long long)desc->rows,
+                              steps);
+  if ((long long)batch * (steps - 1) > 0x7fffffffLL)
+    return b200pets_set_error(B200PETS_EUNSUPPORTED, "sequence_gather: more than 2^31 - 1 frames (batch %d, steps %d)",
+                              batch, steps);
+  int dev = 0;
+  CUDA_TRY(cudaGetDevice(&dev));
+  if (dev < 0 || dev >= 64) return b200pets_set_error(B200PETS_EUNSUPPORTED, "sequence_gather: device ordinal %d", dev);
+  if (g_sms[dev] == 0) CUDA_TRY(cudaDeviceGetAttribute(&g_sms[dev], cudaDevAttrMultiProcessorCount, dev));
+  GatherArgs a{};
+  a.frame_elems = desc->frame_elems;
+  a.rows = desc->rows;
+  a.action_size = desc->action_size;
+  a.chunk_shift = desc->chunk_shift;
+  a.batch = batch;
+  a.steps = steps;
+  a.chunks = obs_chunks;
+  a.act = act;
+  a.rew = rew;
+  a.starts = reinterpret_cast<const long long*>(starts);
+  a.obs_out = obs_out;
+  a.act_out = act_out;
+  a.rew_out = rew_out;
+  const long long frames = (long long)batch * (steps - 1);
+  const unsigned grid = (unsigned)(frames < (long long)g_sms[dev] * kCtasPerSm ? frames : (long long)g_sms[dev] * kCtasPerSm);
+  cudaStream_t s = (cudaStream_t)stream;
+  if (desc->dtype == B200PETS_DTYPE_U8)
+    sequence_gather_kernel<uint8_t><<<grid, kThreads, 0, s>>>(a);
+  else
+    sequence_gather_kernel<float><<<grid, kThreads, 0, s>>>(a);
+  CUDA_TRY(cudaGetLastError());
+  return B200PETS_OK;
+}
+
+}  // extern "C"

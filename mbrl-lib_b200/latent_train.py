@@ -22,16 +22,28 @@ Draws.  In-kernel Philox on ``RNG_STREAM_LATENT_TRAIN`` (csrc/common.cuh), keyed
 makes a run reproducible.  The draws are not the reference's ``torch.randn`` stream, and the ``rng`` is not advanced the
 way the reference's per-step ``torch.randn`` calls advance it.  ``eps=(eps_q, eps_p)``, each ``[T, B, L]``, replaces
 them (tests).
+
+Batches.  :func:`loss`, :func:`update` and :func:`eval_score` take the reference's ``TransitionBatch`` of B sequences of
+T rows, or a :class:`SequenceBatch`: the part of it the loss reads, already on the device and normalised, as
+``replay.DeviceReplayMirror`` gathers it.
 """
 from __future__ import annotations
 
 import ctypes as C
-from typing import Dict, List, Optional, Tuple
+from typing import Dict, List, NamedTuple, Optional, Tuple
 
 import torch
 import torch.nn.functional as F
 
 from . import _lib
+
+class SequenceBatch(NamedTuple):
+    """What PlaNet's loss reads of a batch of B sequences of T rows, on the model's device: ``next_obs`` [B, T-1,
+    *obs_shape] (frames 1 .. T-1 as ``x / 256 - 0.5``), ``act`` [B, T-1, A] and ``rewards`` [B, T-1] (rows 0 .. T-2)."""
+    next_obs: torch.Tensor
+    act: torch.Tensor
+    rewards: torch.Tensor
+
 
 _TAPE_FWD = ("e", "gates", "q1", "p1", "pre_std", "eps")
 _TAPE_BWD = ("de", "dgi", "dghn", "dq", "dv", "dp")
@@ -212,8 +224,11 @@ def _process_batch(model, batch):
 
 def _loss_terms(model, batch, eps=None):
     """Per-(b, t) observation, reward and KL losses and the reconstruction, as planet.py:429-462 computes them."""
-    obs, action, rewards = _process_batch(model, batch)
-    next_obs, act, rew = obs[:, 1:], action[:, :-1], rewards[:, :-1]
+    if isinstance(batch, SequenceBatch):
+        next_obs, act, rew = batch
+    else:
+        obs, action, rewards = _process_batch(model, batch)
+        next_obs, act, rew = obs[:, 1:], action[:, :-1], rewards[:, :-1]
     B, T = int(next_obs.shape[0]), int(next_obs.shape[1])
     Hb, L = model.belief_size, model.latent_state_size
     q1 = model.posterior_transition_model[0]

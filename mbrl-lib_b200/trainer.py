@@ -22,7 +22,13 @@ What runs where:
     ``b200pets_latent_train_supported`` accepts, with fp32 CUDA parameters and one Adam param group over
     ``model.parameters()``: the reference's loop below, with each batch through :func:`latent_train.update` and each
     evaluation batch through :func:`latent_train.eval_score` in place of the model's own methods.  ``batch_callback`` is
-    called per batch with the reference's arguments, as ``mbrl/algorithms/planet.py`` needs;
+    called per batch with the reference's arguments, as ``mbrl/algorithms/planet.py`` needs.  When the dataset is
+    mbrl-lib's ``SequenceTransitionSampler`` / ``SequenceTransitionIterator`` (recognised by their attributes and method
+    owners) over ``get_all()`` of a buffer mirrored on the model's device (:func:`replay.mirror_to_device`), and not a
+    bootstrapping iterator of several members, the batches are gathered on the device instead: the mirror is flushed
+    once at the start of ``train()`` / ``evaluate()``; per batch the start rows are drawn exactly as the iterator draws
+    them (the same batches, the buffer's ``rng`` advanced the same way), B int64 starts cross to the device, and one
+    ``b200pets_sequence_gather`` fills buffers reused for the whole call;
   * otherwise (a ``batch_callback`` on a GaussianMLP, which needs every batch's loss as it happens, another model, a
     model the kernels refuse -- more than 7 hidden layers, or layers too wide for the evaluation kernel's shared memory
     -- or transitions of another element type) the reference's PyTorch loop runs unchanged: ``model.update(batch,
@@ -39,7 +45,7 @@ from typing import Callable, Dict, List, Optional, Tuple
 import numpy as np
 import torch
 
-from . import _lib, functions, latent_train, staging
+from . import _lib, functions, latent_train, replay, staging
 
 MODEL_LOG_FORMAT = [
     ("train_iteration", "I", "int"),
@@ -68,6 +74,48 @@ def _iterator_kind(ds) -> Optional[str]:
     if cls.__name__ == "TransitionIterator":
         return "plain"
     return None
+
+
+_SEQUENCE_MRO = {"sampler": ("SequenceTransitionSampler", "TransitionIterator", "object"),
+                 "iterator": ("SequenceTransitionIterator", "BootstrapIterator", "TransitionIterator", "object")}
+
+
+def _sequence_kind(ds) -> Optional[str]:
+    """"sampler" / "iterator" for mbrl-lib's SequenceTransitionSampler / SequenceTransitionIterator (replay_buffer.py:
+    198-401) whose methods are those classes' own (a subclass that overrides any of them is neither), else None."""
+    if not all(hasattr(ds, a) for a in ("transitions", "_valid_starts", "_sequence_length", "batch_size", "num_stored",
+                                        "_current_batch", "_rng")):
+        return None
+    mro = tuple(c.__name__ for c in type(ds).__mro__)
+    if mro == _SEQUENCE_MRO["sampler"] and hasattr(ds, "_batches_per_loop"):
+        return "sampler"
+    if mro == _SEQUENCE_MRO["iterator"] and hasattr(ds, "_max_batches_per_loop") and hasattr(ds, "_bootstrap_iter") \
+            and hasattr(ds, "_order"):
+        return "iterator"
+    return None
+
+
+def sequence_starts(ds, kind: str):
+    """Yield, batch by batch, the start rows (int64 [B]) of the sequences ``for batch in ds`` forms, drawing from the
+    iterator's ``_rng`` exactly as that loop does: the sampler's ``_rng.choice(num_stored, batch_size, replace=True)``
+    until ``_batches_per_loop`` (replay_buffer.py:380-389), the iterator's ``iter()`` shuffle, ``_get_indices_next_batch``
+    and ``_max_batches_per_loop`` (:285-295); each through ``_valid_starts`` as ``_sequence_getitem_impl`` maps them."""
+    iter(ds)
+    valid = np.asarray(ds._valid_starts)
+    while True:
+        if kind == "sampler":
+            if ds._current_batch >= ds._batches_per_loop:
+                return
+            ds._current_batch += 1
+            idx = ds._rng.choice(ds.num_stored, size=ds.batch_size, replace=True)
+        else:
+            if ds._max_batches_per_loop is not None and ds._current_batch >= ds._max_batches_per_loop:
+                return
+            try:
+                idx = ds._get_indices_next_batch()
+            except StopIteration:
+                return
+        yield valid[idx].astype(np.int64)
 
 
 class _DeviceModel:
@@ -271,6 +319,7 @@ class ModelTrainer:
         self.optimizer = torch.optim.Adam(self.model.parameters(), lr=optim_lr, weight_decay=weight_decay, eps=optim_eps)
         self._dev: Optional[_DeviceModel] = None
         self._latent = False
+        self._gathers: Dict[int, replay.SequenceGather] = {}
 
     # ---- which path ----------------------------------------------------------------------------------------------
     def _device_supported(self) -> bool:
@@ -320,6 +369,37 @@ class ModelTrainer:
             return latent_train.eval_score(self.model, batch)
         return self.model.eval_score(batch)
 
+    def _mirror_of(self, ds):
+        """(mirror, kind) when the latent path gathers ``ds``'s batches from a replay mirror (module docstring)."""
+        kind = _sequence_kind(ds) if self._latent and ds is not None else None
+        if kind is None or int(ds._sequence_length) < 2:
+            return None
+        mirror = replay.find_mirror(ds.transitions)
+        if mirror is None or mirror.device != next(self.model.parameters()).device:
+            return None
+        return mirror, kind
+
+    def _flush_mirrors(self, *datasets):
+        for ds in datasets:
+            found = self._mirror_of(ds)
+            if found is not None:
+                found[0].flush()
+
+    def _batches(self, ds):
+        """``ds`` itself, or the same batches gathered from its buffer's mirror."""
+        found = self._mirror_of(ds)
+        if found is None or (found[1] == "iterator" and ds._bootstrap_iter):
+            return ds
+        return self._gathered(ds, *found)
+
+    def _gathered(self, ds, mirror, kind):
+        g = self._gathers.get(id(mirror))
+        if g is None:
+            g = self._gathers[id(mirror)] = replay.SequenceGather(mirror)
+        T, limit = int(ds._sequence_length), len(ds.transitions.obs)
+        for starts in sequence_starts(ds, kind):
+            yield g(starts, T, limit)
+
     @staticmethod
     def _store_supported(ds) -> bool:
         return transition_dtype(ds.transitions) is not None
@@ -341,9 +421,11 @@ class ModelTrainer:
         device = not self._latent and batch_callback is None and self._device_supported()
         self._dev = None
         try:
+            self._flush_mirrors(dataset_train, dataset_val)
             return self._train(dataset_train, dataset_val, num_epochs, patience, improvement_threshold, callback,
                                batch_callback, evaluate, silent, device)
         finally:
+            self._gathers = {}
             if self._dev is not None:
                 self._dev.close()
                 self._dev = None
@@ -362,7 +444,7 @@ class ModelTrainer:
                 batch_losses = self._device_epoch(dataset_train)
             else:
                 batch_losses = []
-                for batch in dataset_train:
+                for batch in self._batches(dataset_train):
                     loss, meta = self._model_update(batch)
                     batch_losses.append(loss)
                     if batch_callback_epoch:
@@ -452,14 +534,18 @@ class ModelTrainer:
                 if self._dev is not None:
                     self._dev.close()
                     self._dev = None
-        return self._evaluate(dataset, batch_callback, self._dev is not None)
+        try:
+            self._flush_mirrors(dataset)
+            return self._evaluate(dataset, batch_callback, self._dev is not None)
+        finally:
+            self._gathers = {}
 
     def _evaluate_reference(self, dataset, batch_callback=None) -> torch.Tensor:
         bootstrap = hasattr(dataset, "toggle_bootstrap")
         if bootstrap:
             dataset.toggle_bootstrap()
         batch_scores_list = []
-        for batch in dataset:
+        for batch in self._batches(dataset):
             batch_score, meta = self._model_eval_score(batch)
             batch_scores_list.append(batch_score)
             if batch_callback:
