@@ -472,6 +472,31 @@ int b200pets_latent_cem_plan(b200pets_latent_model_t model, const b200pets_rollo
                              const float* upper, const float* z, const float* eps, float* solution, float* values_out,
                              void* workspace, size_t workspace_bytes, void* stream);
 
+/* The two calls above for K = num_problems posteriors at once (K environments, episodes or seeds): one rollout launch
+ * per evaluation for all K, tiles problem-major, rows per CTA chosen from K * N * P rows (b200pets_latent_plan_info of
+ * that count).  Problem k gives, bit for bit, what the single call gives for its inputs at Philox offset
+ * offset + k * 1024 (evaluation) or with counter offset + k, i.e. (offset + k) * 1024 + iteration (plan): a batch
+ * takes the counter values of K consecutive single calls.  Refused before anything touches the device:
+ * num_problems < 1, a sharded cfg, a precision other than f32, a NULL required pointer, a workspace too small.
+ *   latent0 [dev] float[K][L], belief0 [dev] float[K][Hb]: posterior k
+ *   evaluation: actions [dev] float[K][N][H][A]; eps [dev] float[K][H][B][L] or NULL; returns [dev] float[K][N];
+ *     row_returns [dev] float[K][B] or NULL
+ *   plan: x0, solution [dev] float[K][H*A]; lower, upper [dev] float[H*A] shared by all problems;
+ *     z [dev] float[K][it][N][H*A] or NULL; eps [dev] float[K][it][H][B][L] or NULL; values_out [dev] float[K][it][N]
+ *     or NULL.  The plan runs b200pets_cem_plan_batch's launches around the batched latent rollout. */
+size_t b200pets_latent_eval_batch_workspace_bytes(b200pets_latent_model_t model, const b200pets_rollout_cfg* cfg,
+                                                  int32_t num_problems);
+int b200pets_latent_eval_sequences_batch(b200pets_latent_model_t model, const b200pets_rollout_cfg* cfg, int32_t num_problems,
+                                         const float* latent0, const float* belief0, const float* actions, const float* eps,
+                                         float* returns, float* row_returns, void* workspace, size_t workspace_bytes,
+                                         void* stream);
+size_t b200pets_latent_cem_plan_batch_workspace_bytes(b200pets_latent_model_t model, const b200pets_rollout_cfg* rcfg,
+                                                      const b200pets_cem_cfg* ccfg, int32_t num_problems);
+int b200pets_latent_cem_plan_batch(b200pets_latent_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg,
+                                   int32_t num_problems, const float* latent0, const float* belief0, const float* x0,
+                                   const float* lower, const float* upper, const float* z, const float* eps, float* solution,
+                                   float* values_out, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- Training PlaNet's latent model: the recurrence of PlaNetModel.forward (planet.py:354-404) ------------------
  * The belief GRU, the posterior and the prior over T steps from s0 = 0, h0 = 0 (planet.py:364-367), in fp32 FFMA:
  *   e = relu(W_e [s, a_t] + b_e);  h = GRUCell(e, h);

@@ -173,6 +173,12 @@ _SIGNATURES = {
     "b200pets_latent_cem_plan_workspace_bytes": (C.c_size_t, [_P, C.POINTER(RolloutCfg), C.POINTER(CemCfg)]),
     "b200pets_latent_cem_plan": (C.c_int, [_P, C.POINTER(RolloutCfg), C.POINTER(CemCfg), _P, _P, _P, _P, _P, _P, _P, _P, _P,
                                            _P, C.c_size_t, _P]),
+    "b200pets_latent_eval_batch_workspace_bytes": (C.c_size_t, [_P, C.POINTER(RolloutCfg), C.c_int32]),
+    "b200pets_latent_eval_sequences_batch": (C.c_int, [_P, C.POINTER(RolloutCfg), C.c_int32, _P, _P, _P, _P, _P, _P, _P,
+                                                       C.c_size_t, _P]),
+    "b200pets_latent_cem_plan_batch_workspace_bytes": (C.c_size_t, [_P, C.POINTER(RolloutCfg), C.POINTER(CemCfg), C.c_int32]),
+    "b200pets_latent_cem_plan_batch": (C.c_int, [_P, C.POINTER(RolloutCfg), C.POINTER(CemCfg), C.c_int32, _P, _P, _P, _P, _P,
+                                                 _P, _P, _P, _P, _P, C.c_size_t, _P]),
     "b200pets_latent_train_supported": (C.c_int, [C.POINTER(LatentTrainDesc)]),
     "b200pets_latent_train_workspace_bytes": (C.c_size_t, [C.POINTER(LatentTrainDesc), C.c_int32, C.c_int32]),
     "b200pets_latent_train_plan_info": (C.c_int, [C.POINTER(LatentTrainDesc), C.c_int32, C.c_int32,

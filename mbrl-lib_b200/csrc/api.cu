@@ -736,6 +736,8 @@ int b200pets_eval_sequences_batch(b200pets_model_t model, const b200pets_rollout
   return launch_particle_mean(num_problems * N, cfg->particles, total, returns, stream);  // model_env.py:190-191
 }
 
+}  // extern "C"
+
 namespace {
 __global__ void cem_init_batch_kernel(int K, int dims, const float* __restrict__ x0, const float* __restrict__ lb,
                                       const float* __restrict__ ub, int clipped, float* mu, float* disp, float* best_value) {
@@ -756,10 +758,10 @@ struct PlanBatchLayout {
   size_t pop, values, mu, disp, best_sol, best_val, upd, eval, total;
   size_t upd_bytes;  // one problem's refit workspace
 };
-PlanBatchLayout plan_batch_layout(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg, int K) {
-  const size_t N = rcfg->population, dims = (size_t)rcfg->horizon * model->desc.act_dim;
+// N sequences of `dims` values per problem; eval_bytes: the batched evaluation's workspace
+PlanBatchLayout plan_batch_layout(size_t N, size_t dims, int elite_num, size_t eval_bytes, int K) {
   PlanBatchLayout l{};
-  l.upd_bytes = al256(b200pets_cem_update_workspace_bytes((int)N, (int)dims, ccfg->elite_num));
+  l.upd_bytes = al256(b200pets_cem_update_workspace_bytes((int)N, (int)dims, elite_num));
   size_t off = 0;
   l.pop = off; off += al256(K * N * dims * 4);
   l.values = off; off += al256(K * N * 4);
@@ -768,36 +770,26 @@ PlanBatchLayout plan_batch_layout(b200pets_model_t model, const b200pets_rollout
   l.best_sol = off; off += al256(K * dims * 4);
   l.best_val = off; off += (size_t)K * 256;  // per problem: best value, refit flag
   l.upd = off; off += (size_t)K * l.upd_bytes;
-  l.eval = off; off += al256(b200pets_eval_batch_workspace_bytes(model, rcfg, K));
+  l.eval = off; off += al256(eval_bytes);
   l.total = off;
   return l;
 }
-}  // namespace
-
-size_t b200pets_cem_plan_batch_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg,
-                                               int32_t num_problems) {
-  if (!model || !rcfg || !ccfg || num_problems < 1) return 0;
-  return plan_batch_layout(model, rcfg, ccfg, num_problems).total;
+PlanBatchLayout plan_batch_layout(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg, int K) {
+  return plan_batch_layout(rcfg->population, (size_t)rcfg->horizon * model->desc.act_dim, ccfg->elite_num,
+                           b200pets_eval_batch_workspace_bytes(model, rcfg, K), K);
 }
 
-int b200pets_cem_plan_batch(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg,
-                            int32_t num_problems, const float* obs0, const float* x0, const float* lower, const float* upper,
-                            const float* z, const float* eps, const int64_t* perms, float* solution, float* values_out,
-                            void* workspace, size_t workspace_bytes, void* stream_) {
-  if (!model || !rcfg || !ccfg) return b200pets_set_error(B200PETS_EINVAL, "cem_plan_batch: null argument");
-  { int rc = check_batch(model, rcfg, num_problems, "cem_plan_batch"); if (rc) return rc; }
-  if (!obs0 || !x0 || !lower || !upper || !solution || !workspace)
-    return b200pets_set_error(B200PETS_EINVAL, "cem_plan_batch: null argument");
-  const int K = num_problems;
-  if (workspace_bytes < b200pets_cem_plan_batch_workspace_bytes(model, rcfg, ccfg, K))
-    return b200pets_set_error(B200PETS_EINVAL, "cem_plan_batch: workspace too small");
-  cudaStream_t stream = (cudaStream_t)stream_;
-  const b200pets_model_desc& d = model->desc;
-  const int N = rcfg->population, H = rcfg->horizon, P = rcfg->particles, A = d.act_dim, iters = ccfg->num_iterations;
-  const int dims = H * A;
+// The K plans of a batched CEM plan in the workspace `ws` laid out as `l`, around `rollout(it, pop, totals)`: the
+// batched rollout of iteration it, which leaves problem k's per-row totals at totals + k * N * P.  The default plan of
+// b200pets_cem_plan for every problem: rollout, then one kernel that refits and draws the next population (2 launches per
+// iteration for the whole batch).  Outside the single-CTA refit, the sample and refit kernels run once per problem around
+// the batched rollout.  Problem k draws its populations with counter rcfg->offset + k, as its single plan would.
+template <class Rollout>
+int cem_plan_batch_run(const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg, int K, int dims, const PlanBatchLayout& l,
+                       unsigned char* ws, float* totals, const float* x0, const float* lower, const float* upper, const float* z,
+                       float* solution, float* values_out, cudaStream_t stream, Rollout rollout) {
+  const int N = rcfg->population, P = rcfg->particles, iters = ccfg->num_iterations;
   const long long B = (long long)N * P;
-  const PlanBatchLayout l = plan_batch_layout(model, rcfg, ccfg, K);
-  unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
   float* pop = reinterpret_cast<float*>(ws + l.pop);
   float* values = reinterpret_cast<float*>(ws + l.values);
   float* mu = reinterpret_cast<float*>(ws + l.mu);
@@ -805,18 +797,12 @@ int b200pets_cem_plan_batch(b200pets_model_t model, const b200pets_rollout_cfg* 
   float* best_sol = reinterpret_cast<float*>(ws + l.best_sol);
   float* best_val = reinterpret_cast<float*>(ws + l.best_val);
   unsigned char* upd_ws = ws + l.upd;
-  void* eval_ws = ws + l.eval;
-  float* totals = reinterpret_cast<float*>(ws + l.eval + al256((size_t)K * B * d.obs_dim * sizeof(float)));
   const long long popk = (long long)N * dims;  // per-problem strides
-  const int nperm = rcfg->propagation == B200PETS_PROP_FIXED_MODEL ? 1 : H;
 
   const long long tot = (long long)K * dims;
   cem_init_batch_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, stream>>>(K, dims, x0, lower, upper, ccfg->clipped_normal, mu, disp,
                                                                           best_val);
   CUDA_TRY(cudaGetLastError());
-  // The default plan of b200pets_cem_plan for every problem: rollout, then one kernel that refits and draws the next
-  // population (2 launches per iteration for the whole batch).  Outside the single-CTA refit, the sample and refit kernels
-  // run once per problem around the batched rollout.
   const bool merged = cem_refit_sample_supported(N, dims, ccfg->elite_num);
   auto next_pop = [&](int it_next, int refit) -> int {  // refit of it_next - 1 (if any) + population of it_next
     const int sample = it_next < iters;
@@ -839,11 +825,7 @@ int b200pets_cem_plan_batch(b200pets_model_t model, const b200pets_rollout_cfg* 
                                             (rcfg->offset + k) * 1024 + it, ccfg->clipped_normal, pop + (size_t)k * popk, stream);
         if (rcs) return rcs;
       }
-    b200pets_rollout_cfg rc_it = *rcfg;
-    rc_it.offset = rcfg->offset * 1024 + it;
-    int rc = eval_rows_batch(model, &rc_it, K, obs0, pop, popk, perms ? perms + (size_t)it * nperm * B : nullptr,
-                             (long long)iters * nperm * B, eps ? eps + (size_t)it * H * B * d.out_size : nullptr,
-                             (long long)iters * H * B * d.out_size, totals, eval_ws, stream, 1024);
+    int rc = rollout(it, pop, totals);
     if (rc) return rc;
     if (merged) {
       rc = next_pop(it + 1, 1);
@@ -864,6 +846,46 @@ int b200pets_cem_plan_batch(b200pets_model_t model, const b200pets_rollout_cfg* 
   CUDA_TRY(cudaMemcpyAsync(solution, ccfg->return_mean_elites ? mu : best_sol, sizeof(float) * K * dims, cudaMemcpyDeviceToDevice,
                            stream));
   return B200PETS_OK;
+}
+}  // namespace
+
+extern "C" {
+
+size_t b200pets_cem_plan_batch_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg,
+                                               int32_t num_problems) {
+  if (!model || !rcfg || !ccfg || num_problems < 1) return 0;
+  return plan_batch_layout(model, rcfg, ccfg, num_problems).total;
+}
+
+int b200pets_cem_plan_batch(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg,
+                            int32_t num_problems, const float* obs0, const float* x0, const float* lower, const float* upper,
+                            const float* z, const float* eps, const int64_t* perms, float* solution, float* values_out,
+                            void* workspace, size_t workspace_bytes, void* stream_) {
+  if (!model || !rcfg || !ccfg) return b200pets_set_error(B200PETS_EINVAL, "cem_plan_batch: null argument");
+  { int rc = check_batch(model, rcfg, num_problems, "cem_plan_batch"); if (rc) return rc; }
+  if (!obs0 || !x0 || !lower || !upper || !solution || !workspace)
+    return b200pets_set_error(B200PETS_EINVAL, "cem_plan_batch: null argument");
+  const int K = num_problems;
+  if (workspace_bytes < b200pets_cem_plan_batch_workspace_bytes(model, rcfg, ccfg, K))
+    return b200pets_set_error(B200PETS_EINVAL, "cem_plan_batch: workspace too small");
+  cudaStream_t stream = (cudaStream_t)stream_;
+  const b200pets_model_desc& d = model->desc;
+  const int N = rcfg->population, H = rcfg->horizon, P = rcfg->particles, dims = H * d.act_dim, iters = ccfg->num_iterations;
+  const long long B = (long long)N * P;
+  const PlanBatchLayout l = plan_batch_layout(model, rcfg, ccfg, K);
+  unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
+  void* eval_ws = ws + l.eval;
+  float* totals = reinterpret_cast<float*>(ws + l.eval + al256((size_t)K * B * d.obs_dim * sizeof(float)));
+  const int nperm = rcfg->propagation == B200PETS_PROP_FIXED_MODEL ? 1 : H;
+  return cem_plan_batch_run(rcfg, ccfg, K, dims, l, ws, totals, x0, lower, upper, z, solution, values_out, stream,
+                            [&](int it, const float* pop, float* tot) {
+                              b200pets_rollout_cfg rc_it = *rcfg;
+                              rc_it.offset = rcfg->offset * 1024 + it;
+                              return eval_rows_batch(model, &rc_it, K, obs0, pop, (long long)N * dims,
+                                                     perms ? perms + (size_t)it * nperm * B : nullptr, (long long)iters * nperm * B,
+                                                     eps ? eps + (size_t)it * H * B * d.out_size : nullptr,
+                                                     (long long)iters * H * B * d.out_size, tot, eval_ws, stream, 1024);
+                            });
 }
 
 namespace {
@@ -1456,6 +1478,93 @@ int b200pets_latent_cem_plan(b200pets_latent_model_t model, const b200pets_rollo
   }
   CUDA_TRY(cudaMemcpyAsync(solution, ccfg->return_mean_elites ? mu : best_sol, sizeof(float) * dims, cudaMemcpyDeviceToDevice, stream));
   return B200PETS_OK;
+}
+
+// Batches of K posteriors: one batched rollout launch per evaluation, the plan of b200pets_cem_plan_batch around it
+size_t b200pets_latent_eval_batch_workspace_bytes(b200pets_latent_model_t model, const b200pets_rollout_cfg* cfg,
+                                                  int32_t num_problems) {
+  if (!model || !cfg || num_problems < 1) return 0;
+  return al256((size_t)num_problems * cfg->population * cfg->particles * sizeof(float));
+}
+
+static int latent_check_batch(b200pets_latent_model_t model, const b200pets_rollout_cfg* cfg, int32_t num_problems,
+                              const char* who) {
+  if (!model || !cfg) return b200pets_set_error(B200PETS_EINVAL, "%s: null argument", who);
+  if (num_problems < 1) return b200pets_set_error(B200PETS_EINVAL, "%s: num_problems must be at least 1 (got %d)", who, num_problems);
+  return latent_check_cfg(cfg, who);
+}
+
+// problem k of a batch: posterior k, its slice of every per-problem array, Philox offset a.offset + k * offset_step
+static LatentBatch latent_batch_strides(const b200pets_latent_model_desc& d, const b200pets_rollout_cfg* cfg, long long eps_stride,
+                                        unsigned long long offset_step) {
+  LatentBatch bt{};
+  const long long B = (long long)cfg->population * cfg->particles;
+  bt.latent0 = d.latent_size;
+  bt.belief0 = d.belief_size;
+  bt.act = (long long)cfg->population * cfg->horizon * d.action_size;
+  bt.eps = eps_stride;
+  bt.rows = B;
+  bt.seed = cfg->seed;
+  bt.offset_step = offset_step;
+  return bt;
+}
+
+int b200pets_latent_eval_sequences_batch(b200pets_latent_model_t model, const b200pets_rollout_cfg* cfg, int32_t num_problems,
+                                         const float* latent0, const float* belief0, const float* actions, const float* eps,
+                                         float* returns, float* row_returns, void* workspace, size_t workspace_bytes,
+                                         void* stream_) {
+  { int rc = latent_check_batch(model, cfg, num_problems, "latent_eval_sequences_batch"); if (rc) return rc; }
+  if (!latent0 || !belief0 || !actions || !returns || !workspace)
+    return b200pets_set_error(B200PETS_EINVAL, "latent_eval_sequences_batch: null argument");
+  if (workspace_bytes < b200pets_latent_eval_batch_workspace_bytes(model, cfg, num_problems))
+    return b200pets_set_error(B200PETS_EINVAL, "latent_eval_sequences_batch: workspace too small");
+  cudaStream_t stream = (cudaStream_t)stream_;
+  const long long B = (long long)cfg->population * cfg->particles;
+  float* totals = row_returns ? row_returns : reinterpret_cast<float*>(workspace);
+  LatentArgs a;
+  latent_rollout_args(cfg, cfg->offset, latent0, belief0, actions, eps, totals, &a);
+  int rc = launch_latent_rollout_batch(model->dev, a, num_problems,
+                                       latent_batch_strides(model->desc, cfg, (long long)cfg->horizon * B * model->desc.latent_size, 1024),
+                                       stream);
+  if (rc) return rc;
+  // problem k's totals are rows k * B .. k * B + B - 1: one particle mean over K * N sequences
+  return launch_particle_mean(num_problems * cfg->population, cfg->particles, totals, returns, stream);  // model_env.py:190-191
+}
+
+size_t b200pets_latent_cem_plan_batch_workspace_bytes(b200pets_latent_model_t model, const b200pets_rollout_cfg* rcfg,
+                                                      const b200pets_cem_cfg* ccfg, int32_t num_problems) {
+  if (!model || !rcfg || !ccfg || num_problems < 1) return 0;
+  return plan_batch_layout(rcfg->population, (size_t)rcfg->horizon * model->desc.action_size, ccfg->elite_num,
+                           b200pets_latent_eval_batch_workspace_bytes(model, rcfg, num_problems), num_problems).total;
+}
+
+int b200pets_latent_cem_plan_batch(b200pets_latent_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg,
+                                   int32_t num_problems, const float* latent0, const float* belief0, const float* x0,
+                                   const float* lower, const float* upper, const float* z, const float* eps, float* solution,
+                                   float* values_out, void* workspace, size_t workspace_bytes, void* stream_) {
+  { int rc = latent_check_batch(model, rcfg, num_problems, "latent_cem_plan_batch"); if (rc) return rc; }
+  if (!ccfg || !latent0 || !belief0 || !x0 || !lower || !upper || !solution || !workspace)
+    return b200pets_set_error(B200PETS_EINVAL, "latent_cem_plan_batch: null argument");
+  if (ccfg->num_iterations < 0 || ccfg->elite_num < 1 || ccfg->elite_num > rcfg->population)
+    return b200pets_set_error(B200PETS_EINVAL, "latent_cem_plan_batch: %d iterations, %d elites of %d", ccfg->num_iterations,
+                              ccfg->elite_num, rcfg->population);
+  const int K = num_problems;
+  if (workspace_bytes < b200pets_latent_cem_plan_batch_workspace_bytes(model, rcfg, ccfg, K))
+    return b200pets_set_error(B200PETS_EINVAL, "latent_cem_plan_batch: workspace too small");
+  const int H = rcfg->horizon, L = model->desc.latent_size, iters = ccfg->num_iterations;
+  const int dims = H * model->desc.action_size;
+  const long long B = (long long)rcfg->population * rcfg->particles;
+  const PlanBatchLayout l = plan_batch_layout(rcfg->population, dims, ccfg->elite_num,
+                                              b200pets_latent_eval_batch_workspace_bytes(model, rcfg, K), K);
+  unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
+  const LatentBatch bt = latent_batch_strides(model->desc, rcfg, (long long)iters * H * B * L, 1024);
+  return cem_plan_batch_run(rcfg, ccfg, K, dims, l, ws, reinterpret_cast<float*>(ws + l.eval), x0, lower, upper, z, solution,
+                            values_out, (cudaStream_t)stream_, [&](int it, const float* pop, float* totals) {
+                              LatentArgs a;
+                              latent_rollout_args(rcfg, rcfg->offset * 1024 + it, latent0, belief0, pop,
+                                                  eps ? eps + (size_t)it * H * B * L : nullptr, totals, &a);
+                              return launch_latent_rollout_batch(model->dev, a, K, bt, (cudaStream_t)stream_);
+                            });
 }
 
 // ---------------------------------------------------------------------------------------------------------

@@ -334,20 +334,21 @@ static __host__ __device__ inline unsigned long long rng_key(unsigned long long 
   return seed ^ (offset & 0xFFFFFFFF00000000ull);
 }
 
-// Problem k of a batched launch (BatchArgs): the element offset of its slice of a per-problem array, its Philox offset
-// and key.  With BATCH = false (single launches) these are 0, a.offset and a.seed, and `bt` is never read.
-template <bool BATCH>
-__device__ __forceinline__ long long prob_off(const BatchArgs* bt, long long k, long long BatchArgs::*stride) {
+// Problem k of a batched launch (BatchArgs, or latent.cuh's LatentBatch): the element offset of its slice of a per-problem
+// array, its Philox offset and key.  With BATCH = false (single launches) these are 0, a.offset and a.seed, and `bt` is
+// never read.
+template <bool BATCH, class Batch>
+__device__ __forceinline__ long long prob_off(const Batch* bt, long long k, long long Batch::*stride) {
   if constexpr (BATCH) return k * (bt->*stride);
   else return 0;
 }
-template <bool BATCH>
-__device__ __forceinline__ unsigned long long prob_offset(const RolloutArgs& a, const BatchArgs* bt, long long k) {
+template <bool BATCH, class Args, class Batch>
+__device__ __forceinline__ unsigned long long prob_offset(const Args& a, const Batch* bt, long long k) {
   if constexpr (BATCH) return a.offset + (unsigned long long)k * bt->offset_step;
   else return a.offset;
 }
-template <bool BATCH>
-__device__ __forceinline__ unsigned long long prob_seed(const RolloutArgs& a, const BatchArgs* bt, long long k) {
+template <bool BATCH, class Args, class Batch>
+__device__ __forceinline__ unsigned long long prob_seed(const Args& a, const Batch* bt, long long k) {
   if constexpr (BATCH) return rng_key(bt->seed, prob_offset<BATCH>(a, bt, k));
   else return a.seed;
 }

@@ -10,8 +10,10 @@
 
 namespace {
 
-template <int R>
-__global__ void __launch_bounds__(kLatentThreads, 1) latent_rollout_kernel(const LatentDev m, const LatentArgs a) {
+// The kernels' body.  BATCH: K problems in one launch (LatentBatch): CTA j runs local tile j % bt->tiles of problem
+// j / bt->tiles, and everything after that decode is the single-problem code.
+template <int R, bool BATCH>
+__device__ __forceinline__ void latent_rollout_body(const LatentDev& m, const LatentArgs& a, const LatentBatch* bt) {
   extern __shared__ float4 smem4[];
   float* smem = reinterpret_cast<float*>(smem4);
   const int VS = latent_v_stride(m), GS = latent_g_stride(m);
@@ -20,7 +22,9 @@ __global__ void __launch_bounds__(kLatentThreads, 1) latent_rollout_kernel(const
   float* T = G + R * GS;
   const int oH = m.Hb4, oS = 2 * m.Hb4, oA = 2 * m.Hb4 + m.L4;  // the embedding sits at 0
   const int tid = threadIdx.x;
-  const long long row0 = (long long)blockIdx.x * R;
+  long long kp = 0;  // problem of a batched launch
+  long long row0 = (long long)blockIdx.x * R;
+  if constexpr (BATCH) { kp = blockIdx.x / bt->tiles; row0 = (blockIdx.x - kp * bt->tiles) * R; }
   const int A = m.A, L = m.L, Hb = m.Hb, Hf = m.Hf;
 
   // padding must read as zeros (it meets zero weight rows); rows past B run on zeros and store nothing
@@ -29,18 +33,21 @@ __global__ void __launch_bounds__(kLatentThreads, 1) latent_rollout_kernel(const
   for (int i = tid; i < R * Hb; i += kLatentThreads) {
     const int r = i / Hb, c = i % Hb;
     const long long row = row0 + r;
-    if (row < a.B) V[r * VS + oH + c] = a.belief0 ? a.belief0[c] : a.belief_in[row * Hb + c];
+    if (row < a.B)
+      V[r * VS + oH + c] = a.belief0 ? (a.belief0 + prob_off<BATCH>(bt, kp, &LatentBatch::belief0))[c] : a.belief_in[row * Hb + c];
   }
   for (int i = tid; i < R * L; i += kLatentThreads) {
     const int r = i / L, c = i % L;
     const long long row = row0 + r;
-    if (row < a.B) V[r * VS + oS + c] = a.latent0 ? a.latent0[c] : a.latent_in[row * L + c];
+    if (row < a.B)
+      V[r * VS + oS + c] = a.latent0 ? (a.latent0 + prob_off<BATCH>(bt, kp, &LatentBatch::latent0))[c] : a.latent_in[row * L + c];
   }
   auto load_actions = [&](int t) {
     for (int i = tid; i < R * A; i += kLatentThreads) {
       const int r = i / A, j = i % A;
       const long long row = row0 + r;
-      if (row < a.B) V[r * VS + oA + j] = a.act[(row / a.P) * (long long)a.H * A + (long long)t * A + j];
+      if (row < a.B)
+        V[r * VS + oA + j] = (a.act + prob_off<BATCH>(bt, kp, &LatentBatch::act))[(row / a.P) * (long long)a.H * A + (long long)t * A + j];
     }
   };
   load_actions(0);
@@ -95,9 +102,10 @@ __global__ void __launch_bounds__(kLatentThreads, 1) latent_rollout_kernel(const
       if (a.sample && row < a.B) {
         float e;
         if (a.eps) {
-          e = a.eps[((long long)t * a.B + row) * L + j];
+          e = (a.eps + prob_off<BATCH>(bt, kp, &LatentBatch::eps))[((long long)t * a.B + row) * L + j];
         } else {
-          e = latent_draw((uint32_t)row, (uint32_t)t, RNG_STREAM_LATENT, j, (uint32_t)a.offset, a.seed);
+          e = latent_draw((uint32_t)row, (uint32_t)t, RNG_STREAM_LATENT, j, (uint32_t)prob_offset<BATCH>(a, bt, kp),
+                          prob_seed<BATCH>(a, bt, kp));
         }
         const float sd = softplus_f(p[L + j]) + m.min_std;
         s = s + sd * e;
@@ -128,9 +136,11 @@ __global__ void __launch_bounds__(kLatentThreads, 1) latent_rollout_kernel(const
     __syncthreads();
   }
 
+  float* totals = a.totals;
+  if constexpr (BATCH) totals += prob_off<BATCH>(bt, kp, &LatentBatch::rows);
   for (int r = tid; r < R; r += kLatentThreads) {
     const long long row = row0 + r;
-    if (a.totals && row < a.B) a.totals[row] = T[r];
+    if (totals && row < a.B) totals[row] = T[r];
   }
   if (a.latent_out)
     for (int i = tid; i < R * L; i += kLatentThreads) {
@@ -144,6 +154,19 @@ __global__ void __launch_bounds__(kLatentThreads, 1) latent_rollout_kernel(const
       const long long row = row0 + r;
       if (row < a.B) a.belief_out[row * Hb + c] = V[r * VS + oH + c];
     }
+}
+
+template <int R>
+__global__ void __launch_bounds__(kLatentThreads, 1) latent_rollout_kernel(const LatentDev m, const LatentArgs a) {
+  latent_rollout_body<R, false>(m, a, nullptr);
+}
+
+// K independent evaluations in one launch
+template <int R>
+__global__ void __launch_bounds__(kLatentThreads, 1)
+    latent_rollout_batch_kernel(const __grid_constant__ LatentDev m, const __grid_constant__ LatentArgs a,
+                                const __grid_constant__ LatentBatch bt) {
+  latent_rollout_body<R, true>(m, a, &bt);
 }
 
 // dst[kp][n] (Kp x N) from torch's [out, in] weights: row kp < n0 is input column coff0 + kp of src0, rows
@@ -286,6 +309,16 @@ static int launch_rows(const LatentDev& m, const LatentArgs& a, const LatentPlan
   return B200PETS_OK;
 }
 
+template <int R>
+static int launch_rows_batch(const LatentDev& m, const LatentArgs& a, const LatentPlan& p, int num_problems,
+                             LatentBatch bt, cudaStream_t stream) {
+  bt.tiles = (a.B + R - 1) / R;
+  CUDA_TRY(cudaFuncSetAttribute(latent_rollout_batch_kernel<R>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
+  latent_rollout_batch_kernel<R><<<(unsigned)(bt.tiles * num_problems), kLatentThreads, p.smem, stream>>>(m, a, bt);
+  CUDA_TRY(cudaGetLastError());
+  return B200PETS_OK;
+}
+
 int launch_latent_rollout(const LatentDev& m, const LatentArgs& a, cudaStream_t stream) {
   LatentPlan p;
   int rc = latent_plan(m, a.B, &p);
@@ -298,5 +331,22 @@ int launch_latent_rollout(const LatentDev& m, const LatentArgs& a, cudaStream_t 
     case 8: return launch_rows<8>(m, a, p, stream);
     case 16: return launch_rows<16>(m, a, p, stream);
     default: return launch_rows<32>(m, a, p, stream);
+  }
+}
+
+int launch_latent_rollout_batch(const LatentDev& m, const LatentArgs& a, int num_problems, LatentBatch bt, cudaStream_t stream) {
+  if (!a.latent0 || !a.belief0 || a.latent_out || a.belief_out || a.reward_out)
+    return b200pets_set_error(B200PETS_EUNSUPPORTED, "batched latent rollout: evaluations from a posterior only");
+  LatentPlan p;
+  int rc = latent_plan(m, (long long)num_problems * a.B, &p);
+  if (rc) return rc;
+  if (a.B == 0) return B200PETS_OK;
+  switch (p.rows) {
+    case 1: return launch_rows_batch<1>(m, a, p, num_problems, bt, stream);
+    case 2: return launch_rows_batch<2>(m, a, p, num_problems, bt, stream);
+    case 4: return launch_rows_batch<4>(m, a, p, num_problems, bt, stream);
+    case 8: return launch_rows_batch<8>(m, a, p, num_problems, bt, stream);
+    case 16: return launch_rows_batch<16>(m, a, p, num_problems, bt, stream);
+    default: return launch_rows_batch<32>(m, a, p, num_problems, bt, stream);
   }
 }

@@ -39,6 +39,18 @@ struct LatentArgs {
   float* reward_out;        // [B] reward of the last step, or NULL
 };
 
+// A batched launch of the rollout: K evaluations of one LatentArgs in one grid (a.B rows each).  Tiles are
+// problem-major (tile = k * tiles + local tile), so no tile holds two problems.  Problem k starts from
+// latent0 + k * latent0 and belief0 + k * belief0, reads act + k * act and eps + k * eps, writes totals + k * rows and
+// draws with Philox offset a.offset + k * offset_step under key rng_key(seed, that offset) (common.cuh prob_offset /
+// prob_seed).  Its rows do exactly what they do in a single launch.
+struct LatentBatch {
+  long long tiles;          // tiles of one problem
+  long long latent0, belief0, act, eps, rows;
+  unsigned long long seed;  // unkeyed
+  unsigned long long offset_step;
+};
+
 // Rows per CTA and shared memory, chosen from the row count and the device (launcher and b200pets_latent_plan_info).
 struct LatentPlan {
   int rows;          // rows per CTA: 1, 2, 4, 8, 16 or 32
@@ -130,6 +142,9 @@ void latent_pack_bias(float* dst, int N, const float* b0, const float* b1, int o
 int latent_tile(size_t row_bytes, long long rows, LatentPlan* p);
 int latent_plan(const LatentDev& m, long long rows, LatentPlan* p);
 int launch_latent_rollout(const LatentDev& m, const LatentArgs& a, cudaStream_t stream);
+// `num_problems` copies of the evaluation `a` describes (totals only, latent0 / belief0 set) in one grid whose tile comes
+// from latent_plan over all num_problems * a.B rows; bt.tiles is set here
+int launch_latent_rollout_batch(const LatentDev& m, const LatentArgs& a, int num_problems, LatentBatch bt, cudaStream_t stream);
 
 // ---- Training's sequence kernels (latent_train.cu): the RSSM of PlaNetModel.forward (planet.py:354-404) ------------
 // The forward kernel reads packed transposed copies like the rollout's (LatentDev's embedding, GRU and prior fields; the

@@ -10,6 +10,10 @@ a parameter's storage or ``_version`` counter changed, so a training round in be
 interface over ``b200pets_latent_step`` / ``b200pets_latent_eval_sequences``; ``CEMOptimizer`` plans over it with one
 ``b200pets_latent_cem_plan`` call.  Every rollout starts at the model's posterior (``_current_posterior_sample``,
 ``_current_belief``), which ``update_posterior`` (the conv encoder, run by the caller once per environment step) sets.
+
+For K environments at once the env itself holds K posteriors: ``update_posterior_batch`` (or ``set_posterior_batch``)
+sets them, ``evaluate_action_sequences_batch`` and ``cem_plan_batch`` (``b200pets_latent_eval_sequences_batch`` /
+``b200pets_latent_cem_plan_batch``) plan from them, and ``TrajectoryOptimizerAgent.act_batch`` plans with them.
 """
 from __future__ import annotations
 
@@ -146,6 +150,96 @@ class StagedLatentModel:
             pass
 
 
+class PosteriorBatch:
+    """The K posteriors a :class:`LatentModelEnv` plans K observations from, kept apart from the model's own posterior:
+    ``latent [K, L]`` and ``belief [K, Hb]`` on ``device``, plus the entries whose next :meth:`update` starts a new
+    episode.  Reads the model only in :meth:`update`."""
+
+    def __init__(self, model, latent_size: int, belief_size: int, action_size: int, device):
+        self.model, self.L, self.Hb, self.A = model, latent_size, belief_size, action_size
+        self.device = torch.device(device)
+        self.latent: Optional[torch.Tensor] = None
+        self.belief: Optional[torch.Tensor] = None
+        self.fresh: Optional[np.ndarray] = None
+
+    def set(self, latent, belief):
+        latent = torch.as_tensor(latent).detach().to(self.device, torch.float32).contiguous()
+        belief = torch.as_tensor(belief).detach().to(self.device, torch.float32).contiguous()
+        K = latent.shape[0] if latent.ndim == 2 else 0
+        if K < 1 or latent.shape != (K, self.L) or belief.shape != (K, self.Hb):
+            raise ValueError(f"set_posterior_batch: latent {tuple(latent.shape)} and belief {tuple(belief.shape)} must be "
+                             f"[K, {self.L}] and [K, {self.Hb}]")
+        self.latent, self.belief = latent, belief
+        self.fresh = np.zeros(K, dtype=bool)
+
+    def update(self, obs, action=None, rng: Optional[torch.Generator] = None, *,
+               _eps: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
+        """``PlaNetModel.update_posterior`` (planet.py:592-641) for K observations ``obs [K, C, H, W]`` and the actions
+        ``action [K, A]`` that led to them, with the model's own ``encoder``, ``belief_model`` and
+        ``posterior_transition_model`` and the reference's ``x / 256 - 0.5``.  Entries of a new batch and entries listed
+        to :meth:`reset` start from zero latent, belief and action (``action`` may be None only when every entry does).
+        The posterior draw is one N(0, 1) ``[K, L]`` from ``rng`` (else the model's ``rng``); ``_eps`` replaces it.
+        Returns ``{"latent": [K, L], "belief": [K, Hb]}``."""
+        model = self.model
+        missing = [n for n in ("encoder", "belief_model", "posterior_transition_model") if not hasattr(model, n)]
+        if missing:
+            raise NotImplementedError(f"update_posterior_batch runs the model's encoder, belief_model and "
+                                      f"posterior_transition_model; this model has no {', '.join(missing)}")
+        with torch.no_grad():
+            x = torch.as_tensor(obs).float().to(self.device) / 256.0 - 0.5  # planet.py:274-275
+            if x.ndim != 4:
+                raise ValueError(f"update_posterior_batch: obs must be [K, C, H, W], got {tuple(x.shape)}")
+            K = x.shape[0]
+            if self.latent is None:
+                fresh = np.ones(K, dtype=bool)
+            elif self.latent.shape[0] != K:
+                raise ValueError(f"update_posterior_batch: {K} observations for a batch of {self.latent.shape[0]} "
+                                 "posteriors (reset_posterior_batch() starts a new batch)")
+            else:
+                fresh = self.fresh
+            latent = torch.zeros(K, self.L, device=self.device)
+            belief = torch.zeros(K, self.Hb, device=self.device)
+            act = torch.zeros(K, self.A, device=self.device)
+            if not fresh.all():
+                if action is None:
+                    raise ValueError("update_posterior_batch: action is None but some entries continue an episode")
+                keep = torch.from_numpy(~fresh).to(self.device)[:, None]
+                act = torch.where(keep, torch.as_tensor(action).float().to(self.device).reshape(K, self.A), act)
+                latent = torch.where(keep, self.latent, latent)
+                belief = torch.where(keep, self.belief, belief)
+            bm = model.belief_model  # BeliefModel.forward (planet.py:90-101)
+            next_belief = bm.rnn(bm.embedding_layer(torch.cat([latent, act], dim=1)), belief)
+            params = model.posterior_transition_model(torch.cat([next_belief, model.encoder(x)], dim=1))
+            mean, std = params[:, :self.L], params[:, self.L:]
+            if _eps is None:
+                _eps = torch.randn(mean.size(), dtype=mean.dtype, layout=mean.layout, device=mean.device,
+                                   generator=model.rng if rng is None else rng)
+            self.set(mean + std * _eps.to(mean.device, mean.dtype), next_belief)
+            return {"latent": self.latent, "belief": self.belief}
+
+    def reset(self, indices=None):
+        """``indices`` None drops the batch (the next update sets K from its observations); otherwise the listed entries
+        start their next :meth:`update` from zero latent, belief and action, as ``reset_posterior()`` followed by
+        ``update_posterior(obs, action=None)`` does."""
+        if indices is None or self.latent is None:
+            self.latent = self.belief = self.fresh = None
+            return
+        self.fresh[np.asarray(list(indices), dtype=np.int64)] = True
+
+    def get(self, K: Optional[int] = None):
+        """``(latent [K, L], belief [K, Hb])``: ``NotImplementedError`` when none is set, ``ValueError`` when ``K``
+        differs, ``RuntimeError`` when an entry was reset and not updated since."""
+        if self.latent is None:
+            raise NotImplementedError("the latent model holds one posterior; to plan for K observations set K posteriors "
+                                      "first with update_posterior_batch(obs) or set_posterior_batch")
+        if K is not None and K != self.latent.shape[0]:
+            raise ValueError(f"{K} problems for a batch of {self.latent.shape[0]} posteriors")
+        if self.fresh.any():
+            raise RuntimeError(f"entries {np.flatnonzero(self.fresh).tolist()} were reset: call "
+                               "update_posterior_batch(obs) before planning")
+        return self.latent, self.belief
+
+
 class LatentModelEnv(ModelEnv):
     """``ModelEnv`` over PlaNet's latent model (model_env.py:15-191 with ``PlaNetModel.sample``).  The states are
     ``{"latent": [B, L], "belief": [B, Hb]}``; rewards come from the reward model and nothing terminates."""
@@ -177,6 +271,8 @@ class LatentModelEnv(ModelEnv):
         self._offset = 0
         self._ws: Optional[torch.Tensor] = None
         self._auto_refresh = True
+        d = self.staged.desc
+        self.posteriors = PosteriorBatch(model, d.latent_size, d.belief_size, d.action_size, self.device)
 
     def has_external_callables(self) -> bool:
         return False
@@ -229,16 +325,20 @@ class LatentModelEnv(ModelEnv):
 
     def evaluate_action_sequences(self, action_sequences: torch.Tensor, initial_state: np.ndarray, num_particles: int, *,
                                   _eps: Optional[torch.Tensor] = None, _row_returns: Optional[torch.Tensor] = None,
-                                  _offset: Optional[int] = None) -> torch.Tensor:
+                                  _offset: Optional[int] = None, _entry: Optional[int] = None) -> torch.Tensor:
         """model_env.py:145-191 as one launch from the posterior: ``initial_state`` (a 1-D or a 3-D pixel observation)
         is only checked for its rank, since PlaNetModel.reset reads nothing but the batch size.  ``_eps [H, B, L]``
-        replaces the in-kernel draws."""
+        replaces the in-kernel draws; ``_entry`` k starts from the batch's posterior k instead of the model's."""
         with torch.no_grad():
             assert len(action_sequences.shape) == 3  # model_env.py:166
             population_size, horizon, action_dim = action_sequences.shape
             assert np.ndim(initial_state) in (1, 3)  # model_env.py:169
             self._fresh()
-            latent0, belief0 = self.staged.posterior()
+            if _entry is None:
+                latent0, belief0 = self.staged.posterior()
+            else:
+                latent, belief = self._posterior_batch()
+                latent0, belief0 = latent[_entry], belief[_entry]
             actions = action_sequences.to(self.device, torch.float32).contiguous()
             cfg = self._rollout_cfg(population_size, horizon, num_particles,
                                     self._call_offset() if _offset is None else _offset)
@@ -253,9 +353,51 @@ class LatentModelEnv(ModelEnv):
                     "latent_eval_sequences")
             return returns
 
-    def evaluate_action_sequences_batch(self, *args, **kwargs):
-        raise NotImplementedError("the latent model holds one posterior, so it evaluates one observation's sequences at a "
-                                  "time: call evaluate_action_sequences")
+    # ---- K posteriors (PosteriorBatch) ------------------------------------------------------------------------------
+    def set_posterior_batch(self, latent, belief):
+        """Set the K posteriors batched planning starts from: ``latent [K, L]``, ``belief [K, Hb]``."""
+        self.posteriors.set(latent, belief)
+
+    def update_posterior_batch(self, obs, action=None, rng: Optional[torch.Generator] = None, *,
+                               _eps: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
+        """:meth:`PosteriorBatch.update`: ``PlaNetModel.update_posterior`` for K observations ``obs [K, C, H, W]``."""
+        return self.posteriors.update(obs, action, rng, _eps=_eps)
+
+    def reset_posterior_batch(self, indices=None):
+        """:meth:`PosteriorBatch.reset`: drop the batch (None) or restart the listed entries."""
+        self.posteriors.reset(indices)
+
+    def _posterior_batch(self, K: Optional[int] = None):
+        return self.posteriors.get(K)
+
+    def evaluate_action_sequences_batch(self, action_sequences: torch.Tensor, initial_states: np.ndarray, num_particles: int,
+                                        *, _eps: Optional[torch.Tensor] = None, _row_returns: Optional[torch.Tensor] = None,
+                                        _offset: Optional[int] = None) -> torch.Tensor:
+        """:meth:`evaluate_action_sequences` for the K posteriors in one launch: ``action_sequences [K, N, H, A]``, returns
+        ``[K, N]``.  Only the leading K of ``initial_states`` is checked.  Problem k gets what a single call from
+        posterior k would give at the offset of the k-th of K consecutive calls; ``_eps [K, H, B, L]``,
+        ``_row_returns [K, B]``."""
+        with torch.no_grad():
+            assert len(action_sequences.shape) == 4  # problems, population, horizon, action_dim
+            K, population_size, horizon, _ = action_sequences.shape
+            latent0, belief0 = self._posterior_batch(K)
+            if np.shape(initial_states)[0] != K:
+                raise ValueError(f"{np.shape(initial_states)[0]} initial states for {K} problems")
+            self._fresh()
+            actions = action_sequences.to(self.device, torch.float32).contiguous()
+            if _offset is None:
+                _offset = self._call_offset()
+                self._offset += K - 1  # problem k uses the offset of the k-th of K consecutive calls
+            cfg = self._rollout_cfg(population_size, horizon, num_particles, _offset)
+            eps = None if _eps is None else _eps.to(self.device, torch.float32).contiguous()
+            returns = torch.empty(K, population_size, dtype=torch.float32, device=self.device)
+            ws = self._workspace(self.lib.b200pets_latent_eval_batch_workspace_bytes(self.staged.handle, C.byref(cfg), K))
+            with torch.cuda.device(self.device):
+                _lib.check(self.lib.b200pets_latent_eval_sequences_batch(
+                    self.staged.handle, C.byref(cfg), K, _lib.ptr(latent0), _lib.ptr(belief0), _lib.ptr(actions),
+                    _lib.ptr(eps), _lib.ptr(returns), _lib.ptr(_row_returns), _lib.ptr(ws), ws.numel(), _lib.stream_ptr()),
+                    "latent_eval_sequences_batch")
+            return returns
 
     def shuffle_member_assignment(self, *args, **kwargs):
         raise NotImplementedError("the latent model has no ensemble members")
@@ -285,3 +427,33 @@ class LatentModelEnv(ModelEnv):
                 _lib.ptr(optimizer.lower_bound), _lib.ptr(optimizer.upper_bound), _lib.ptr(z), _lib.ptr(eps), _lib.ptr(sol),
                 _lib.ptr(optimizer.last_values), _lib.ptr(ws), ws.numel(), _lib.stream_ptr()), "latent_cem_plan")
         return sol.view(H, A)
+
+    def cem_plan_batch(self, optimizer, x0: torch.Tensor, num_particles: int, noise: Optional[torch.Tensor] = None,
+                       eps: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """:meth:`cem_plan` for the K posteriors from the warm starts ``x0 [K, H, A]`` as one
+        ``b200pets_latent_cem_plan_batch`` call; problem k plans with counter value first + k, the one its own single
+        plan would take k calls later.  ``noise [K, it, N, H, A]`` / ``eps [K, it, H, B, L]``; with ``record_values``
+        ``last_values`` is ``[K, it, N]``."""
+        K, H, A = x0.shape
+        latent0, belief0 = self._posterior_batch(K)
+        self._fresh()
+        rcfg = self._rollout_cfg(optimizer.population_size, H, num_particles, self._next_offset())
+        self._offset += K - 1
+        ccfg = _lib.CemCfg(optimizer.num_iterations, optimizer.elite_num, float(optimizer.alpha),
+                           int(optimizer.return_mean_elites), int(optimizer._clipped_normal))
+        ws = self._workspace(self.lib.b200pets_latent_cem_plan_batch_workspace_bytes(self.staged.handle, C.byref(rcfg),
+                                                                                      C.byref(ccfg), K))
+        x0 = x0.to(self.device, torch.float32).contiguous()
+        sol = torch.empty(K, H * A, dtype=torch.float32, device=self.device)
+        z = None if noise is None else noise.to(self.device, torch.float32).contiguous()
+        if eps is not None:
+            eps = eps.to(self.device, torch.float32).contiguous()
+        optimizer.last_values = None
+        if optimizer.record_values:
+            optimizer.last_values = torch.empty(K, optimizer.num_iterations, optimizer.population_size, device=self.device)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.b200pets_latent_cem_plan_batch(
+                self.staged.handle, C.byref(rcfg), C.byref(ccfg), K, _lib.ptr(latent0), _lib.ptr(belief0), _lib.ptr(x0),
+                _lib.ptr(optimizer.lower_bound), _lib.ptr(optimizer.upper_bound), _lib.ptr(z), _lib.ptr(eps), _lib.ptr(sol),
+                _lib.ptr(optimizer.last_values), _lib.ptr(ws), ws.numel(), _lib.stream_ptr()), "latent_cem_plan_batch")
+        return sol.view(K, H, A)

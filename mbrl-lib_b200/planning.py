@@ -11,7 +11,9 @@
   With a reward or termination callable the kernels do not know it runs the per-iteration loop instead, the
   objective applying the callable to windows of the rollout (``ModelEnv.evaluate_action_sequences``).
 * Over PlaNet's latent model (:class:`mbrl_lib_b200.latent.LatentModelEnv`) the fused plan is one
-  ``b200pets_latent_cem_plan`` call; iCEM and MPPI evaluate through its ``evaluate_action_sequences``.
+  ``b200pets_latent_cem_plan`` call; iCEM and MPPI evaluate through its ``evaluate_action_sequences``.  For K
+  observations the environment's K posteriors plan as one ``b200pets_latent_cem_plan_batch`` call, and MPPI plans
+  entry k from posterior k.
 * ``TrajectoryOptimizer`` / ``TrajectoryOptimizerAgent`` / ``create_trajectory_optim_agent_for_model``:
   reference semantics (warm-start shift, action cache, RuntimeError when the eval fn is unset).
 """
@@ -81,8 +83,11 @@ class _FusedBatchObjective:
     def __init__(self, model_env, obs: np.ndarray, num_particles: int):
         self.model_env, self.obs, self.num_particles = model_env, obs, num_particles
 
-    def entries(self) -> List[_FusedObjective]:
-        return [_FusedObjective(self.model_env, o, self.num_particles) for o in self.obs]
+    def entries(self) -> List[Callable[[torch.Tensor], torch.Tensor]]:
+        env, P = self.model_env, self.num_particles
+        if getattr(env, "is_latent", False):  # entry k evaluates from the environment's posterior k
+            return [lambda seqs, k=k, o=o: env.evaluate_action_sequences(seqs, o, P, _entry=k) for k, o in enumerate(self.obs)]
+        return [_FusedObjective(env, o, P) for o in self.obs]
 
 
 def _next_seed_offset(obj) -> int:
@@ -185,6 +190,8 @@ class CEMOptimizer(Optimizer):
 
     def _optimize_fused_batch(self, obj: _FusedBatchObjective, x0, noise, model_noise) -> torch.Tensor:
         env = obj.model_env
+        if getattr(env, "is_latent", False):  # the K posteriors: b200pets_latent_cem_plan_batch, model noise = eps only
+            return env.cem_plan_batch(self, x0, obj.num_particles, noise, None if model_noise is None else model_noise[1])
         env._fresh()
         K, H, A = x0.shape
         obs = np.asarray(obj.obs)
@@ -436,7 +443,8 @@ class MPPIOptimizer(Optimizer):
             self.batch_mean = torch.zeros((K, H, A), device=self.device, dtype=torch.float32)
         self.last_values = None
         if isinstance(obj_funs, _FusedBatchObjective):
-            if callback is None and not obj_funs.model_env.has_external_callables():
+            env = obj_funs.model_env
+            if callback is None and not env.has_external_callables() and not getattr(env, "is_latent", False):
                 return self._optimize_fused_batch(obj_funs, _noise, _model_noise)
             obj_funs = obj_funs.entries()
         saved = self.mean
@@ -656,11 +664,10 @@ class TrajectoryOptimizerAgent(Agent):
         :meth:`reset_batch` restores them."""
         if self.trajectory_eval_fn is None:
             raise RuntimeError("Please call `set_trajectory_eval_fn()` before using TrajectoryOptimizerAgent")
-        if getattr(self._fused_env, "is_latent", False):
-            raise NotImplementedError("act_batch plans for K observations, but a latent model holds one posterior: call "
-                                      "act once per observation after update_posterior")
         obs = np.asarray(obs)
         K = obs.shape[0]
+        if getattr(self._fused_env, "is_latent", False):  # plans from the environment's K posteriors (update_posterior_batch)
+            self._fused_env._posterior_batch(K)
         if self._batch_actions and self._batch_actions[0].shape[0] != K:
             self._batch_actions = []
         plan_time = 0.0
