@@ -21,18 +21,13 @@ int launch_rollout_f32_batch(const ModelDev& m, const RolloutArgs& a, int num_pr
 int launch_rollout_tc_batch(const ModelDev& m, const RolloutArgs& a, int num_problems, BatchArgs bt, cudaStream_t stream);
 int launch_particle_mean(int N, int P, const float* total, float* returns, cudaStream_t stream);
 bool cem_refit_sample_supported(int population, int dims, int elite_num);
-int launch_cem_refit_sample_batch(int num_problems, int population, int dims, int elite_num, float alpha, int use_std,
-                                  const float* row_totals, long long rows_stride, int particles, float* values, long long values_stride,
-                                  float* mu, float* dispersion, float* best_solution, long long dims_stride, float* best_value,
-                                  long long best_stride, void* workspace, long long ws_stride_bytes, size_t workspace_bytes, int refit,
-                                  int sample, const float* lb, const float* ub, const float* z_next, long long z_stride,
-                                  unsigned long long seed, unsigned long long offset, unsigned long long offset_step, int clipped,
-                                  unsigned int tag, float* pop, long long pop_stride, void* stream);
-int launch_cem_refit_sample(int population, int dims, int elite_num, float alpha, int use_std, const float* row_totals,
-                            int particles, float* values, float* mu, float* dispersion, float* best_value, float* best_solution,
-                            void* workspace, size_t workspace_bytes, int refit, int sample, const float* lb, const float* ub,
-                            const float* z_next, unsigned long long seed, unsigned long long offset, int clipped, int seq0,
-                            unsigned int* flag, unsigned int tag, float* pop, void* stream);
+int launch_cem_refit_sample(int num_problems, int population, int dims, int elite_num, float alpha, int use_std,
+                            const float* row_totals, long long rows_stride, int particles, float* values, long long values_stride,
+                            float* mu, float* dispersion, float* best_solution, long long dims_stride, float* best_value,
+                            long long best_stride, void* workspace, long long ws_stride_bytes, size_t workspace_bytes, int refit,
+                            int sample, const float* lb, const float* ub, const float* z_next, long long z_stride,
+                            unsigned long long seed, unsigned long long offset, unsigned long long offset_step, int clipped,
+                            int seq0, unsigned int tag, float* pop, long long pop_stride, void* stream);
 int launch_cem_update_rows(int population, int dims, int elite_num, float alpha, int unbiased, int use_std,
                            const float* population_in, const float* row_totals, int particles, float* values, float* mu,
                            float* dispersion, float* best_value, float* best_solution, void* workspace,
@@ -335,24 +330,15 @@ static int shard_of(const b200pets_rollout_cfg* cfg, int* seq0, int* n_glob) {
   return B200PETS_OK;
 }
 
-static int dispatch(const b200pets_model_s* mdl, int precision, const RolloutArgs& a_in, cudaStream_t stream) {
-  RolloutArgs a = a_in;
+// the rollout kernel of `precision` over `a`; bt (or NULL): a batched launch of `num_problems` copies of `a`
+static int dispatch(const b200pets_model_s* mdl, int precision, const RolloutArgs& a, cudaStream_t stream, int num_problems = 1,
+                    const BatchArgs* bt = nullptr) {
   if (precision == B200PETS_PREC_BF16_TC) {
     if (!mdl->tc_ok) return b200pets_set_error(B200PETS_EUNSUPPORTED, "tensor-core path does not cover this model; use B200PETS_PREC_F32");
-    return launch_rollout_tc(mdl->dev, a, stream);
+    return bt ? launch_rollout_tc_batch(mdl->dev, a, num_problems, *bt, stream) : launch_rollout_tc(mdl->dev, a, stream);
   }
-  if (precision == B200PETS_PREC_F32) return launch_rollout_f32(mdl->dev, a, stream);
-  return b200pets_set_error(B200PETS_EINVAL, "unknown precision %d", precision);
-}
-
-// a batched launch (BatchArgs) of `num_problems` copies of `a_in`
-static int dispatch_batch(const b200pets_model_s* mdl, int precision, const RolloutArgs& a, int num_problems, const BatchArgs& bt,
-                          cudaStream_t stream) {
-  if (precision == B200PETS_PREC_BF16_TC) {
-    if (!mdl->tc_ok) return b200pets_set_error(B200PETS_EUNSUPPORTED, "tensor-core path does not cover this model; use B200PETS_PREC_F32");
-    return launch_rollout_tc_batch(mdl->dev, a, num_problems, bt, stream);
-  }
-  if (precision == B200PETS_PREC_F32) return launch_rollout_f32_batch(mdl->dev, a, num_problems, bt, stream);
+  if (precision == B200PETS_PREC_F32)
+    return bt ? launch_rollout_f32_batch(mdl->dev, a, num_problems, *bt, stream) : launch_rollout_f32(mdl->dev, a, stream);
   return b200pets_set_error(B200PETS_EINVAL, "unknown precision %d", precision);
 }
 
@@ -414,7 +400,7 @@ static int rollout_steps(b200pets_model_t model, const b200pets_rollout_cfg* cfg
       s.traj_obs = traj_obs ? traj_obs + (size_t)(t - t0) * B * d.obs_dim : nullptr;
       s.traj_reward = traj_reward ? traj_reward + (size_t)(t - t0) * B : nullptr;
       s.traj_done = traj_done ? traj_done + (size_t)(t - t0) * B : nullptr;
-      int rc = bt ? dispatch_batch(model, precision, s, num_problems, *bt, stream) : dispatch(model, precision, s, stream);
+      int rc = dispatch(model, precision, s, stream, num_problems, bt);
       if (rc) return rc;
     }
   } else {
@@ -430,7 +416,7 @@ static int rollout_steps(b200pets_model_t model, const b200pets_rollout_cfg* cfg
     } else {             // in-kernel member draw: per (tile, step) for TS1, per tile for TSinf
       a.slot_mode = ts1 ? 1 : 2; a.perm = nullptr;
     }
-    int rc = bt ? dispatch_batch(model, precision, a, num_problems, *bt, stream) : dispatch(model, precision, a, stream);
+    int rc = dispatch(model, precision, a, stream, num_problems, bt);
     if (rc) return rc;
   }
   return B200PETS_OK;
@@ -571,100 +557,6 @@ int b200pets_step(b200pets_model_t model, int32_t precision, int32_t propagation
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// fused CEM plan
-// ---------------------------------------------------------------------------------------------------------
-namespace {
-__global__ void cem_init_kernel(int dims, const float* __restrict__ x0, const float* __restrict__ lb,
-                                const float* __restrict__ ub, int clipped, float* mu, float* disp, float* best_value) {
-  const int d = blockIdx.x * blockDim.x + threadIdx.x;
-  if (d == 0) {
-    *best_value = -INFINITY;
-    *reinterpret_cast<unsigned int*>(best_value + 2) = 0u;  // "refit done" tag of cem_refit_sample_kernel
-  }
-  if (d >= dims) return;
-  mu[d] = x0[d];
-  const float w = ub[d] - lb[d];
-  disp[d] = clipped ? 1.0f : (w * w) / 16.0f;  // trajectory_opt.py:100-108
-}
-}  // namespace
-
-size_t b200pets_cem_plan_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg) {
-  if (!model || !rcfg || !ccfg) return 0;
-  const size_t N = rcfg->population, dims = (size_t)rcfg->horizon * model->desc.act_dim;
-  return al256(N * dims * 4) + al256(N * 4) + 3 * al256(dims * 4) + 256 +
-         al256(b200pets_cem_update_workspace_bytes((int)N, (int)dims, ccfg->elite_num)) +
-         al256(b200pets_eval_workspace_bytes(model, rcfg));
-}
-
-int b200pets_cem_plan(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg,
-                      const float* obs0, const float* x0, const float* lower, const float* upper, const float* z,
-                      const float* eps, const int64_t* perms, float* solution, float* values_out, void* workspace,
-                      size_t workspace_bytes, void* stream_) {
-  if (!model || !rcfg || !ccfg || !obs0 || !x0 || !lower || !upper || !solution || !workspace)
-    return b200pets_set_error(B200PETS_EINVAL, "cem_plan: null argument");
-  cudaStream_t stream = (cudaStream_t)stream_;
-  const int N = rcfg->population, H = rcfg->horizon, P = rcfg->particles, A = model->desc.act_dim;
-  const int dims = H * A;
-  const long long B = (long long)N * P;
-  if (workspace_bytes < b200pets_cem_plan_workspace_bytes(model, rcfg, ccfg)) return b200pets_set_error(B200PETS_EINVAL, "cem_plan: workspace too small");
-  unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
-  float* pop = reinterpret_cast<float*>(ws); ws += al256((size_t)N * dims * 4);
-  float* values = reinterpret_cast<float*>(ws); ws += al256((size_t)N * 4);
-  float* mu = reinterpret_cast<float*>(ws); ws += al256((size_t)dims * 4);
-  float* disp = reinterpret_cast<float*>(ws); ws += al256((size_t)dims * 4);
-  float* best_sol = reinterpret_cast<float*>(ws); ws += al256((size_t)dims * 4);
-  float* best_val = reinterpret_cast<float*>(ws); ws += 256;
-  void* upd_ws = ws; const size_t upd_bytes = al256(b200pets_cem_update_workspace_bytes(N, dims, ccfg->elite_num)); ws += upd_bytes;
-  void* eval_ws = ws; const size_t eval_bytes = al256(b200pets_eval_workspace_bytes(model, rcfg));
-
-  cem_init_kernel<<<(dims + 255) / 256, 256, 0, stream>>>(dims, x0, lower, upper, ccfg->clipped_normal, mu, disp, best_val);
-  CUDA_TRY(cudaGetLastError());
-  // Per iteration: the rollout, then ONE kernel that refits (particle mean + top-k + mean / variance) and draws the next
-  // iteration's population (cem.cu cem_refit_sample_kernel); the first population comes from the same kernel in
-  // sample-only mode.  A population outside that kernel's single-CTA refit runs sample -> rollout -> refit instead.
-  const bool merged = cem_refit_sample_supported(N, dims, ccfg->elite_num);
-  unsigned int* refit_flag = reinterpret_cast<unsigned int*>(best_val + 2);
-  auto next_pop = [&](int it_next, int refit, const float* totals) -> int {  // refit of it_next - 1 (if any) + population of it_next
-    const int sample = it_next < ccfg->num_iterations;
-    const unsigned long long off = rcfg->offset * 1024 + (unsigned long long)it_next;
-    return launch_cem_refit_sample(N, dims, ccfg->elite_num, ccfg->alpha, ccfg->clipped_normal, totals, P, values, mu, disp,
-                                   best_val, best_sol, upd_ws, upd_bytes, refit, sample, lower, upper,
-                                   (z && sample) ? z + (size_t)it_next * N * dims : nullptr, rng_key(rcfg->seed, off), off,
-                                   ccfg->clipped_normal, rcfg->first_sequence, refit_flag, (unsigned int)it_next, pop, stream);
-  };
-  if (merged) {
-    int rc0 = next_pop(0, 0, nullptr);
-    if (rc0) return rc0;
-  }
-  for (int it = 0; it < ccfg->num_iterations; ++it) {
-    if (!merged) {
-      int rcs = b200pets_cem_sample_shard(N, rcfg->first_sequence, dims, mu, disp, lower, upper,
-                                          z ? z + (size_t)it * N * dims : nullptr, rcfg->seed, rcfg->offset * 1024 + it,
-                                          ccfg->clipped_normal, pop, stream);
-      if (rcs) return rcs;
-    }
-    b200pets_rollout_cfg rc_it = *rcfg;
-    rc_it.offset = rcfg->offset * 1024 + it;
-    const int nperm = rcfg->propagation == B200PETS_PROP_FIXED_MODEL ? 1 : H;
-    float* totals = nullptr;
-    int rc = eval_rows(model, &rc_it, obs0, pop, perms ? perms + (size_t)it * nperm * B : nullptr,
-                       eps ? eps + (size_t)it * H * B * model->desc.out_size : nullptr, nullptr, eval_ws, eval_bytes, stream,
-                       &totals);
-    if (rc) return rc;
-    if (merged)
-      rc = next_pop(it + 1, 1, totals);
-    else  // particle mean + NaN rule + top-k + refit in one kernel
-      rc = launch_cem_update_rows(N, dims, ccfg->elite_num, ccfg->alpha, 1, ccfg->clipped_normal, pop, totals, P, values, mu,
-                                  disp, best_val, best_sol, upd_ws, upd_bytes, stream);
-    if (rc) return rc;
-    // NB: values_out then holds the values AFTER the reference's in-place NaN rule (trajectory_opt.py:178)
-    if (values_out) CUDA_TRY(cudaMemcpyAsync(values_out + (size_t)it * N, values, sizeof(float) * N, cudaMemcpyDeviceToDevice, stream));
-  }
-  CUDA_TRY(cudaMemcpyAsync(solution, ccfg->return_mean_elites ? mu : best_sol, sizeof(float) * dims, cudaMemcpyDeviceToDevice, stream));
-  return B200PETS_OK;
-}
-
-// ---------------------------------------------------------------------------------------------------------
 // batches of independent problems: one launch per rollout / refit for all of them
 // ---------------------------------------------------------------------------------------------------------
 
@@ -738,13 +630,16 @@ int b200pets_eval_sequences_batch(b200pets_model_t model, const b200pets_rollout
 
 }  // extern "C"
 
+// ---------------------------------------------------------------------------------------------------------
+// fused CEM plan: K independent problems (K = 1: the single plan), one launch per rollout / refit for all of them
+// ---------------------------------------------------------------------------------------------------------
 namespace {
-__global__ void cem_init_batch_kernel(int K, int dims, const float* __restrict__ x0, const float* __restrict__ lb,
+__global__ void cem_init_kernel(int K, int dims, const float* __restrict__ x0, const float* __restrict__ lb,
                                       const float* __restrict__ ub, int clipped, float* mu, float* disp, float* best_value) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= (long long)K * dims) return;
   const int k = (int)(idx / dims), d = (int)(idx % dims);
-  if (d == 0) {  // per problem: best value, the refit flag of cem_refit_sample_batch_kernel
+  if (d == 0) {  // per problem: best value, the refit flag of the refit-and-sample kernel
     best_value[(size_t)k * 64] = -INFINITY;
     *reinterpret_cast<unsigned int*>(best_value + (size_t)k * 64 + 2) = 0u;
   }
@@ -753,12 +648,12 @@ __global__ void cem_init_batch_kernel(int K, int dims, const float* __restrict__
   disp[idx] = clipped ? 1.0f : (w * w) / 16.0f;  // trajectory_opt.py:100-108
 }
 
-// the workspace of a batched plan: per-problem arrays side by side, [K][...] each
+// the workspace of a plan: per-problem arrays side by side, [K][...] each
 struct PlanBatchLayout {
   size_t pop, values, mu, disp, best_sol, best_val, upd, eval, total;
   size_t upd_bytes;  // one problem's refit workspace
 };
-// N sequences of `dims` values per problem; eval_bytes: the batched evaluation's workspace
+// N sequences of `dims` values per problem; eval_bytes: the evaluation's workspace (all K problems)
 PlanBatchLayout plan_batch_layout(size_t N, size_t dims, int elite_num, size_t eval_bytes, int K) {
   PlanBatchLayout l{};
   l.upd_bytes = al256(b200pets_cem_update_workspace_bytes((int)N, (int)dims, elite_num));
@@ -779,13 +674,15 @@ PlanBatchLayout plan_batch_layout(b200pets_model_t model, const b200pets_rollout
                            b200pets_eval_batch_workspace_bytes(model, rcfg, K), K);
 }
 
-// The K plans of a batched CEM plan in the workspace `ws` laid out as `l`, around `rollout(it, pop, totals)`: the
-// batched rollout of iteration it, which leaves problem k's per-row totals at totals + k * N * P.  The default plan of
-// b200pets_cem_plan for every problem: rollout, then one kernel that refits and draws the next population (2 launches per
-// iteration for the whole batch).  Outside the single-CTA refit, the sample and refit kernels run once per problem around
-// the batched rollout.  Problem k draws its populations with counter rcfg->offset + k, as its single plan would.
+// The K plans of a CEM plan in the workspace `ws` laid out as `l`, around `rollout(it, pop, totals)`: the rollout of
+// iteration it (all K problems), which leaves problem k's per-row totals at totals + k * N * P.  Per iteration: the
+// rollout, then one kernel that refits (particle mean + top-k + mean / variance) and draws the next iteration's
+// population (cem.cu launch_cem_refit_sample; 2 launches per iteration for the whole batch); the first population comes
+// from the same kernel in sample-only mode.  Outside that kernel's single-CTA refit, the sample and refit kernels run once
+// per problem around the rollout instead.  Problem k draws its populations with counter rcfg->offset + k, as its single
+// plan would; rcfg->first_sequence (non-zero only for a single plan over a shard) is the first sequence drawn.
 template <class Rollout>
-int cem_plan_batch_run(const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg, int K, int dims, const PlanBatchLayout& l,
+int cem_plan_run(const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg, int K, int dims, const PlanBatchLayout& l,
                        unsigned char* ws, float* totals, const float* x0, const float* lower, const float* upper, const float* z,
                        float* solution, float* values_out, cudaStream_t stream, Rollout rollout) {
   const int N = rcfg->population, P = rcfg->particles, iters = ccfg->num_iterations;
@@ -800,18 +697,17 @@ int cem_plan_batch_run(const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg*
   const long long popk = (long long)N * dims;  // per-problem strides
 
   const long long tot = (long long)K * dims;
-  cem_init_batch_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, stream>>>(K, dims, x0, lower, upper, ccfg->clipped_normal, mu, disp,
-                                                                          best_val);
+  cem_init_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, stream>>>(K, dims, x0, lower, upper, ccfg->clipped_normal, mu, disp,
+                                                                    best_val);
   CUDA_TRY(cudaGetLastError());
   const bool merged = cem_refit_sample_supported(N, dims, ccfg->elite_num);
   auto next_pop = [&](int it_next, int refit) -> int {  // refit of it_next - 1 (if any) + population of it_next
     const int sample = it_next < iters;
-    return launch_cem_refit_sample_batch(K, N, dims, ccfg->elite_num, ccfg->alpha, ccfg->clipped_normal, refit ? totals : nullptr, B, P,
-                                         values, N, mu, disp, best_sol, dims, best_val, 64, upd_ws, (long long)l.upd_bytes,
-                                         l.upd_bytes, refit, sample, lower, upper,
-                                         (z && sample) ? z + (size_t)it_next * N * dims : nullptr, (long long)iters * N * dims,
-                                         rcfg->seed, rcfg->offset * 1024 + (unsigned long long)it_next, 1024, ccfg->clipped_normal,
-                                         (unsigned int)it_next, pop, popk, stream);
+    return launch_cem_refit_sample(K, N, dims, ccfg->elite_num, ccfg->alpha, ccfg->clipped_normal, refit ? totals : nullptr, B, P,
+                                   values, N, mu, disp, best_sol, dims, best_val, 64, upd_ws, (long long)l.upd_bytes, l.upd_bytes,
+                                   refit, sample, lower, upper, (z && sample) ? z + (size_t)it_next * N * dims : nullptr,
+                                   (long long)iters * N * dims, rcfg->seed, rcfg->offset * 1024 + (unsigned long long)it_next, 1024,
+                                   ccfg->clipped_normal, rcfg->first_sequence, (unsigned int)it_next, pop, popk, stream);
   };
   if (merged) {
     int rc0 = next_pop(0, 0);
@@ -820,7 +716,7 @@ int cem_plan_batch_run(const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg*
   for (int it = 0; it < iters; ++it) {
     if (!merged)
       for (int k = 0; k < K; ++k) {
-        int rcs = b200pets_cem_sample_shard(N, 0, dims, mu + (size_t)k * dims, disp + (size_t)k * dims, lower, upper,
+        int rcs = b200pets_cem_sample_shard(N, rcfg->first_sequence, dims, mu + (size_t)k * dims, disp + (size_t)k * dims, lower, upper,
                                             z ? z + ((size_t)k * iters + it) * N * dims : nullptr, rcfg->seed,
                                             (rcfg->offset + k) * 1024 + it, ccfg->clipped_normal, pop + (size_t)k * popk, stream);
         if (rcs) return rcs;
@@ -839,7 +735,8 @@ int cem_plan_batch_run(const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg*
         if (rc) return rc;
       }
     }
-    if (values_out)  // problem k's values of iteration it -> values_out[k][it]
+    // problem k's values of iteration it -> values_out[k][it], after the reference's in-place NaN rule (trajectory_opt.py:178)
+    if (values_out)
       CUDA_TRY(cudaMemcpy2DAsync(values_out + (size_t)it * N, sizeof(float) * iters * N, values, sizeof(float) * N, sizeof(float) * N,
                                  K, cudaMemcpyDeviceToDevice, stream));
   }
@@ -850,6 +747,40 @@ int cem_plan_batch_run(const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg*
 }  // namespace
 
 extern "C" {
+
+size_t b200pets_cem_plan_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg) {
+  if (!model || !rcfg || !ccfg) return 0;
+  return plan_batch_layout(rcfg->population, (size_t)rcfg->horizon * model->desc.act_dim, ccfg->elite_num,
+                           b200pets_eval_workspace_bytes(model, rcfg), 1).total;
+}
+
+int b200pets_cem_plan(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg,
+                      const float* obs0, const float* x0, const float* lower, const float* upper, const float* z,
+                      const float* eps, const int64_t* perms, float* solution, float* values_out, void* workspace,
+                      size_t workspace_bytes, void* stream_) {
+  if (!model || !rcfg || !ccfg || !obs0 || !x0 || !lower || !upper || !solution || !workspace)
+    return b200pets_set_error(B200PETS_EINVAL, "cem_plan: null argument");
+  if (workspace_bytes < b200pets_cem_plan_workspace_bytes(model, rcfg, ccfg)) return b200pets_set_error(B200PETS_EINVAL, "cem_plan: workspace too small");
+  cudaStream_t stream = (cudaStream_t)stream_;
+  const b200pets_model_desc& d = model->desc;
+  const int N = rcfg->population, H = rcfg->horizon, P = rcfg->particles, dims = H * d.act_dim;
+  const long long B = (long long)N * P;
+  const size_t eval_bytes = b200pets_eval_workspace_bytes(model, rcfg);
+  const PlanBatchLayout l = plan_batch_layout(N, dims, ccfg->elite_num, eval_bytes, 1);
+  unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
+  void* eval_ws = ws + l.eval;
+  float* totals = reinterpret_cast<float*>(ws + l.eval + al256((size_t)B * d.obs_dim * sizeof(float)));  // eval_rows' slot
+  const int nperm = rcfg->propagation == B200PETS_PROP_FIXED_MODEL ? 1 : H;
+  return cem_plan_run(rcfg, ccfg, 1, dims, l, ws, totals, x0, lower, upper, z, solution, values_out, stream,
+                      [&](int it, const float* pop, float* tot) {
+                        b200pets_rollout_cfg rc_it = *rcfg;
+                        rc_it.offset = rcfg->offset * 1024 + it;
+                        float* rows = nullptr;
+                        return eval_rows(model, &rc_it, obs0, pop, perms ? perms + (size_t)it * nperm * B : nullptr,
+                                         eps ? eps + (size_t)it * H * B * d.out_size : nullptr, tot, eval_ws, eval_bytes, stream,
+                                         &rows);
+                      });
+}
 
 size_t b200pets_cem_plan_batch_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg,
                                                int32_t num_problems) {
@@ -877,15 +808,15 @@ int b200pets_cem_plan_batch(b200pets_model_t model, const b200pets_rollout_cfg* 
   void* eval_ws = ws + l.eval;
   float* totals = reinterpret_cast<float*>(ws + l.eval + al256((size_t)K * B * d.obs_dim * sizeof(float)));
   const int nperm = rcfg->propagation == B200PETS_PROP_FIXED_MODEL ? 1 : H;
-  return cem_plan_batch_run(rcfg, ccfg, K, dims, l, ws, totals, x0, lower, upper, z, solution, values_out, stream,
-                            [&](int it, const float* pop, float* tot) {
-                              b200pets_rollout_cfg rc_it = *rcfg;
-                              rc_it.offset = rcfg->offset * 1024 + it;
-                              return eval_rows_batch(model, &rc_it, K, obs0, pop, (long long)N * dims,
-                                                     perms ? perms + (size_t)it * nperm * B : nullptr, (long long)iters * nperm * B,
-                                                     eps ? eps + (size_t)it * H * B * d.out_size : nullptr,
-                                                     (long long)iters * H * B * d.out_size, tot, eval_ws, stream, 1024);
-                            });
+  return cem_plan_run(rcfg, ccfg, K, dims, l, ws, totals, x0, lower, upper, z, solution, values_out, stream,
+                      [&](int it, const float* pop, float* tot) {
+                        b200pets_rollout_cfg rc_it = *rcfg;
+                        rc_it.offset = rcfg->offset * 1024 + it;
+                        return eval_rows_batch(model, &rc_it, K, obs0, pop, (long long)N * dims,
+                                               perms ? perms + (size_t)it * nperm * B : nullptr, (long long)iters * nperm * B,
+                                               eps ? eps + (size_t)it * H * B * d.out_size : nullptr,
+                                               (long long)iters * H * B * d.out_size, tot, eval_ws, stream, 1024);
+                      });
 }
 
 namespace {
@@ -1407,13 +1338,11 @@ int b200pets_latent_eval_sequences(b200pets_latent_model_t model, const b200pets
 size_t b200pets_latent_cem_plan_workspace_bytes(b200pets_latent_model_t model, const b200pets_rollout_cfg* rcfg,
                                                 const b200pets_cem_cfg* ccfg) {
   if (!model || !rcfg || !ccfg) return 0;
-  const size_t N = rcfg->population, dims = (size_t)rcfg->horizon * model->desc.action_size;
-  return al256(N * dims * 4) + al256(N * 4) + 3 * al256(dims * 4) + 256 +
-         al256(b200pets_cem_update_workspace_bytes((int)N, (int)dims, ccfg->elite_num)) +
-         b200pets_latent_eval_workspace_bytes(model, rcfg);
+  return plan_batch_layout(rcfg->population, (size_t)rcfg->horizon * model->desc.action_size, ccfg->elite_num,
+                           b200pets_latent_eval_workspace_bytes(model, rcfg), 1).total;
 }
 
-// b200pets_cem_plan with the latent rollout: the same launches, offsets and buffers around a different model
+// b200pets_cem_plan with the latent rollout: the same plan around a different model
 int b200pets_latent_cem_plan(b200pets_latent_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg,
                              const float* latent0, const float* belief0, const float* x0, const float* lower,
                              const float* upper, const float* z, const float* eps, float* solution, float* values_out,
@@ -1427,57 +1356,19 @@ int b200pets_latent_cem_plan(b200pets_latent_model_t model, const b200pets_rollo
   if (workspace_bytes < b200pets_latent_cem_plan_workspace_bytes(model, rcfg, ccfg))
     return b200pets_set_error(B200PETS_EINVAL, "latent_cem_plan: workspace too small");
   cudaStream_t stream = (cudaStream_t)stream_;
-  const int N = rcfg->population, H = rcfg->horizon, P = rcfg->particles, L = model->desc.latent_size;
+  const int H = rcfg->horizon, L = model->desc.latent_size;
   const int dims = H * model->desc.action_size;
-  const long long B = (long long)N * P;
+  const long long B = (long long)rcfg->population * rcfg->particles;
+  const PlanBatchLayout l = plan_batch_layout(rcfg->population, dims, ccfg->elite_num,
+                                              b200pets_latent_eval_workspace_bytes(model, rcfg), 1);
   unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
-  float* pop = reinterpret_cast<float*>(ws); ws += al256((size_t)N * dims * 4);
-  float* values = reinterpret_cast<float*>(ws); ws += al256((size_t)N * 4);
-  float* mu = reinterpret_cast<float*>(ws); ws += al256((size_t)dims * 4);
-  float* disp = reinterpret_cast<float*>(ws); ws += al256((size_t)dims * 4);
-  float* best_sol = reinterpret_cast<float*>(ws); ws += al256((size_t)dims * 4);
-  float* best_val = reinterpret_cast<float*>(ws); ws += 256;
-  void* upd_ws = ws; const size_t upd_bytes = al256(b200pets_cem_update_workspace_bytes(N, dims, ccfg->elite_num)); ws += upd_bytes;
-  float* totals = reinterpret_cast<float*>(ws);
-
-  cem_init_kernel<<<(dims + 255) / 256, 256, 0, stream>>>(dims, x0, lower, upper, ccfg->clipped_normal, mu, disp, best_val);
-  CUDA_TRY(cudaGetLastError());
-  const bool merged = cem_refit_sample_supported(N, dims, ccfg->elite_num);
-  unsigned int* refit_flag = reinterpret_cast<unsigned int*>(best_val + 2);
-  auto next_pop = [&](int it_next, int refit, const float* rows) -> int {  // refit of it_next - 1 (if any) + population of it_next
-    const int sample = it_next < ccfg->num_iterations;
-    const unsigned long long off = rcfg->offset * 1024 + (unsigned long long)it_next;
-    return launch_cem_refit_sample(N, dims, ccfg->elite_num, ccfg->alpha, ccfg->clipped_normal, rows, P, values, mu, disp,
-                                   best_val, best_sol, upd_ws, upd_bytes, refit, sample, lower, upper,
-                                   (z && sample) ? z + (size_t)it_next * N * dims : nullptr, rng_key(rcfg->seed, off), off,
-                                   ccfg->clipped_normal, 0, refit_flag, (unsigned int)it_next, pop, stream);
-  };
-  if (merged) {
-    int rc0 = next_pop(0, 0, nullptr);
-    if (rc0) return rc0;
-  }
-  for (int it = 0; it < ccfg->num_iterations; ++it) {
-    const unsigned long long off = rcfg->offset * 1024 + it;
-    if (!merged) {
-      int rcs = b200pets_cem_sample_shard(N, 0, dims, mu, disp, lower, upper, z ? z + (size_t)it * N * dims : nullptr,
-                                          rcfg->seed, off, ccfg->clipped_normal, pop, stream);
-      if (rcs) return rcs;
-    }
-    LatentArgs a;
-    latent_rollout_args(rcfg, off, latent0, belief0, pop, eps ? eps + (size_t)it * H * B * L : nullptr, totals, &a);
-    int rc = launch_latent_rollout(model->dev, a, stream);
-    if (rc) return rc;
-    if (merged)
-      rc = next_pop(it + 1, 1, totals);
-    else  // particle mean + NaN rule + top-k + refit in one kernel
-      rc = launch_cem_update_rows(N, dims, ccfg->elite_num, ccfg->alpha, 1, ccfg->clipped_normal, pop, totals, P, values, mu,
-                                  disp, best_val, best_sol, upd_ws, upd_bytes, stream);
-    if (rc) return rc;
-    // values_out holds the values after the reference's in-place NaN rule (trajectory_opt.py:178), as b200pets_cem_plan's
-    if (values_out) CUDA_TRY(cudaMemcpyAsync(values_out + (size_t)it * N, values, sizeof(float) * N, cudaMemcpyDeviceToDevice, stream));
-  }
-  CUDA_TRY(cudaMemcpyAsync(solution, ccfg->return_mean_elites ? mu : best_sol, sizeof(float) * dims, cudaMemcpyDeviceToDevice, stream));
-  return B200PETS_OK;
+  return cem_plan_run(rcfg, ccfg, 1, dims, l, ws, reinterpret_cast<float*>(ws + l.eval), x0, lower, upper, z, solution,
+                      values_out, stream, [&](int it, const float* pop, float* totals) {
+                        LatentArgs a;
+                        latent_rollout_args(rcfg, rcfg->offset * 1024 + it, latent0, belief0, pop,
+                                            eps ? eps + (size_t)it * H * B * L : nullptr, totals, &a);
+                        return launch_latent_rollout(model->dev, a, stream);
+                      });
 }
 
 // Batches of K posteriors: one batched rollout launch per evaluation, the plan of b200pets_cem_plan_batch around it
@@ -1558,13 +1449,13 @@ int b200pets_latent_cem_plan_batch(b200pets_latent_model_t model, const b200pets
                                               b200pets_latent_eval_batch_workspace_bytes(model, rcfg, K), K);
   unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
   const LatentBatch bt = latent_batch_strides(model->desc, rcfg, (long long)iters * H * B * L, 1024);
-  return cem_plan_batch_run(rcfg, ccfg, K, dims, l, ws, reinterpret_cast<float*>(ws + l.eval), x0, lower, upper, z, solution,
-                            values_out, (cudaStream_t)stream_, [&](int it, const float* pop, float* totals) {
-                              LatentArgs a;
-                              latent_rollout_args(rcfg, rcfg->offset * 1024 + it, latent0, belief0, pop,
-                                                  eps ? eps + (size_t)it * H * B * L : nullptr, totals, &a);
-                              return launch_latent_rollout_batch(model->dev, a, K, bt, (cudaStream_t)stream_);
-                            });
+  return cem_plan_run(rcfg, ccfg, K, dims, l, ws, reinterpret_cast<float*>(ws + l.eval), x0, lower, upper, z, solution,
+                      values_out, (cudaStream_t)stream_, [&](int it, const float* pop, float* totals) {
+                        LatentArgs a;
+                        latent_rollout_args(rcfg, rcfg->offset * 1024 + it, latent0, belief0, pop,
+                                            eps ? eps + (size_t)it * H * B * L : nullptr, totals, &a);
+                        return launch_latent_rollout_batch(model->dev, a, K, bt, (cudaStream_t)stream_);
+                      });
 }
 
 // ---------------------------------------------------------------------------------------------------------

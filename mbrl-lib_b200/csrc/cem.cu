@@ -579,7 +579,7 @@ cem_refit_sample_kernel(const SelArgs s, const float* __restrict__ row_totals, i
   }
 }
 
-// cem_refit_sample_kernel for K independent problems in one launch.  Problem k works on base + k * stride of every
+// cem_refit_sample_kernel for K > 1 independent problems in one launch.  Problem k works on base + k * stride of every
 // per-problem array and draws with Philox offset q.offset + k * offset_step; its work is the single kernel's, split the
 // same way.  CTA k < K is problem k's refit CTA (and its first sampling CTA); CTA K + j is sampling CTA 1 + j % (G - 1)
 // of problem j / (G - 1).  A CTA that waits for a refit therefore waits only for a CTA of lower index, which the
@@ -1236,13 +1236,19 @@ bool cem_refit_sample_supported(int population, int dims, int elite_num) {
   return population <= kSmallN && (size_t)elite_num * dims * sizeof(float) <= 150 * 1024 && elite_num >= 2 && elite_num <= population;
 }
 
-// refit (particle mean fused, rows = per-particle totals) + next population; returns B200PETS_EUNSUPPORTED when the population
-// is outside the single-CTA refit (the caller then uses the separate kernels)
-int launch_cem_refit_sample(int population, int dims, int elite_num, float alpha, int use_std, const float* row_totals,
-                            int particles, float* values, float* mu, float* dispersion, float* best_value, float* best_solution,
-                            void* workspace, size_t workspace_bytes, int refit, int sample, const float* lb, const float* ub,
-                            const float* z_next, unsigned long long seed, unsigned long long offset, int clipped, int seq0,
-                            unsigned int* flag, unsigned int tag, float* pop, void* stream) {
+// refit (particle mean fused, rows = per-particle totals) + next population of `num_problems` problems whose per-problem
+// arrays lie `*_stride` elements apart (see RefitBatch); seed is the unkeyed seed, problem k draws with offset + k *
+// offset_step, sequences seq0 .. seq0 + population - 1.  Returns B200PETS_EUNSUPPORTED when the population is outside the
+// single-CTA refit (the caller then uses the separate kernels).  One problem runs cem_refit_sample_kernel: the batched
+// kernel gives the same bits but took 6 % longer per launch at K = 1 (27.7 against 26.1 us at PETS HalfCheetah's 500
+// sequences of 180 values with 50 elites, H100 80GB HBM3 at 700 W).
+int launch_cem_refit_sample(int num_problems, int population, int dims, int elite_num, float alpha, int use_std,
+                            const float* row_totals, long long rows_stride, int particles, float* values, long long values_stride,
+                            float* mu, float* dispersion, float* best_solution, long long dims_stride, float* best_value,
+                            long long best_stride, void* workspace, long long ws_stride_bytes, size_t workspace_bytes, int refit,
+                            int sample, const float* lb, const float* ub, const float* z_next, long long z_stride,
+                            unsigned long long seed, unsigned long long offset, unsigned long long offset_step, int clipped,
+                            int seq0, unsigned int tag, float* pop, long long pop_stride, void* stream) {
   const int n = population, k = elite_num;
   if (!(n <= kSmallN && (size_t)k * dims * sizeof(float) <= 150 * 1024)) return B200PETS_EUNSUPPORTED;
   if (refit && (k < 2 || k > n)) return b200pets_set_error(B200PETS_EINVAL, "cem_update: need 2 <= elite_num (%d) <= population (%d)", k, n);
@@ -1254,48 +1260,23 @@ int launch_cem_refit_sample(int population, int dims, int elite_num, float alpha
   s.partial = reinterpret_cast<float*>(workspace);
   s.elite_idx = reinterpret_cast<int*>(reinterpret_cast<float*>(workspace) + 33 * (size_t)dims);
   NextPop q{};
-  q.refit = refit; q.sample = sample; q.n_pop = n; q.lb = lb; q.ub = ub; q.z = z_next; q.seed = seed; q.offset = offset;
-  q.clipped = clipped; q.seq0 = seq0; q.flag = flag; q.tag = tag; q.pop_out = pop;
-  const long long tot = (long long)n * dims;
-  unsigned grid = sample ? (unsigned)min((long long)64, (tot + kSelThreads - 1) / kSelThreads) : 1u;
-  if (grid < 1) grid = 1;
-  const size_t esm = (size_t)k * dims * sizeof(float);
-  CUDA_TRY(cudaFuncSetAttribute(cem_refit_sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 150 * 1024));
-  CUDA_TRY(launch_pdl(cem_refit_sample_kernel, dim3(grid), dim3(kSelThreads), esm, (cudaStream_t)stream, s, row_totals, particles, q));
-  return B200PETS_OK;
-}
-
-// launch_cem_refit_sample for `num_problems` problems whose per-problem arrays lie `*_stride` elements apart (see
-// RefitBatch); seed is the unkeyed seed, problem k draws with offset + k * offset_step
-int launch_cem_refit_sample_batch(int num_problems, int population, int dims, int elite_num, float alpha, int use_std,
-                                  const float* row_totals, long long rows_stride, int particles, float* values, long long values_stride,
-                                  float* mu, float* dispersion, float* best_solution, long long dims_stride, float* best_value,
-                                  long long best_stride, void* workspace, long long ws_stride_bytes, size_t workspace_bytes, int refit,
-                                  int sample, const float* lb, const float* ub, const float* z_next, long long z_stride,
-                                  unsigned long long seed, unsigned long long offset, unsigned long long offset_step, int clipped,
-                                  unsigned int tag, float* pop, long long pop_stride, void* stream) {
-  const int n = population, k = elite_num;
-  if (!(n <= kSmallN && (size_t)k * dims * sizeof(float) <= 150 * 1024)) return B200PETS_EUNSUPPORTED;
-  if (refit && (k < 2 || k > n)) return b200pets_set_error(B200PETS_EINVAL, "cem_update: need 2 <= elite_num (%d) <= population (%d)", k, n);
-  if (workspace_bytes < b200pets_cem_update_workspace_bytes(n, dims, k)) return b200pets_set_error(B200PETS_EINVAL, "cem_update: workspace too small");
-  SelArgs s{};
-  s.n = n; s.dims = dims; s.k = k; s.alpha = alpha; s.unbiased = 1; s.use_std = use_std; s.mode = 0;
-  s.pop = pop; s.pstride = dims; s.values = values; s.vstride = 1; s.mu = mu; s.disp = dispersion;
-  s.best_value = best_value; s.best_solution = best_solution;
-  s.partial = reinterpret_cast<float*>(workspace);
-  s.elite_idx = reinterpret_cast<int*>(reinterpret_cast<float*>(workspace) + 33 * (size_t)dims);
-  NextPop q{};
-  q.refit = refit; q.sample = sample; q.n_pop = n; q.lb = lb; q.ub = ub; q.z = z_next; q.offset = offset;
-  q.clipped = clipped; q.seq0 = 0; q.flag = reinterpret_cast<unsigned int*>(best_value + 2); q.tag = tag; q.pop_out = pop;
+  q.refit = refit; q.sample = sample; q.n_pop = n; q.lb = lb; q.ub = ub; q.z = z_next; q.seed = rng_key(seed, offset);
+  q.offset = offset; q.clipped = clipped; q.seq0 = seq0; q.flag = reinterpret_cast<unsigned int*>(best_value + 2); q.tag = tag;
+  q.pop_out = pop;
   const long long tot = (long long)n * dims;
   unsigned G = sample ? (unsigned)min((long long)64, (tot + kSelThreads - 1) / kSelThreads) : 1u;
   if (G < 1) G = 1;
+  const size_t esm = (size_t)k * dims * sizeof(float);
+  if (num_problems == 1) {
+    CUDA_TRY(cudaFuncSetAttribute(cem_refit_sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 150 * 1024));
+    CUDA_TRY(launch_pdl(cem_refit_sample_kernel, dim3(G), dim3(kSelThreads), esm, (cudaStream_t)stream, s, row_totals, particles, q));
+    return B200PETS_OK;
+  }
   RefitBatch rb{};
   rb.K = num_problems; rb.G = (int)G;
   rb.pop = pop_stride; rb.values = values_stride; rb.dims = dims_stride; rb.best = best_stride;
   rb.ws = ws_stride_bytes / (long long)sizeof(int); rb.rows = rows_stride; rb.z = z_stride;
   rb.seed = seed; rb.offset_step = offset_step;
-  const size_t esm = (size_t)k * dims * sizeof(float);
   CUDA_TRY(cudaFuncSetAttribute(cem_refit_sample_batch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 150 * 1024));
   CUDA_TRY(launch_pdl(cem_refit_sample_batch_kernel, dim3((unsigned)num_problems * G), dim3(kSelThreads), esm, (cudaStream_t)stream, s,
                       row_totals, particles, q, rb));

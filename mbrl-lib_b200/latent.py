@@ -410,8 +410,7 @@ class LatentModelEnv(ModelEnv):
         H, A = x0.shape
         latent0, belief0 = self.staged.posterior()
         rcfg = self._rollout_cfg(optimizer.population_size, H, num_particles, self._next_offset())
-        ccfg = _lib.CemCfg(optimizer.num_iterations, optimizer.elite_num, float(optimizer.alpha),
-                           int(optimizer.return_mean_elites), int(optimizer._clipped_normal))
+        ccfg = optimizer._cem_cfg()
         need = self.lib.b200pets_latent_cem_plan_workspace_bytes(self.staged.handle, C.byref(rcfg), C.byref(ccfg))
         ws = self._workspace(need)
         sol = torch.empty(H * A, dtype=torch.float32, device=self.device)
@@ -439,8 +438,7 @@ class LatentModelEnv(ModelEnv):
         self._fresh()
         rcfg = self._rollout_cfg(optimizer.population_size, H, num_particles, self._next_offset())
         self._offset += K - 1
-        ccfg = _lib.CemCfg(optimizer.num_iterations, optimizer.elite_num, float(optimizer.alpha),
-                           int(optimizer.return_mean_elites), int(optimizer._clipped_normal))
+        ccfg = optimizer._cem_cfg()
         ws = self._workspace(self.lib.b200pets_latent_cem_plan_batch_workspace_bytes(self.staged.handle, C.byref(rcfg),
                                                                                       C.byref(ccfg), K))
         x0 = x0.to(self.device, torch.float32).contiguous()

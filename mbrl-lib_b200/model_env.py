@@ -288,17 +288,8 @@ class ModelEnv:
             actions = action_sequences.to(self.device, torch.float32).contiguous()
             prop = self._propagation()
             perms = _perms
-            B = population_size * num_particles
             if perms is None:
-                if prop == "fixed_model":
-                    M = len(self.staged.members())
-                    if B % M != 0:
-                        raise ValueError("To use GaussianMLP's ensemble propagation, the batch size must "
-                                         "be a multiple of the number of models in the ensemble.")
-                    if self.ts1 == "perms" or self._few_groups(population_size, num_particles):
-                        perms = torch.randperm(B, device=self.device).view(1, B)
-                elif prop == "random_model" and (self.ts1 == "perms" or self._few_groups(population_size, num_particles)):
-                    perms = torch.stack([torch.randperm(B, device=self.device) for _ in range(horizon)])
+                perms = self._eval_perms(prop, population_size, horizon, num_particles)
             cfg = _lib.RolloutCfg(population_size, horizon, num_particles, _lib.PREC[self.precision_for(prop)], _lib.PROP[prop],
                                   _lib.TS1_PERMS if perms is not None else _lib.TS1_TILE_SHUFFLE, self._seed,
                                   self._call_offset() if _offset is None else _offset, int(_shard[0]), int(_shard[1]))

@@ -188,6 +188,21 @@ class CEMOptimizer(Optimizer):
             raise ValueError(f"{len(obj_funs)} objectives for {x0.shape[0]} warm starts")
         return torch.stack([self.optimize(f, x0=x0[k], callback=callback) for k, f in enumerate(obj_funs)])
 
+    def _cem_cfg(self) -> _lib.CemCfg:
+        """This optimizer's settings as the fused plans' ``b200pets_cem_cfg``."""
+        return _lib.CemCfg(self.num_iterations, self.elite_num, float(self.alpha), int(self.return_mean_elites),
+                           int(self._clipped_normal))
+
+    def _plan_perms(self, env, prop: str, horizon: int, num_particles: int) -> Optional[torch.Tensor]:
+        """The permutations one fused plan draws, ``[iterations, horizon or 1, N * P]`` (None: members drawn in kernel)."""
+        if prop not in ("random_model", "fixed_model") or not (
+                env.ts1 == "perms" or env._few_groups(self.population_size, num_particles)):
+            return None
+        B = self.population_size * num_particles
+        n = horizon if prop == "random_model" else 1
+        return torch.stack([torch.stack([torch.randperm(B, device=self.device) for _ in range(n)])
+                            for _ in range(self.num_iterations)])
+
     def _optimize_fused_batch(self, obj: _FusedBatchObjective, x0, noise, model_noise) -> torch.Tensor:
         env = obj.model_env
         if getattr(env, "is_latent", False):  # the K posteriors: b200pets_latent_cem_plan_batch, model noise = eps only
@@ -201,19 +216,15 @@ class CEMOptimizer(Optimizer):
         perms = eps = None
         if model_noise is not None:
             perms, eps = model_noise
-        if perms is None and prop in ("random_model", "fixed_model") and (
-                env.ts1 == "perms" or env._few_groups(self.population_size, obj.num_particles)):
-            B = self.population_size * obj.num_particles
-            n = H if prop == "random_model" else 1
-            perms = torch.stack([torch.stack([torch.stack([torch.randperm(B, device=self.device) for _ in range(n)])
-                                              for _ in range(self.num_iterations)]) for _ in range(K)])
+        if perms is None:
+            per = [self._plan_perms(env, prop, H, obj.num_particles) for _ in range(K)]
+            perms = None if not per or per[0] is None else torch.stack(per)
         # problem k plans with counter value first + k: the one its own single plan would take k calls later
         rcfg = _lib.RolloutCfg(self.population_size, H, obj.num_particles, _lib.PREC[env.precision_for(prop)], _lib.PROP[prop],
                                _lib.TS1_PERMS if perms is not None else _lib.TS1_TILE_SHUFFLE, env._seed,
                                env._next_offset())
         env._offset += K - 1
-        ccfg = _lib.CemCfg(self.num_iterations, self.elite_num, float(self.alpha), int(self.return_mean_elites),
-                           int(self._clipped_normal))
+        ccfg = self._cem_cfg()
         need = self.lib.b200pets_cem_plan_batch_workspace_bytes(env.staged.handle, C.byref(rcfg), C.byref(ccfg), K)
         if self._plan_batch_ws is None or self._plan_batch_ws.numel() < need:
             self._plan_batch_ws = torch.empty(max(need, 1), dtype=torch.uint8, device=self.device)
@@ -243,17 +254,12 @@ class CEMOptimizer(Optimizer):
         perms = eps = None
         if model_noise is not None:
             perms, eps = model_noise
-        if perms is None and prop in ("random_model", "fixed_model") and (
-                env.ts1 == "perms" or env._few_groups(self.population_size, obj.num_particles)):
-            B = self.population_size * obj.num_particles
-            n = H if prop == "random_model" else 1
-            perms = torch.stack([torch.stack([torch.randperm(B, device=self.device) for _ in range(n)])
-                                 for _ in range(self.num_iterations)])
+        if perms is None:
+            perms = self._plan_perms(env, prop, H, obj.num_particles)
         rcfg = _lib.RolloutCfg(self.population_size, H, obj.num_particles, _lib.PREC[env.precision_for(prop)], _lib.PROP[prop],
                                _lib.TS1_PERMS if perms is not None else _lib.TS1_TILE_SHUFFLE, env._seed,
                                env._next_offset())
-        ccfg = _lib.CemCfg(self.num_iterations, self.elite_num, float(self.alpha), int(self.return_mean_elites),
-                           int(self._clipped_normal))
+        ccfg = self._cem_cfg()
         need = self.lib.b200pets_cem_plan_workspace_bytes(env.staged.handle, C.byref(rcfg), C.byref(ccfg))
         if self._plan_ws is None or self._plan_ws.numel() < need:
             self._plan_ws = torch.empty(need, dtype=torch.uint8, device=self.device)
