@@ -327,7 +327,9 @@ int b200pets_shift_solution(int32_t horizon, int32_t act_dim, int32_t replan_fre
  * sample -> rollout -> refit instead (three launches per iteration).  z / eps / perms as above with a leading
  * [num_iterations] dimension, or NULL.
  *   x0 [dev] float[H*A]; lower/upper [dev] float[H*A]
- *   solution [dev] float[H*A]; values_out [dev] float[num_iterations][N] or NULL */
+ *   solution [dev] float[H*A]; values_out [dev] float[num_iterations][N] or NULL
+ * Refused before the first launch: a NULL required pointer, the configuration b200pets_eval_sequences refuses,
+ * num_iterations < 0, elite_num outside [1, population], a workspace too small. */
 typedef struct {
   int32_t num_iterations;
   int32_t elite_num;
@@ -356,8 +358,10 @@ int b200pets_cem_plan(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, 
  *   perms [dev] int64[K][it][H or 1][B] (each or NULL); solution [dev] float[K][H*A];
  *   values_out [dev] float[K][it][N] or NULL.
  * The plan runs the default structure of b200pets_cem_plan (rollout, then refit + next population: two launches per
- * iteration for the whole batch).  Refused: num_problems < 1, a sharded cfg (first_sequence != 0 or global_population
- * other than 0 / population), external reward / termination callables. */
+ * iteration for the whole batch).  A single call is the batch of one: at num_problems = 1 these launch what
+ * b200pets_eval_sequences / b200pets_cem_plan launch, and each single workspace query is its batched query at 1.
+ * Refused before the first launch: num_problems < 1, a sharded cfg (first_sequence != 0 or global_population other than
+ * 0 / population), external reward / termination callables, and what the single call refuses. */
 size_t b200pets_eval_batch_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* cfg, int32_t num_problems);
 int b200pets_eval_sequences_batch(b200pets_model_t model, const b200pets_rollout_cfg* cfg, int32_t num_problems,
                                   const float* obs0, const float* actions, const int64_t* perms, const float* eps,
@@ -476,8 +480,11 @@ int b200pets_latent_cem_plan(b200pets_latent_model_t model, const b200pets_rollo
  * per evaluation for all K, tiles problem-major, rows per CTA chosen from K * N * P rows (b200pets_latent_plan_info of
  * that count).  Problem k gives, bit for bit, what the single call gives for its inputs at Philox offset
  * offset + k * 1024 (evaluation) or with counter offset + k, i.e. (offset + k) * 1024 + iteration (plan): a batch
- * takes the counter values of K consecutive single calls.  Refused before anything touches the device:
- * num_problems < 1, a sharded cfg, a precision other than f32, a NULL required pointer, a workspace too small.
+ * takes the counter values of K consecutive single calls.  A single call is the batch of one: at num_problems = 1
+ * these launch what the single calls launch, and each single workspace query is its batched query at 1.  Every latent
+ * evaluation and plan refuses before anything touches the device: num_problems < 1 (batches), a sharded cfg, a
+ * precision other than f32, a NULL required pointer, a workspace too small, and for the plans num_iterations < 0 or
+ * elite_num outside [1, population].
  *   latent0 [dev] float[K][L], belief0 [dev] float[K][Hb]: posterior k
  *   evaluation: actions [dev] float[K][N][H][A]; eps [dev] float[K][H][B][L] or NULL; returns [dev] float[K][N];
  *     row_returns [dev] float[K][B] or NULL

@@ -14,11 +14,9 @@
 #include "train.cuh"
 
 // launchers defined in the kernel translation units
-int launch_rollout_f32(const ModelDev& m, const RolloutArgs& a, cudaStream_t stream);
-int launch_rollout_tc(const ModelDev& m, const RolloutArgs& a, cudaStream_t stream);
+int launch_rollout_f32(const ModelDev& m, const RolloutArgs& a, int num_problems, BatchArgs bt, cudaStream_t stream);
+int launch_rollout_tc(const ModelDev& m, const RolloutArgs& a, int num_problems, BatchArgs bt, cudaStream_t stream);
 int launch_wgmma_selftest(int k, int n, const float* a, const float* b, float* d, cudaStream_t stream);
-int launch_rollout_f32_batch(const ModelDev& m, const RolloutArgs& a, int num_problems, BatchArgs bt, cudaStream_t stream);
-int launch_rollout_tc_batch(const ModelDev& m, const RolloutArgs& a, int num_problems, BatchArgs bt, cudaStream_t stream);
 int launch_particle_mean(int N, int P, const float* total, float* returns, cudaStream_t stream);
 bool cem_refit_sample_supported(int population, int dims, int elite_num);
 int launch_cem_refit_sample(int num_problems, int population, int dims, int elite_num, float alpha, int use_std,
@@ -330,27 +328,32 @@ static int shard_of(const b200pets_rollout_cfg* cfg, int* seq0, int* n_glob) {
   return B200PETS_OK;
 }
 
-// the rollout kernel of `precision` over `a`; bt (or NULL): a batched launch of `num_problems` copies of `a`
-static int dispatch(const b200pets_model_s* mdl, int precision, const RolloutArgs& a, cudaStream_t stream, int num_problems = 1,
-                    const BatchArgs* bt = nullptr) {
+// the rollout kernel of `precision` over `num_problems` copies of `a` (bt: per-problem strides, read when there are more
+// than one)
+static int dispatch(const b200pets_model_s* mdl, int precision, const RolloutArgs& a, int num_problems, const BatchArgs& bt,
+                    cudaStream_t stream) {
   if (precision == B200PETS_PREC_BF16_TC) {
     if (!mdl->tc_ok) return b200pets_set_error(B200PETS_EUNSUPPORTED, "tensor-core path does not cover this model; use B200PETS_PREC_F32");
-    return bt ? launch_rollout_tc_batch(mdl->dev, a, num_problems, *bt, stream) : launch_rollout_tc(mdl->dev, a, stream);
+    return launch_rollout_tc(mdl->dev, a, num_problems, bt, stream);
   }
-  if (precision == B200PETS_PREC_F32)
-    return bt ? launch_rollout_f32_batch(mdl->dev, a, num_problems, *bt, stream) : launch_rollout_f32(mdl->dev, a, stream);
+  if (precision == B200PETS_PREC_F32) return launch_rollout_f32(mdl->dev, a, num_problems, bt, stream);
   return b200pets_set_error(B200PETS_EINVAL, "unknown precision %d", precision);
 }
 
 static size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 
-size_t b200pets_eval_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* cfg) {
-  if (!model || !cfg) return 0;
-  const size_t B = (size_t)cfg->population * cfg->particles;
-  return al256(B * model->desc.obs_dim * sizeof(float)) + al256(B * sizeof(float)) + al256(B);
+// evaluation workspace: observations [K][B][D], reward totals [K][B], dead flags [K][B]
+size_t b200pets_eval_batch_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* cfg, int32_t num_problems) {
+  if (!model || !cfg || num_problems < 1) return 0;
+  const size_t KB = (size_t)num_problems * cfg->population * cfg->particles;
+  return al256(KB * model->desc.obs_dim * sizeof(float)) + al256(KB * sizeof(float)) + al256(KB);
 }
 
-// checks shared by every evaluation entry point
+size_t b200pets_eval_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* cfg) {
+  return b200pets_eval_batch_workspace_bytes(model, cfg, 1);
+}
+
+// checks shared by every evaluation and plan entry point
 static int check_eval(b200pets_model_t model, const b200pets_rollout_cfg* cfg, const char* what) {
   const b200pets_model_desc& d = model->desc;
   const int N = cfg->population, H = cfg->horizon, P = cfg->particles;
@@ -362,15 +365,24 @@ static int check_eval(b200pets_model_t model, const b200pets_rollout_cfg* cfg, c
   return B200PETS_OK;
 }
 
+// the single evaluation and plan: external callables run through b200pets_eval_trajectory instead
+static int check_no_external(b200pets_model_t model) {
+  const b200pets_model_desc& d = model->desc;
+  if (d.reward_fn == B200PETS_REWARD_EXTERNAL || d.term_fn == B200PETS_TERM_EXTERNAL)
+    return b200pets_set_error(B200PETS_EUNSUPPORTED, "eval_sequences: external reward/termination callables cannot run inside "
+                                                     "this call; use b200pets_eval_trajectory, the callable, then b200pets_trajectory_returns");
+  return B200PETS_OK;
+}
+
 // Rollout launches for steps [t0, t1) of the evaluation `cfg` describes.  Between launches a row's observation is carried
 // in obs_state [B][D] (stored when keep_obs, or when the window is split into per-step launches); its reward total and
 // dead flag in total / dead when those are given (NULL: the kernel's own accumulation is not kept).  traj_* (or NULL)
-// receive every step's next observation, reward and done at [t - t0][row].  bt (or NULL): the launches are batched over
-// num_problems problems with these per-problem strides; every pointer is then problem 0's.
+// receive every step's next observation, reward and done at [t - t0][row].  The launches cover num_problems problems with
+// bt's per-problem strides (read when there are more than one); every pointer is problem 0's.
 static int rollout_steps(b200pets_model_t model, const b200pets_rollout_cfg* cfg, int t0, int t1, bool keep_obs,
                          const float* obs0, const float* actions, const int64_t* perms, const float* eps, float* obs_state,
                          float* total, uint8_t* dead, float* traj_obs, float* traj_reward, uint8_t* traj_done,
-                         cudaStream_t stream, int num_problems = 1, const BatchArgs* bt = nullptr) {
+                         cudaStream_t stream, int num_problems = 1, const BatchArgs& bt = BatchArgs{}) {
   const b200pets_model_desc& d = model->desc;
   const int N = cfg->population, H = cfg->horizon, P = cfg->particles;
   const long long B = (long long)N * P;
@@ -400,7 +412,7 @@ static int rollout_steps(b200pets_model_t model, const b200pets_rollout_cfg* cfg
       s.traj_obs = traj_obs ? traj_obs + (size_t)(t - t0) * B * d.obs_dim : nullptr;
       s.traj_reward = traj_reward ? traj_reward + (size_t)(t - t0) * B : nullptr;
       s.traj_done = traj_done ? traj_done + (size_t)(t - t0) * B : nullptr;
-      int rc = dispatch(model, precision, s, stream, num_problems, bt);
+      int rc = dispatch(model, precision, s, num_problems, bt, stream);
       if (rc) return rc;
     }
   } else {
@@ -416,34 +428,54 @@ static int rollout_steps(b200pets_model_t model, const b200pets_rollout_cfg* cfg
     } else {             // in-kernel member draw: per (tile, step) for TS1, per tile for TSinf
       a.slot_mode = ts1 ? 1 : 2; a.perm = nullptr;
     }
-    int rc = dispatch(model, precision, a, stream, num_problems, bt);
+    int rc = dispatch(model, precision, a, num_problems, bt, stream);
     if (rc) return rc;
   }
   return B200PETS_OK;
 }
 
-// the rollout of one evaluation: per-row totals [B] (row r = n * P + p) in *totals_out, no particle mean
-static int eval_rows(b200pets_model_t model, const b200pets_rollout_cfg* cfg, const float* obs0, const float* actions,
-                     const int64_t* perms, const float* eps, float* row_returns, void* workspace, size_t workspace_bytes,
-                     void* stream_, float** totals_out) {
-  if (!model || !cfg || !obs0 || !actions || !workspace) return b200pets_set_error(B200PETS_EINVAL, "eval_sequences: null argument");
+// The rollouts of K evaluations (K = 1: one evaluation, single-problem launches): problem k starts from obs0 + k * D,
+// reads actions + k * act_stride, perms + k * perm_stride, eps + k * eps_stride and draws with Philox offset
+// cfg->offset + k * offset_step.  Per-row totals land in `total` [K][B]; observations and dead flags are carried in the
+// evaluation workspace.
+static int eval_rows(b200pets_model_t model, const b200pets_rollout_cfg* cfg, int K, const float* obs0, const float* actions,
+                     long long act_stride, const int64_t* perms, long long perm_stride, const float* eps, long long eps_stride,
+                     float* total, void* workspace, cudaStream_t stream, unsigned long long offset_step) {
   const b200pets_model_desc& d = model->desc;
-  { int rc = check_eval(model, cfg, "eval_sequences"); if (rc) return rc; }
-  if (d.reward_fn == B200PETS_REWARD_EXTERNAL || d.term_fn == B200PETS_TERM_EXTERNAL)
-    return b200pets_set_error(B200PETS_EUNSUPPORTED, "eval_sequences: external reward/termination callables cannot run inside "
-                                                     "this call; use b200pets_eval_trajectory, the callable, then b200pets_trajectory_returns");
-  if (workspace_bytes < b200pets_eval_workspace_bytes(model, cfg)) return b200pets_set_error(B200PETS_EINVAL, "eval_sequences: workspace too small");
-  const size_t B = (size_t)cfg->population * cfg->particles;
+  const size_t B = (size_t)cfg->population * cfg->particles, KB = (size_t)K * B;
   unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
   float* obs_state = reinterpret_cast<float*>(ws);
-  const size_t o1 = al256(B * d.obs_dim * sizeof(float));
-  float* total = row_returns ? row_returns : reinterpret_cast<float*>(ws + o1);
-  uint8_t* dead = ws + o1 + al256(B * sizeof(float));
-  int rc = rollout_steps(model, cfg, 0, cfg->horizon, false, obs0, actions, perms, eps, obs_state, total, dead, nullptr, nullptr,
-                         nullptr, (cudaStream_t)stream_);
+  uint8_t* dead = ws + al256(KB * d.obs_dim * sizeof(float)) + al256(KB * sizeof(float));
+  BatchArgs bt{};
+  bt.obs0 = d.obs_dim;
+  bt.obs_state = (long long)B * d.obs_dim;
+  bt.act = act_stride;
+  bt.rows = (long long)B;
+  bt.perm = perm_stride;
+  bt.eps = eps_stride;
+  bt.seed = cfg->seed;
+  bt.offset_step = offset_step;
+  return rollout_steps(model, cfg, 0, cfg->horizon, false, obs0, actions, perms, eps, obs_state, total, dead, nullptr, nullptr,
+                       nullptr, stream, K, bt);
+}
+
+// b200pets_eval_sequences(_batch) past their own checks: K evaluations and one particle mean over their K * N sequences
+static int eval_sequences(b200pets_model_t model, const b200pets_rollout_cfg* cfg, int K, const float* obs0, const float* actions,
+                          const int64_t* perms, const float* eps, float* returns, float* row_returns, void* workspace,
+                          size_t workspace_bytes, cudaStream_t stream, const char* who) {
+  if (workspace_bytes < b200pets_eval_batch_workspace_bytes(model, cfg, K))
+    return b200pets_set_error(B200PETS_EINVAL, "%s: workspace too small", who);
+  const b200pets_model_desc& d = model->desc;
+  const int N = cfg->population, H = cfg->horizon;
+  const size_t B = (size_t)N * cfg->particles, KB = (size_t)K * B;
+  const int nperm = cfg->propagation == B200PETS_PROP_FIXED_MODEL ? 1 : H;
+  float* total = row_returns ? row_returns
+                             : reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(workspace) + al256(KB * d.obs_dim * sizeof(float)));
+  int rc = eval_rows(model, cfg, K, obs0, actions, (long long)N * H * d.act_dim, perms, (long long)nperm * B, eps,
+                     (long long)H * B * d.out_size, total, workspace, stream, 1024);
   if (rc) return rc;
-  *totals_out = total;
-  return B200PETS_OK;
+  // problem k's totals are rows k * B .. k * B + B - 1: one particle mean over K * N sequences
+  return launch_particle_mean(K * N, cfg->particles, total, returns, stream);  // model_env.py:190-191
 }
 
 namespace {
@@ -518,11 +550,12 @@ int b200pets_trajectory_returns(const b200pets_rollout_cfg* cfg, int32_t t0, int
 int b200pets_eval_sequences(b200pets_model_t model, const b200pets_rollout_cfg* cfg, const float* obs0,
                             const float* actions, const int64_t* perms, const float* eps, float* returns,
                             float* row_returns, void* workspace, size_t workspace_bytes, void* stream_) {
-  if (!returns) return b200pets_set_error(B200PETS_EINVAL, "eval_sequences: null argument");
-  float* total = nullptr;
-  int rc = eval_rows(model, cfg, obs0, actions, perms, eps, row_returns, workspace, workspace_bytes, stream_, &total);
-  if (rc) return rc;
-  return launch_particle_mean(cfg->population, cfg->particles, total, returns, (cudaStream_t)stream_);  // model_env.py:190-191
+  if (!model || !cfg || !obs0 || !actions || !returns || !workspace)
+    return b200pets_set_error(B200PETS_EINVAL, "eval_sequences: null argument");
+  { int rc = check_eval(model, cfg, "eval_sequences"); if (rc) return rc; }
+  { int rc = check_no_external(model); if (rc) return rc; }
+  return eval_sequences(model, cfg, 1, obs0, actions, perms, eps, returns, row_returns, workspace, workspace_bytes,
+                        (cudaStream_t)stream_, "eval_sequences");
 }
 
 int b200pets_step(b200pets_model_t model, int32_t precision, int32_t propagation, int64_t batch, const float* obs,
@@ -553,7 +586,7 @@ int b200pets_step(b200pets_model_t model, int32_t precision, int32_t propagation
   } else {
     a.slot_mode = 1;
   }
-  return dispatch(model, precision, a, (cudaStream_t)stream_);
+  return dispatch(model, precision, a, 1, BatchArgs{}, (cudaStream_t)stream_);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -575,57 +608,14 @@ static int check_batch(b200pets_model_t model, const b200pets_rollout_cfg* cfg, 
   return B200PETS_OK;
 }
 
-// evaluation workspace of a batch: observations [K][B][D], reward totals [K][B], dead flags [K][B]
-size_t b200pets_eval_batch_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* cfg, int32_t num_problems) {
-  if (!model || !cfg || num_problems < 1) return 0;
-  const size_t KB = (size_t)num_problems * cfg->population * cfg->particles;
-  return al256(KB * model->desc.obs_dim * sizeof(float)) + al256(KB * sizeof(float)) + al256(KB);
-}
-
-// The rollouts of K evaluations in batched launches: problem k starts from obs0 + k * D, reads actions + k * act_stride,
-// perms + k * perm_stride, eps + k * eps_stride and draws with Philox offset cfg->offset + k * offset_step.  Per-row
-// totals land in `total` [K][B].
-static int eval_rows_batch(b200pets_model_t model, const b200pets_rollout_cfg* cfg, int K, const float* obs0, const float* actions,
-                           long long act_stride, const int64_t* perms, long long perm_stride, const float* eps, long long eps_stride,
-                           float* total, void* workspace, cudaStream_t stream, unsigned long long offset_step) {
-  const b200pets_model_desc& d = model->desc;
-  const size_t B = (size_t)cfg->population * cfg->particles, KB = (size_t)K * B;
-  unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
-  float* obs_state = reinterpret_cast<float*>(ws);
-  uint8_t* dead = ws + al256(KB * d.obs_dim * sizeof(float)) + al256(KB * sizeof(float));
-  BatchArgs bt{};
-  bt.obs0 = d.obs_dim;
-  bt.obs_state = (long long)B * d.obs_dim;
-  bt.act = act_stride;
-  bt.rows = (long long)B;
-  bt.perm = perm_stride;
-  bt.eps = eps_stride;
-  bt.seed = cfg->seed;
-  bt.offset_step = offset_step;
-  return rollout_steps(model, cfg, 0, cfg->horizon, false, obs0, actions, perms, eps, obs_state, total, dead, nullptr, nullptr,
-                       nullptr, stream, K, &bt);
-}
-
 int b200pets_eval_sequences_batch(b200pets_model_t model, const b200pets_rollout_cfg* cfg, int32_t num_problems,
                                   const float* obs0, const float* actions, const int64_t* perms, const float* eps,
                                   float* returns, float* row_returns, void* workspace, size_t workspace_bytes, void* stream_) {
   if (!model || !cfg) return b200pets_set_error(B200PETS_EINVAL, "eval_sequences_batch: null argument");
   { int rc = check_batch(model, cfg, num_problems, "eval_sequences_batch"); if (rc) return rc; }
   if (!obs0 || !actions || !returns || !workspace) return b200pets_set_error(B200PETS_EINVAL, "eval_sequences_batch: null argument");
-  if (workspace_bytes < b200pets_eval_batch_workspace_bytes(model, cfg, num_problems))
-    return b200pets_set_error(B200PETS_EINVAL, "eval_sequences_batch: workspace too small");
-  const b200pets_model_desc& d = model->desc;
-  const int N = cfg->population, H = cfg->horizon;
-  const size_t B = (size_t)N * cfg->particles, KB = (size_t)num_problems * B;
-  const int nperm = cfg->propagation == B200PETS_PROP_FIXED_MODEL ? 1 : H;
-  float* total = row_returns ? row_returns
-                             : reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(workspace) + al256(KB * d.obs_dim * sizeof(float)));
-  cudaStream_t stream = (cudaStream_t)stream_;
-  int rc = eval_rows_batch(model, cfg, num_problems, obs0, actions, (long long)N * H * d.act_dim, perms, (long long)nperm * B, eps,
-                           (long long)H * B * d.out_size, total, workspace, stream, 1024);
-  if (rc) return rc;
-  // problem k's totals are rows k * B .. k * B + B - 1: one particle mean over K * N sequences
-  return launch_particle_mean(num_problems * N, cfg->particles, total, returns, stream);  // model_env.py:190-191
+  return eval_sequences(model, cfg, num_problems, obs0, actions, perms, eps, returns, row_returns, workspace, workspace_bytes,
+                        (cudaStream_t)stream_, "eval_sequences_batch");
 }
 
 }  // extern "C"
@@ -672,6 +662,14 @@ PlanBatchLayout plan_batch_layout(size_t N, size_t dims, int elite_num, size_t e
 PlanBatchLayout plan_batch_layout(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg, int K) {
   return plan_batch_layout(rcfg->population, (size_t)rcfg->horizon * model->desc.act_dim, ccfg->elite_num,
                            b200pets_eval_batch_workspace_bytes(model, rcfg, K), K);
+}
+
+// the CEM settings every plan entry point checks before its first launch
+int check_cem(const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg, const char* who) {
+  if (ccfg->num_iterations < 0 || ccfg->elite_num < 1 || ccfg->elite_num > rcfg->population)
+    return b200pets_set_error(B200PETS_EINVAL, "%s: %d iterations, %d elites of %d", who, ccfg->num_iterations, ccfg->elite_num,
+                              rcfg->population);
+  return B200PETS_OK;
 }
 
 // The K plans of a CEM plan in the workspace `ws` laid out as `l`, around `rollout(it, pop, totals)`: the rollout of
@@ -744,66 +742,17 @@ int cem_plan_run(const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg,
                            stream));
   return B200PETS_OK;
 }
-}  // namespace
 
-extern "C" {
-
-size_t b200pets_cem_plan_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg) {
-  if (!model || !rcfg || !ccfg) return 0;
-  return plan_batch_layout(rcfg->population, (size_t)rcfg->horizon * model->desc.act_dim, ccfg->elite_num,
-                           b200pets_eval_workspace_bytes(model, rcfg), 1).total;
-}
-
-int b200pets_cem_plan(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg,
-                      const float* obs0, const float* x0, const float* lower, const float* upper, const float* z,
-                      const float* eps, const int64_t* perms, float* solution, float* values_out, void* workspace,
-                      size_t workspace_bytes, void* stream_) {
-  if (!model || !rcfg || !ccfg || !obs0 || !x0 || !lower || !upper || !solution || !workspace)
-    return b200pets_set_error(B200PETS_EINVAL, "cem_plan: null argument");
-  if (workspace_bytes < b200pets_cem_plan_workspace_bytes(model, rcfg, ccfg)) return b200pets_set_error(B200PETS_EINVAL, "cem_plan: workspace too small");
-  cudaStream_t stream = (cudaStream_t)stream_;
-  const b200pets_model_desc& d = model->desc;
-  const int N = rcfg->population, H = rcfg->horizon, P = rcfg->particles, dims = H * d.act_dim;
-  const long long B = (long long)N * P;
-  const size_t eval_bytes = b200pets_eval_workspace_bytes(model, rcfg);
-  const PlanBatchLayout l = plan_batch_layout(N, dims, ccfg->elite_num, eval_bytes, 1);
-  unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
-  void* eval_ws = ws + l.eval;
-  float* totals = reinterpret_cast<float*>(ws + l.eval + al256((size_t)B * d.obs_dim * sizeof(float)));  // eval_rows' slot
-  const int nperm = rcfg->propagation == B200PETS_PROP_FIXED_MODEL ? 1 : H;
-  return cem_plan_run(rcfg, ccfg, 1, dims, l, ws, totals, x0, lower, upper, z, solution, values_out, stream,
-                      [&](int it, const float* pop, float* tot) {
-                        b200pets_rollout_cfg rc_it = *rcfg;
-                        rc_it.offset = rcfg->offset * 1024 + it;
-                        float* rows = nullptr;
-                        return eval_rows(model, &rc_it, obs0, pop, perms ? perms + (size_t)it * nperm * B : nullptr,
-                                         eps ? eps + (size_t)it * H * B * d.out_size : nullptr, tot, eval_ws, eval_bytes, stream,
-                                         &rows);
-                      });
-}
-
-size_t b200pets_cem_plan_batch_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg,
-                                               int32_t num_problems) {
-  if (!model || !rcfg || !ccfg || num_problems < 1) return 0;
-  return plan_batch_layout(model, rcfg, ccfg, num_problems).total;
-}
-
-int b200pets_cem_plan_batch(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg,
-                            int32_t num_problems, const float* obs0, const float* x0, const float* lower, const float* upper,
-                            const float* z, const float* eps, const int64_t* perms, float* solution, float* values_out,
-                            void* workspace, size_t workspace_bytes, void* stream_) {
-  if (!model || !rcfg || !ccfg) return b200pets_set_error(B200PETS_EINVAL, "cem_plan_batch: null argument");
-  { int rc = check_batch(model, rcfg, num_problems, "cem_plan_batch"); if (rc) return rc; }
-  if (!obs0 || !x0 || !lower || !upper || !solution || !workspace)
-    return b200pets_set_error(B200PETS_EINVAL, "cem_plan_batch: null argument");
-  const int K = num_problems;
-  if (workspace_bytes < b200pets_cem_plan_batch_workspace_bytes(model, rcfg, ccfg, K))
-    return b200pets_set_error(B200PETS_EINVAL, "cem_plan_batch: workspace too small");
-  cudaStream_t stream = (cudaStream_t)stream_;
+// b200pets_cem_plan(_batch) past their own checks: K plans, one rollout launch per iteration for all of them
+int cem_plan(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg, int K, const float* obs0,
+             const float* x0, const float* lower, const float* upper, const float* z, const float* eps, const int64_t* perms,
+             float* solution, float* values_out, void* workspace, size_t workspace_bytes, cudaStream_t stream, const char* who) {
+  { int rc = check_cem(rcfg, ccfg, who); if (rc) return rc; }
+  const PlanBatchLayout l = plan_batch_layout(model, rcfg, ccfg, K);
+  if (workspace_bytes < l.total) return b200pets_set_error(B200PETS_EINVAL, "%s: workspace too small", who);
   const b200pets_model_desc& d = model->desc;
   const int N = rcfg->population, H = rcfg->horizon, P = rcfg->particles, dims = H * d.act_dim, iters = ccfg->num_iterations;
   const long long B = (long long)N * P;
-  const PlanBatchLayout l = plan_batch_layout(model, rcfg, ccfg, K);
   unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
   void* eval_ws = ws + l.eval;
   float* totals = reinterpret_cast<float*>(ws + l.eval + al256((size_t)K * B * d.obs_dim * sizeof(float)));
@@ -812,11 +761,48 @@ int b200pets_cem_plan_batch(b200pets_model_t model, const b200pets_rollout_cfg* 
                       [&](int it, const float* pop, float* tot) {
                         b200pets_rollout_cfg rc_it = *rcfg;
                         rc_it.offset = rcfg->offset * 1024 + it;
-                        return eval_rows_batch(model, &rc_it, K, obs0, pop, (long long)N * dims,
-                                               perms ? perms + (size_t)it * nperm * B : nullptr, (long long)iters * nperm * B,
-                                               eps ? eps + (size_t)it * H * B * d.out_size : nullptr,
-                                               (long long)iters * H * B * d.out_size, tot, eval_ws, stream, 1024);
+                        return eval_rows(model, &rc_it, K, obs0, pop, (long long)N * dims,
+                                         perms ? perms + (size_t)it * nperm * B : nullptr, (long long)iters * nperm * B,
+                                         eps ? eps + (size_t)it * H * B * d.out_size : nullptr,
+                                         (long long)iters * H * B * d.out_size, tot, eval_ws, stream, 1024);
                       });
+}
+}  // namespace
+
+extern "C" {
+
+size_t b200pets_cem_plan_batch_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg,
+                                               int32_t num_problems) {
+  if (!model || !rcfg || !ccfg || num_problems < 1) return 0;
+  return plan_batch_layout(model, rcfg, ccfg, num_problems).total;
+}
+
+size_t b200pets_cem_plan_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg) {
+  return b200pets_cem_plan_batch_workspace_bytes(model, rcfg, ccfg, 1);
+}
+
+int b200pets_cem_plan(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg,
+                      const float* obs0, const float* x0, const float* lower, const float* upper, const float* z,
+                      const float* eps, const int64_t* perms, float* solution, float* values_out, void* workspace,
+                      size_t workspace_bytes, void* stream) {
+  if (!model || !rcfg || !ccfg || !obs0 || !x0 || !lower || !upper || !solution || !workspace)
+    return b200pets_set_error(B200PETS_EINVAL, "cem_plan: null argument");
+  { int rc = check_eval(model, rcfg, "cem_plan"); if (rc) return rc; }
+  { int rc = check_no_external(model); if (rc) return rc; }
+  return cem_plan(model, rcfg, ccfg, 1, obs0, x0, lower, upper, z, eps, perms, solution, values_out, workspace, workspace_bytes,
+                  (cudaStream_t)stream, "cem_plan");
+}
+
+int b200pets_cem_plan_batch(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg,
+                            int32_t num_problems, const float* obs0, const float* x0, const float* lower, const float* upper,
+                            const float* z, const float* eps, const int64_t* perms, float* solution, float* values_out,
+                            void* workspace, size_t workspace_bytes, void* stream) {
+  if (!model || !rcfg || !ccfg) return b200pets_set_error(B200PETS_EINVAL, "cem_plan_batch: null argument");
+  { int rc = check_batch(model, rcfg, num_problems, "cem_plan_batch"); if (rc) return rc; }
+  if (!obs0 || !x0 || !lower || !upper || !solution || !workspace)
+    return b200pets_set_error(B200PETS_EINVAL, "cem_plan_batch: null argument");
+  return cem_plan(model, rcfg, ccfg, num_problems, obs0, x0, lower, upper, z, eps, perms, solution, values_out, workspace,
+                  workspace_bytes, (cudaStream_t)stream, "cem_plan_batch");
 }
 
 namespace {
@@ -899,7 +885,7 @@ int b200pets_mppi_plan_batch(b200pets_model_t model, const b200pets_rollout_cfg*
     if (rc) return rc;
     b200pets_rollout_cfg rc_r = *rcfg;
     rc_r.offset = (rcfg->offset + (unsigned long long)r) * 1024;
-    rc = eval_rows_batch(model, &rc_r, K, obs0, pop, popk, perms ? perms + (size_t)r * nperm * B : nullptr, (long long)R * nperm * B,
+    rc = eval_rows(model, &rc_r, K, obs0, pop, popk, perms ? perms + (size_t)r * nperm * B : nullptr, (long long)R * nperm * B,
                          eps ? eps + (size_t)r * H * B * d.out_size : nullptr, (long long)R * H * B * d.out_size, totals, eval_ws,
                          stream, (unsigned long long)R * 1024);
     if (rc) return rc;
@@ -1210,8 +1196,10 @@ static int latent_check_params(const float* const* params, const char* who) {
   return B200PETS_OK;
 }
 
-// checks of the latent evaluation and plan entry points: the fields of b200pets_rollout_cfg they read or constrain
-static int latent_check_cfg(const b200pets_rollout_cfg* cfg, const char* who) {
+// checks of the latent evaluation and plan entry points: the problem count and the fields of b200pets_rollout_cfg they
+// read or constrain
+static int latent_check_cfg(const b200pets_rollout_cfg* cfg, int32_t num_problems, const char* who) {
+  if (num_problems < 1) return b200pets_set_error(B200PETS_EINVAL, "%s: num_problems must be at least 1 (got %d)", who, num_problems);
   if (cfg->population <= 0 || cfg->horizon <= 0 || cfg->particles <= 0)
     return b200pets_set_error(B200PETS_EINVAL, "%s: population, horizon, particles must be positive", who);
   if (cfg->precision != B200PETS_PREC_F32)
@@ -1236,6 +1224,65 @@ static void latent_rollout_args(const b200pets_rollout_cfg* cfg, unsigned long l
   a->seed = rng_key(cfg->seed, offset);
   a->offset = offset;
   a->totals = totals;
+}
+
+// problem k of a batch: posterior k, its slice of every per-problem array, Philox offset a.offset + k * offset_step
+static LatentBatch latent_batch_strides(const b200pets_latent_model_desc& d, const b200pets_rollout_cfg* cfg, long long eps_stride,
+                                        unsigned long long offset_step) {
+  LatentBatch bt{};
+  const long long B = (long long)cfg->population * cfg->particles;
+  bt.latent0 = d.latent_size;
+  bt.belief0 = d.belief_size;
+  bt.act = (long long)cfg->population * cfg->horizon * d.action_size;
+  bt.eps = eps_stride;
+  bt.rows = B;
+  bt.seed = cfg->seed;
+  bt.offset_step = offset_step;
+  return bt;
+}
+
+// b200pets_latent_eval_sequences(_batch) past their own checks: K evaluations from K posteriors, one particle mean over
+// their K * N sequences
+static int latent_eval_sequences(b200pets_latent_model_t model, const b200pets_rollout_cfg* cfg, int K, const float* latent0,
+                                 const float* belief0, const float* actions, const float* eps, float* returns,
+                                 float* row_returns, void* workspace, size_t workspace_bytes, cudaStream_t stream,
+                                 const char* who) {
+  if (workspace_bytes < b200pets_latent_eval_batch_workspace_bytes(model, cfg, K))
+    return b200pets_set_error(B200PETS_EINVAL, "%s: workspace too small", who);
+  const long long B = (long long)cfg->population * cfg->particles;
+  float* totals = row_returns ? row_returns : reinterpret_cast<float*>(workspace);
+  LatentArgs a;
+  latent_rollout_args(cfg, cfg->offset, latent0, belief0, actions, eps, totals, &a);
+  int rc = launch_latent_rollout(model->dev, a, K,
+                                 latent_batch_strides(model->desc, cfg, (long long)cfg->horizon * B * model->desc.latent_size, 1024),
+                                 stream);
+  if (rc) return rc;
+  // problem k's totals are rows k * B .. k * B + B - 1: one particle mean over K * N sequences
+  return launch_particle_mean(K * cfg->population, cfg->particles, totals, returns, stream);  // model_env.py:190-191
+}
+
+// b200pets_latent_cem_plan(_batch) past their own checks: the plan of b200pets_cem_plan_batch around the latent rollout
+static int latent_cem_plan(b200pets_latent_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg, int K,
+                           const float* latent0, const float* belief0, const float* x0, const float* lower, const float* upper,
+                           const float* z, const float* eps, float* solution, float* values_out, void* workspace,
+                           size_t workspace_bytes, cudaStream_t stream, const char* who) {
+  { int rc = check_cem(rcfg, ccfg, who); if (rc) return rc; }
+  if (workspace_bytes < b200pets_latent_cem_plan_batch_workspace_bytes(model, rcfg, ccfg, K))
+    return b200pets_set_error(B200PETS_EINVAL, "%s: workspace too small", who);
+  const int H = rcfg->horizon, L = model->desc.latent_size, iters = ccfg->num_iterations;
+  const int dims = H * model->desc.action_size;
+  const long long B = (long long)rcfg->population * rcfg->particles;
+  const PlanBatchLayout l = plan_batch_layout(rcfg->population, dims, ccfg->elite_num,
+                                              b200pets_latent_eval_batch_workspace_bytes(model, rcfg, K), K);
+  unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
+  const LatentBatch bt = latent_batch_strides(model->desc, rcfg, (long long)iters * H * B * L, 1024);
+  return cem_plan_run(rcfg, ccfg, K, dims, l, ws, reinterpret_cast<float*>(ws + l.eval), x0, lower, upper, z, solution,
+                      values_out, stream, [&](int it, const float* pop, float* totals) {
+                        LatentArgs a;
+                        latent_rollout_args(rcfg, rcfg->offset * 1024 + it, latent0, belief0, pop,
+                                            eps ? eps + (size_t)it * H * B * L : nullptr, totals, &a);
+                        return launch_latent_rollout(model->dev, a, K, bt, stream);
+                      });
 }
 
 extern "C" {
@@ -1310,116 +1357,40 @@ int b200pets_latent_step(b200pets_latent_model_t model, int64_t batch, const flo
   a.eps = eps; a.sample = sample ? 1 : 0;
   a.seed = rng_key(seed, offset); a.offset = offset;
   a.latent_out = next_latent; a.belief_out = next_belief; a.reward_out = reward;
-  return launch_latent_rollout(model->dev, a, (cudaStream_t)stream);
+  return launch_latent_rollout(model->dev, a, 1, LatentBatch{}, (cudaStream_t)stream);
 }
 
-size_t b200pets_latent_eval_workspace_bytes(b200pets_latent_model_t model, const b200pets_rollout_cfg* cfg) {
-  if (!model || !cfg) return 0;
-  return al256((size_t)cfg->population * cfg->particles * sizeof(float));
-}
-
-int b200pets_latent_eval_sequences(b200pets_latent_model_t model, const b200pets_rollout_cfg* cfg, const float* latent0,
-                                   const float* belief0, const float* actions, const float* eps, float* returns,
-                                   float* row_returns, void* workspace, size_t workspace_bytes, void* stream_) {
-  if (!model || !cfg || !latent0 || !belief0 || !actions || !returns || !workspace)
-    return b200pets_set_error(B200PETS_EINVAL, "latent_eval_sequences: null argument");
-  { int rc = latent_check_cfg(cfg, "latent_eval_sequences"); if (rc) return rc; }
-  if (workspace_bytes < b200pets_latent_eval_workspace_bytes(model, cfg))
-    return b200pets_set_error(B200PETS_EINVAL, "latent_eval_sequences: workspace too small");
-  cudaStream_t stream = (cudaStream_t)stream_;
-  float* totals = row_returns ? row_returns : reinterpret_cast<float*>(workspace);
-  LatentArgs a;
-  latent_rollout_args(cfg, cfg->offset, latent0, belief0, actions, eps, totals, &a);
-  int rc = launch_latent_rollout(model->dev, a, stream);
-  if (rc) return rc;
-  return launch_particle_mean(cfg->population, cfg->particles, totals, returns, stream);  // model_env.py:190-191
-}
-
-size_t b200pets_latent_cem_plan_workspace_bytes(b200pets_latent_model_t model, const b200pets_rollout_cfg* rcfg,
-                                                const b200pets_cem_cfg* ccfg) {
-  if (!model || !rcfg || !ccfg) return 0;
-  return plan_batch_layout(rcfg->population, (size_t)rcfg->horizon * model->desc.action_size, ccfg->elite_num,
-                           b200pets_latent_eval_workspace_bytes(model, rcfg), 1).total;
-}
-
-// b200pets_cem_plan with the latent rollout: the same plan around a different model
-int b200pets_latent_cem_plan(b200pets_latent_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg,
-                             const float* latent0, const float* belief0, const float* x0, const float* lower,
-                             const float* upper, const float* z, const float* eps, float* solution, float* values_out,
-                             void* workspace, size_t workspace_bytes, void* stream_) {
-  if (!model || !rcfg || !ccfg || !latent0 || !belief0 || !x0 || !lower || !upper || !solution || !workspace)
-    return b200pets_set_error(B200PETS_EINVAL, "latent_cem_plan: null argument");
-  { int rc = latent_check_cfg(rcfg, "latent_cem_plan"); if (rc) return rc; }
-  if (ccfg->num_iterations < 0 || ccfg->elite_num < 1 || ccfg->elite_num > rcfg->population)
-    return b200pets_set_error(B200PETS_EINVAL, "latent_cem_plan: %d iterations, %d elites of %d", ccfg->num_iterations,
-                              ccfg->elite_num, rcfg->population);
-  if (workspace_bytes < b200pets_latent_cem_plan_workspace_bytes(model, rcfg, ccfg))
-    return b200pets_set_error(B200PETS_EINVAL, "latent_cem_plan: workspace too small");
-  cudaStream_t stream = (cudaStream_t)stream_;
-  const int H = rcfg->horizon, L = model->desc.latent_size;
-  const int dims = H * model->desc.action_size;
-  const long long B = (long long)rcfg->population * rcfg->particles;
-  const PlanBatchLayout l = plan_batch_layout(rcfg->population, dims, ccfg->elite_num,
-                                              b200pets_latent_eval_workspace_bytes(model, rcfg), 1);
-  unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
-  return cem_plan_run(rcfg, ccfg, 1, dims, l, ws, reinterpret_cast<float*>(ws + l.eval), x0, lower, upper, z, solution,
-                      values_out, stream, [&](int it, const float* pop, float* totals) {
-                        LatentArgs a;
-                        latent_rollout_args(rcfg, rcfg->offset * 1024 + it, latent0, belief0, pop,
-                                            eps ? eps + (size_t)it * H * B * L : nullptr, totals, &a);
-                        return launch_latent_rollout(model->dev, a, stream);
-                      });
-}
-
-// Batches of K posteriors: one batched rollout launch per evaluation, the plan of b200pets_cem_plan_batch around it
+// Batches of K posteriors: one rollout launch per evaluation for all K (K = 1: the single calls)
 size_t b200pets_latent_eval_batch_workspace_bytes(b200pets_latent_model_t model, const b200pets_rollout_cfg* cfg,
                                                   int32_t num_problems) {
   if (!model || !cfg || num_problems < 1) return 0;
   return al256((size_t)num_problems * cfg->population * cfg->particles * sizeof(float));
 }
 
-static int latent_check_batch(b200pets_latent_model_t model, const b200pets_rollout_cfg* cfg, int32_t num_problems,
-                              const char* who) {
-  if (!model || !cfg) return b200pets_set_error(B200PETS_EINVAL, "%s: null argument", who);
-  if (num_problems < 1) return b200pets_set_error(B200PETS_EINVAL, "%s: num_problems must be at least 1 (got %d)", who, num_problems);
-  return latent_check_cfg(cfg, who);
+size_t b200pets_latent_eval_workspace_bytes(b200pets_latent_model_t model, const b200pets_rollout_cfg* cfg) {
+  return b200pets_latent_eval_batch_workspace_bytes(model, cfg, 1);
 }
 
-// problem k of a batch: posterior k, its slice of every per-problem array, Philox offset a.offset + k * offset_step
-static LatentBatch latent_batch_strides(const b200pets_latent_model_desc& d, const b200pets_rollout_cfg* cfg, long long eps_stride,
-                                        unsigned long long offset_step) {
-  LatentBatch bt{};
-  const long long B = (long long)cfg->population * cfg->particles;
-  bt.latent0 = d.latent_size;
-  bt.belief0 = d.belief_size;
-  bt.act = (long long)cfg->population * cfg->horizon * d.action_size;
-  bt.eps = eps_stride;
-  bt.rows = B;
-  bt.seed = cfg->seed;
-  bt.offset_step = offset_step;
-  return bt;
+int b200pets_latent_eval_sequences(b200pets_latent_model_t model, const b200pets_rollout_cfg* cfg, const float* latent0,
+                                   const float* belief0, const float* actions, const float* eps, float* returns,
+                                   float* row_returns, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!model || !cfg || !latent0 || !belief0 || !actions || !returns || !workspace)
+    return b200pets_set_error(B200PETS_EINVAL, "latent_eval_sequences: null argument");
+  { int rc = latent_check_cfg(cfg, 1, "latent_eval_sequences"); if (rc) return rc; }
+  return latent_eval_sequences(model, cfg, 1, latent0, belief0, actions, eps, returns, row_returns, workspace, workspace_bytes,
+                               (cudaStream_t)stream, "latent_eval_sequences");
 }
 
 int b200pets_latent_eval_sequences_batch(b200pets_latent_model_t model, const b200pets_rollout_cfg* cfg, int32_t num_problems,
                                          const float* latent0, const float* belief0, const float* actions, const float* eps,
                                          float* returns, float* row_returns, void* workspace, size_t workspace_bytes,
-                                         void* stream_) {
-  { int rc = latent_check_batch(model, cfg, num_problems, "latent_eval_sequences_batch"); if (rc) return rc; }
+                                         void* stream) {
+  if (!model || !cfg) return b200pets_set_error(B200PETS_EINVAL, "latent_eval_sequences_batch: null argument");
+  { int rc = latent_check_cfg(cfg, num_problems, "latent_eval_sequences_batch"); if (rc) return rc; }
   if (!latent0 || !belief0 || !actions || !returns || !workspace)
     return b200pets_set_error(B200PETS_EINVAL, "latent_eval_sequences_batch: null argument");
-  if (workspace_bytes < b200pets_latent_eval_batch_workspace_bytes(model, cfg, num_problems))
-    return b200pets_set_error(B200PETS_EINVAL, "latent_eval_sequences_batch: workspace too small");
-  cudaStream_t stream = (cudaStream_t)stream_;
-  const long long B = (long long)cfg->population * cfg->particles;
-  float* totals = row_returns ? row_returns : reinterpret_cast<float*>(workspace);
-  LatentArgs a;
-  latent_rollout_args(cfg, cfg->offset, latent0, belief0, actions, eps, totals, &a);
-  int rc = launch_latent_rollout_batch(model->dev, a, num_problems,
-                                       latent_batch_strides(model->desc, cfg, (long long)cfg->horizon * B * model->desc.latent_size, 1024),
-                                       stream);
-  if (rc) return rc;
-  // problem k's totals are rows k * B .. k * B + B - 1: one particle mean over K * N sequences
-  return launch_particle_mean(num_problems * cfg->population, cfg->particles, totals, returns, stream);  // model_env.py:190-191
+  return latent_eval_sequences(model, cfg, num_problems, latent0, belief0, actions, eps, returns, row_returns, workspace,
+                               workspace_bytes, (cudaStream_t)stream, "latent_eval_sequences_batch");
 }
 
 size_t b200pets_latent_cem_plan_batch_workspace_bytes(b200pets_latent_model_t model, const b200pets_rollout_cfg* rcfg,
@@ -1429,33 +1400,32 @@ size_t b200pets_latent_cem_plan_batch_workspace_bytes(b200pets_latent_model_t mo
                            b200pets_latent_eval_batch_workspace_bytes(model, rcfg, num_problems), num_problems).total;
 }
 
+size_t b200pets_latent_cem_plan_workspace_bytes(b200pets_latent_model_t model, const b200pets_rollout_cfg* rcfg,
+                                                const b200pets_cem_cfg* ccfg) {
+  return b200pets_latent_cem_plan_batch_workspace_bytes(model, rcfg, ccfg, 1);
+}
+
+int b200pets_latent_cem_plan(b200pets_latent_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg,
+                             const float* latent0, const float* belief0, const float* x0, const float* lower,
+                             const float* upper, const float* z, const float* eps, float* solution, float* values_out,
+                             void* workspace, size_t workspace_bytes, void* stream) {
+  if (!model || !rcfg || !ccfg || !latent0 || !belief0 || !x0 || !lower || !upper || !solution || !workspace)
+    return b200pets_set_error(B200PETS_EINVAL, "latent_cem_plan: null argument");
+  { int rc = latent_check_cfg(rcfg, 1, "latent_cem_plan"); if (rc) return rc; }
+  return latent_cem_plan(model, rcfg, ccfg, 1, latent0, belief0, x0, lower, upper, z, eps, solution, values_out, workspace,
+                         workspace_bytes, (cudaStream_t)stream, "latent_cem_plan");
+}
+
 int b200pets_latent_cem_plan_batch(b200pets_latent_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_cem_cfg* ccfg,
                                    int32_t num_problems, const float* latent0, const float* belief0, const float* x0,
                                    const float* lower, const float* upper, const float* z, const float* eps, float* solution,
-                                   float* values_out, void* workspace, size_t workspace_bytes, void* stream_) {
-  { int rc = latent_check_batch(model, rcfg, num_problems, "latent_cem_plan_batch"); if (rc) return rc; }
+                                   float* values_out, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!model || !rcfg) return b200pets_set_error(B200PETS_EINVAL, "latent_cem_plan_batch: null argument");
+  { int rc = latent_check_cfg(rcfg, num_problems, "latent_cem_plan_batch"); if (rc) return rc; }
   if (!ccfg || !latent0 || !belief0 || !x0 || !lower || !upper || !solution || !workspace)
     return b200pets_set_error(B200PETS_EINVAL, "latent_cem_plan_batch: null argument");
-  if (ccfg->num_iterations < 0 || ccfg->elite_num < 1 || ccfg->elite_num > rcfg->population)
-    return b200pets_set_error(B200PETS_EINVAL, "latent_cem_plan_batch: %d iterations, %d elites of %d", ccfg->num_iterations,
-                              ccfg->elite_num, rcfg->population);
-  const int K = num_problems;
-  if (workspace_bytes < b200pets_latent_cem_plan_batch_workspace_bytes(model, rcfg, ccfg, K))
-    return b200pets_set_error(B200PETS_EINVAL, "latent_cem_plan_batch: workspace too small");
-  const int H = rcfg->horizon, L = model->desc.latent_size, iters = ccfg->num_iterations;
-  const int dims = H * model->desc.action_size;
-  const long long B = (long long)rcfg->population * rcfg->particles;
-  const PlanBatchLayout l = plan_batch_layout(rcfg->population, dims, ccfg->elite_num,
-                                              b200pets_latent_eval_batch_workspace_bytes(model, rcfg, K), K);
-  unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
-  const LatentBatch bt = latent_batch_strides(model->desc, rcfg, (long long)iters * H * B * L, 1024);
-  return cem_plan_run(rcfg, ccfg, K, dims, l, ws, reinterpret_cast<float*>(ws + l.eval), x0, lower, upper, z, solution,
-                      values_out, (cudaStream_t)stream_, [&](int it, const float* pop, float* totals) {
-                        LatentArgs a;
-                        latent_rollout_args(rcfg, rcfg->offset * 1024 + it, latent0, belief0, pop,
-                                            eps ? eps + (size_t)it * H * B * L : nullptr, totals, &a);
-                        return launch_latent_rollout_batch(model->dev, a, K, bt, (cudaStream_t)stream_);
-                      });
+  return latent_cem_plan(model, rcfg, ccfg, num_problems, latent0, belief0, x0, lower, upper, z, eps, solution, values_out,
+                         workspace, workspace_bytes, (cudaStream_t)stream, "latent_cem_plan_batch");
 }
 
 // ---------------------------------------------------------------------------------------------------------

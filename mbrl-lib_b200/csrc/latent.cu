@@ -302,51 +302,33 @@ int latent_plan(const LatentDev& m, long long rows, LatentPlan* p) {
 }
 
 template <int R>
-static int launch_rows(const LatentDev& m, const LatentArgs& a, const LatentPlan& p, cudaStream_t stream) {
-  CUDA_TRY(cudaFuncSetAttribute(latent_rollout_kernel<R>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
-  latent_rollout_kernel<R><<<(unsigned)p.ctas, kLatentThreads, p.smem, stream>>>(m, a);
-  CUDA_TRY(cudaGetLastError());
-  return B200PETS_OK;
-}
-
-template <int R>
-static int launch_rows_batch(const LatentDev& m, const LatentArgs& a, const LatentPlan& p, int num_problems,
-                             LatentBatch bt, cudaStream_t stream) {
-  bt.tiles = (a.B + R - 1) / R;
-  CUDA_TRY(cudaFuncSetAttribute(latent_rollout_batch_kernel<R>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
-  latent_rollout_batch_kernel<R><<<(unsigned)(bt.tiles * num_problems), kLatentThreads, p.smem, stream>>>(m, a, bt);
-  CUDA_TRY(cudaGetLastError());
-  return B200PETS_OK;
-}
-
-int launch_latent_rollout(const LatentDev& m, const LatentArgs& a, cudaStream_t stream) {
-  LatentPlan p;
-  int rc = latent_plan(m, a.B, &p);
-  if (rc) return rc;
-  if (p.ctas == 0) return B200PETS_OK;
-  switch (p.rows) {
-    case 1: return launch_rows<1>(m, a, p, stream);
-    case 2: return launch_rows<2>(m, a, p, stream);
-    case 4: return launch_rows<4>(m, a, p, stream);
-    case 8: return launch_rows<8>(m, a, p, stream);
-    case 16: return launch_rows<16>(m, a, p, stream);
-    default: return launch_rows<32>(m, a, p, stream);
+static int launch_rows(const LatentDev& m, const LatentArgs& a, const LatentPlan& p, int num_problems, LatentBatch bt,
+                       cudaStream_t stream) {
+  if (num_problems == 1) {
+    CUDA_TRY(cudaFuncSetAttribute(latent_rollout_kernel<R>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
+    latent_rollout_kernel<R><<<(unsigned)p.ctas, kLatentThreads, p.smem, stream>>>(m, a);
+  } else {
+    bt.tiles = (a.B + R - 1) / R;
+    CUDA_TRY(cudaFuncSetAttribute(latent_rollout_batch_kernel<R>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
+    latent_rollout_batch_kernel<R><<<(unsigned)(bt.tiles * num_problems), kLatentThreads, p.smem, stream>>>(m, a, bt);
   }
+  CUDA_TRY(cudaGetLastError());
+  return B200PETS_OK;
 }
 
-int launch_latent_rollout_batch(const LatentDev& m, const LatentArgs& a, int num_problems, LatentBatch bt, cudaStream_t stream) {
-  if (!a.latent0 || !a.belief0 || a.latent_out || a.belief_out || a.reward_out)
+int launch_latent_rollout(const LatentDev& m, const LatentArgs& a, int num_problems, LatentBatch bt, cudaStream_t stream) {
+  if (num_problems > 1 && (!a.latent0 || !a.belief0 || a.latent_out || a.belief_out || a.reward_out))
     return b200pets_set_error(B200PETS_EUNSUPPORTED, "batched latent rollout: evaluations from a posterior only");
   LatentPlan p;
   int rc = latent_plan(m, (long long)num_problems * a.B, &p);
   if (rc) return rc;
-  if (a.B == 0) return B200PETS_OK;
+  if (p.ctas == 0) return B200PETS_OK;
   switch (p.rows) {
-    case 1: return launch_rows_batch<1>(m, a, p, num_problems, bt, stream);
-    case 2: return launch_rows_batch<2>(m, a, p, num_problems, bt, stream);
-    case 4: return launch_rows_batch<4>(m, a, p, num_problems, bt, stream);
-    case 8: return launch_rows_batch<8>(m, a, p, num_problems, bt, stream);
-    case 16: return launch_rows_batch<16>(m, a, p, num_problems, bt, stream);
-    default: return launch_rows_batch<32>(m, a, p, num_problems, bt, stream);
+    case 1: return launch_rows<1>(m, a, p, num_problems, bt, stream);
+    case 2: return launch_rows<2>(m, a, p, num_problems, bt, stream);
+    case 4: return launch_rows<4>(m, a, p, num_problems, bt, stream);
+    case 8: return launch_rows<8>(m, a, p, num_problems, bt, stream);
+    case 16: return launch_rows<16>(m, a, p, num_problems, bt, stream);
+    default: return launch_rows<32>(m, a, p, num_problems, bt, stream);
   }
 }

@@ -141,10 +141,10 @@ void latent_pack_bias(float* dst, int N, const float* b0, const float* b1, int o
 // gives one row per CTA and no CTAs.
 int latent_tile(size_t row_bytes, long long rows, LatentPlan* p);
 int latent_plan(const LatentDev& m, long long rows, LatentPlan* p);
-int launch_latent_rollout(const LatentDev& m, const LatentArgs& a, cudaStream_t stream);
-// `num_problems` copies of the evaluation `a` describes (totals only, latent0 / belief0 set) in one grid whose tile comes
-// from latent_plan over all num_problems * a.B rows; bt.tiles is set here
-int launch_latent_rollout_batch(const LatentDev& m, const LatentArgs& a, int num_problems, LatentBatch bt, cudaStream_t stream);
+// `num_problems` copies of the launch `a` describes in one grid whose tile comes from latent_plan over all
+// num_problems * a.B rows.  One problem runs latent_rollout_kernel and ignores bt; more (totals only, latent0 / belief0
+// set) run latent_rollout_batch_kernel with bt's per-problem strides (bt.tiles is set here).
+int launch_latent_rollout(const LatentDev& m, const LatentArgs& a, int num_problems, LatentBatch bt, cudaStream_t stream);
 
 // ---- Training's sequence kernels (latent_train.cu): the RSSM of PlaNetModel.forward (planet.py:354-404) ------------
 // The forward kernel reads packed transposed copies like the rollout's (LatentDev's embedding, GRU and prior fields; the

@@ -359,40 +359,31 @@ int f32_tile_plan(const ModelDev& m, F32Plan* p) {
   return B200PETS_OK;
 }
 
-int launch_rollout_f32(const ModelDev& m, const RolloutArgs& a, cudaStream_t stream) {
-  F32Plan p;
-  int rc = f32_tile_plan(m, &p);
-  if (rc) return rc;
-  const size_t sm = p.smem;
-  if (p.rows == 64) {
-    CUDA_TRY(cudaFuncSetAttribute(rollout_f32_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-    rollout_f32_kernel<64><<<(unsigned)f32_num_tiles(m, a, 64), kThreads, sm, stream>>>(m, a, p.LD);
-  } else if (p.rows == 32) {
-    CUDA_TRY(cudaFuncSetAttribute(rollout_f32_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-    rollout_f32_kernel<32><<<(unsigned)f32_num_tiles(m, a, 32), kThreads, sm, stream>>>(m, a, p.LD);
-  } else if (p.rows == 16) {
-    CUDA_TRY(cudaFuncSetAttribute(rollout_f32_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-    rollout_f32_kernel<16><<<(unsigned)f32_num_tiles(m, a, 16), kThreads, sm, stream>>>(m, a, p.LD);
+template <int TR>
+static int launch_f32_rows(const ModelDev& m, const RolloutArgs& a, const F32Plan& p, int num_problems, BatchArgs bt,
+                           cudaStream_t stream) {
+  bt.tiles = f32_num_tiles(m, a, TR);
+  if (num_problems == 1) {
+    CUDA_TRY(cudaFuncSetAttribute(rollout_f32_kernel<TR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
+    rollout_f32_kernel<TR><<<(unsigned)bt.tiles, kThreads, p.smem, stream>>>(m, a, p.LD);
   } else {
-    return b200pets_set_error(B200PETS_EUNSUPPORTED, "layer width %d needs more shared memory than a CTA has", p.wmax);
+    CUDA_TRY(cudaFuncSetAttribute(rollout_f32_batch_kernel<TR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
+    rollout_f32_batch_kernel<TR><<<(unsigned)(bt.tiles * num_problems), kThreads, p.smem, stream>>>(m, a, p.LD, bt);
   }
   CUDA_TRY(cudaGetLastError());
   return B200PETS_OK;
 }
 
-// `num_problems` evaluations of the launch `a` describes in one grid (bt: per-problem strides, bt.tiles is set here)
-int launch_rollout_f32_batch(const ModelDev& m, const RolloutArgs& a, int num_problems, BatchArgs bt, cudaStream_t stream) {
-  if (a.traj_obs || a.traj_reward || a.traj_done || a.reward_out || a.done_out)
+// `num_problems` evaluations of the launch `a` describes in one grid.  One problem runs rollout_f32_kernel and ignores
+// bt; more run rollout_f32_batch_kernel with bt's per-problem strides (bt.tiles is set here).
+int launch_rollout_f32(const ModelDev& m, const RolloutArgs& a, int num_problems, BatchArgs bt, cudaStream_t stream) {
+  if (num_problems > 1 && (a.traj_obs || a.traj_reward || a.traj_done || a.reward_out || a.done_out))
     return b200pets_set_error(B200PETS_EUNSUPPORTED, "batched rollout: evaluation outputs only");
   F32Plan p;
   int rc = f32_tile_plan(m, &p);
   if (rc) return rc;
-  if (p.rows == 0) return b200pets_set_error(B200PETS_EUNSUPPORTED, "layer width %d needs more shared memory than a CTA has", p.wmax);
-  bt.tiles = f32_num_tiles(m, a, p.rows);
-  const unsigned grid = (unsigned)(bt.tiles * num_problems);
-  auto kern = p.rows == 64 ? rollout_f32_batch_kernel<64> : p.rows == 32 ? rollout_f32_batch_kernel<32> : rollout_f32_batch_kernel<16>;
-  CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
-  kern<<<grid, kThreads, p.smem, stream>>>(m, a, p.LD, bt);
-  CUDA_TRY(cudaGetLastError());
-  return B200PETS_OK;
+  if (p.rows == 64) return launch_f32_rows<64>(m, a, p, num_problems, bt, stream);
+  if (p.rows == 32) return launch_f32_rows<32>(m, a, p, num_problems, bt, stream);
+  if (p.rows == 16) return launch_f32_rows<16>(m, a, p, num_problems, bt, stream);
+  return b200pets_set_error(B200PETS_EUNSUPPORTED, "layer width %d needs more shared memory than a CTA has", p.wmax);
 }

@@ -752,18 +752,24 @@ int tc_plan_info(const ModelDev& m, bool expectation, int* kslice, int* nstages,
 using TcKernel = void (*)(const ModelDev, const RolloutArgs, const TcPlan, const long long);
 using TcBatchKernel = void (*)(const ModelDev, const RolloutArgs, const TcPlan, const long long, const BatchArgs);
 
-// the variant of a launch: "expectation", per-step trajectory stores (b200pets_eval_trajectory)
-template <int ACT, int NWG>
-static TcKernel tc_variant(bool expect, bool traj) {
-  if (traj) return expect ? rollout_tc_kernel<ACT, true, true, NWG> : rollout_tc_kernel<ACT, false, true, NWG>;
-  return expect ? rollout_tc_kernel<ACT, true, false, NWG> : rollout_tc_kernel<ACT, false, false, NWG>;
+// The kernels of a launch: the single-problem kernel of its variant ("expectation", per-step trajectory stores for
+// b200pets_eval_trajectory) and the batched kernel of the same activation and propagation.
+struct TcKernels {
+  TcKernel single;
+  TcBatchKernel batch;
+};
+
+template <int ACT, bool EXPECT, int NWG>
+static TcKernels tc_kernels(bool traj) {
+  return {traj ? rollout_tc_kernel<ACT, EXPECT, true, NWG> : rollout_tc_kernel<ACT, EXPECT, false, NWG>,
+          rollout_tc_batch_kernel<ACT, EXPECT, NWG>};
 }
 
 template <int NWG>
-static TcKernel tc_kernel(int act, bool expect, bool traj) {
-  return act == B200PETS_ACT_SILU   ? tc_variant<B200PETS_ACT_SILU, NWG>(expect, traj)
-         : act == B200PETS_ACT_RELU ? tc_variant<B200PETS_ACT_RELU, NWG>(expect, traj)
-                                    : tc_variant<B200PETS_ACT_LEAKY_RELU, NWG>(expect, traj);
+static TcKernels tc_kernels(int act, bool expect, bool traj) {
+  if (act == B200PETS_ACT_SILU) return expect ? tc_kernels<B200PETS_ACT_SILU, true, NWG>(traj) : tc_kernels<B200PETS_ACT_SILU, false, NWG>(traj);
+  if (act == B200PETS_ACT_RELU) return expect ? tc_kernels<B200PETS_ACT_RELU, true, NWG>(traj) : tc_kernels<B200PETS_ACT_RELU, false, NWG>(traj);
+  return expect ? tc_kernels<B200PETS_ACT_LEAKY_RELU, true, NWG>(traj) : tc_kernels<B200PETS_ACT_LEAKY_RELU, false, NWG>(traj);
 }
 
 // 128-row tiles of one launch
@@ -775,53 +781,34 @@ static long long tc_launch_tiles(const ModelDev& m, const RolloutArgs& a) {
   return (long long)m.M * ((Bm + kTileM - 1) / kTileM);
 }
 
-template <int NWG>
-static TcBatchKernel tc_batch_kernel(int act, bool expect) {
-  if (act == B200PETS_ACT_SILU) return expect ? rollout_tc_batch_kernel<B200PETS_ACT_SILU, true, NWG> : rollout_tc_batch_kernel<B200PETS_ACT_SILU, false, NWG>;
-  if (act == B200PETS_ACT_RELU) return expect ? rollout_tc_batch_kernel<B200PETS_ACT_RELU, true, NWG> : rollout_tc_batch_kernel<B200PETS_ACT_RELU, false, NWG>;
-  return expect ? rollout_tc_batch_kernel<B200PETS_ACT_LEAKY_RELU, true, NWG> : rollout_tc_batch_kernel<B200PETS_ACT_LEAKY_RELU, false, NWG>;
-}
-
-// `num_problems` evaluations of the launch `a` describes in one grid (bt: per-problem strides, bt.tiles is set here).
-// The CTA shape follows the total tile count, as for a single launch of that many tiles.
-int launch_rollout_tc_batch(const ModelDev& m, const RolloutArgs& a, int num_problems, BatchArgs bt, cudaStream_t stream) {
+// `num_problems` evaluations of the launch `a` describes in one grid.  One problem runs rollout_tc_kernel and ignores
+// bt; more run rollout_tc_batch_kernel with bt's per-problem strides (bt.tiles is set here).  The CTA shape follows the
+// total tile count, as for a single launch of that many tiles.
+int launch_rollout_tc(const ModelDev& m, const RolloutArgs& a, int num_problems, BatchArgs bt, cudaStream_t stream) {
   int rc = tc_device_limits();
   if (rc) return rc;
-  if (a.traj_obs || a.traj_reward || a.traj_done || a.reward_out || a.done_out)
+  if (num_problems > 1 && (a.traj_obs || a.traj_reward || a.traj_done || a.reward_out || a.done_out))
     return b200pets_set_error(B200PETS_EUNSUPPORTED, "batched rollout: evaluation outputs only");
   const bool expect = a.propagation == B200PETS_PROP_EXPECTATION;
+  const bool traj = a.traj_obs || a.traj_reward || a.traj_done;
   bt.tiles = tc_launch_tiles(m, a);
   const long long tiles = bt.tiles * num_problems;
   TcPlan p;
   if (!tc_choose_plan(m, tiles, &p, expect))
     return b200pets_set_error(B200PETS_EUNSUPPORTED, "model dimensions outside the tensor-core path (in %d hid %d out %d)",
                               m.in, m.hid, m.out);
-  const TcBatchKernel kern = p.nwg == 1 ? tc_batch_kernel<1>(m.act, expect) : tc_batch_kernel<2>(m.act, expect);
+  const TcKernels kern = p.nwg == 1 ? tc_kernels<1>(m.act, expect, traj) : tc_kernels<2>(m.act, expect, traj);
   const int threads = p.nwg == 1 ? threads_of<1>() : threads_of<2>();
   const long long cta_tiles = tiles * (2 / p.nwg);
-  CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem_bytes));
-  const unsigned grid = (unsigned)min((long long)g_sm_count * (2 / p.nwg), cta_tiles);
-  CUDA_TRY(launch_pdl(kern, dim3(grid), dim3(threads), (size_t)p.smem_bytes, stream, m, a, p, cta_tiles, bt));
-  return B200PETS_OK;
-}
-
-int launch_rollout_tc(const ModelDev& m, const RolloutArgs& a, cudaStream_t stream) {
-  int rc = tc_device_limits();
-  if (rc) return rc;
-  const bool expect = a.propagation == B200PETS_PROP_EXPECTATION;
-  const bool traj = a.traj_obs || a.traj_reward || a.traj_done;
-  const long long tiles = tc_launch_tiles(m, a);  // 128-row tiles
-  TcPlan p;
-  if (!tc_choose_plan(m, tiles, &p, expect))
-    return b200pets_set_error(B200PETS_EUNSUPPORTED, "model dimensions outside the tensor-core path (in %d hid %d out %d)",
-                              m.in, m.hid, m.out);
-  const TcKernel kern = p.nwg == 1 ? tc_kernel<1>(m.act, expect, traj) : tc_kernel<2>(m.act, expect, traj);
-  const int threads = p.nwg == 1 ? threads_of<1>() : threads_of<2>();
-  const long long cta_tiles = tiles * (2 / p.nwg);
-  CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem_bytes));
   // 64-row CTAs: fewer than two per SM, all resident (registers: tests/test_sass_occupancy.py; shared memory: the plan)
   const unsigned grid = (unsigned)min((long long)g_sm_count * (2 / p.nwg), cta_tiles);
-  CUDA_TRY(launch_pdl(kern, dim3(grid), dim3(threads), (size_t)p.smem_bytes, stream, m, a, p, cta_tiles));
+  if (num_problems == 1) {
+    CUDA_TRY(cudaFuncSetAttribute(kern.single, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem_bytes));
+    CUDA_TRY(launch_pdl(kern.single, dim3(grid), dim3(threads), (size_t)p.smem_bytes, stream, m, a, p, cta_tiles));
+  } else {
+    CUDA_TRY(cudaFuncSetAttribute(kern.batch, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem_bytes));
+    CUDA_TRY(launch_pdl(kern.batch, dim3(grid), dim3(threads), (size_t)p.smem_bytes, stream, m, a, p, cta_tiles, bt));
+  }
   return B200PETS_OK;
 }
 

@@ -7,13 +7,14 @@
 a parameter's storage or ``_version`` counter changed, so a training round in between needs no extra call.
 
 :class:`LatentModelEnv` is what ``ModelEnv(env, planet_model, no_termination, generator=rng)`` returns: the reference's
-interface over ``b200pets_latent_step`` / ``b200pets_latent_eval_sequences``; ``CEMOptimizer`` plans over it with one
-``b200pets_latent_cem_plan`` call.  Every rollout starts at the model's posterior (``_current_posterior_sample``,
-``_current_belief``), which ``update_posterior`` (the conv encoder, run by the caller once per environment step) sets.
+interface over ``b200pets_latent_step`` and ``b200pets_latent_eval_sequences_batch``; ``CEMOptimizer`` plans over it
+with one ``b200pets_latent_cem_plan_batch`` call.  A single call is the batch of one.  Every rollout starts at the
+model's posterior (``_current_posterior_sample``, ``_current_belief``), which ``update_posterior`` (the conv encoder, run
+by the caller once per environment step) sets.
 
 For K environments at once the env itself holds K posteriors: ``update_posterior_batch`` (or ``set_posterior_batch``)
-sets them, ``evaluate_action_sequences_batch`` and ``cem_plan_batch`` (``b200pets_latent_eval_sequences_batch`` /
-``b200pets_latent_cem_plan_batch``) plan from them, and ``TrajectoryOptimizerAgent.act_batch`` plans with them.
+sets them, ``evaluate_action_sequences_batch`` and ``cem_plan(..., batch=True)`` plan from them, and
+``TrajectoryOptimizerAgent.act_batch`` plans with them.
 """
 from __future__ import annotations
 
@@ -331,7 +332,6 @@ class LatentModelEnv(ModelEnv):
         replaces the in-kernel draws; ``_entry`` k starts from the batch's posterior k instead of the model's."""
         with torch.no_grad():
             assert len(action_sequences.shape) == 3  # model_env.py:166
-            population_size, horizon, action_dim = action_sequences.shape
             assert np.ndim(initial_state) in (1, 3)  # model_env.py:169
             self._fresh()
             if _entry is None:
@@ -339,19 +339,25 @@ class LatentModelEnv(ModelEnv):
             else:
                 latent, belief = self._posterior_batch()
                 latent0, belief0 = latent[_entry], belief[_entry]
-            actions = action_sequences.to(self.device, torch.float32).contiguous()
-            cfg = self._rollout_cfg(population_size, horizon, num_particles,
-                                    self._call_offset() if _offset is None else _offset)
-            eps = None if _eps is None else _eps.to(self.device, torch.float32).contiguous()
-            returns = torch.empty(population_size, dtype=torch.float32, device=self.device)
-            need = self.lib.b200pets_latent_eval_workspace_bytes(self.staged.handle, C.byref(cfg))
-            ws = self._workspace(need)
-            with torch.cuda.device(self.device):
-                _lib.check(self.lib.b200pets_latent_eval_sequences(
-                    self.staged.handle, C.byref(cfg), _lib.ptr(latent0), _lib.ptr(belief0), _lib.ptr(actions), _lib.ptr(eps),
-                    _lib.ptr(returns), _lib.ptr(_row_returns), _lib.ptr(ws), ws.numel(), _lib.stream_ptr()),
-                    "latent_eval_sequences")
-            return returns
+            offset = self._call_offset() if _offset is None else _offset
+            return self._evaluate(action_sequences[None], latent0.view(1, -1), belief0.view(1, -1), num_particles, offset,
+                                  _eps, _row_returns)[0]
+
+    def _evaluate(self, action_sequences, latent0, belief0, num_particles, offset, eps, row_returns) -> torch.Tensor:
+        """One ``b200pets_latent_eval_sequences_batch`` launch: ``action_sequences [K, N, H, A]`` from the posteriors
+        ``latent0 [K, L]``, ``belief0 [K, Hb]``, problem k at Philox offset ``offset + k * 1024``; returns ``[K, N]``."""
+        K, population_size, horizon, _ = action_sequences.shape
+        actions = action_sequences.to(self.device, torch.float32).contiguous()
+        cfg = self._rollout_cfg(population_size, horizon, num_particles, offset)
+        eps = None if eps is None else eps.to(self.device, torch.float32).contiguous()
+        returns = torch.empty(K, population_size, dtype=torch.float32, device=self.device)
+        ws = self._workspace(self.lib.b200pets_latent_eval_batch_workspace_bytes(self.staged.handle, C.byref(cfg), K))
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.b200pets_latent_eval_sequences_batch(
+                self.staged.handle, C.byref(cfg), K, _lib.ptr(latent0), _lib.ptr(belief0), _lib.ptr(actions),
+                _lib.ptr(eps), _lib.ptr(returns), _lib.ptr(row_returns), _lib.ptr(ws), ws.numel(), _lib.stream_ptr()),
+                "latent_eval_sequences_batch")
+        return returns
 
     # ---- K posteriors (PosteriorBatch) ------------------------------------------------------------------------------
     def set_posterior_batch(self, latent, belief):
@@ -379,63 +385,33 @@ class LatentModelEnv(ModelEnv):
         ``_row_returns [K, B]``."""
         with torch.no_grad():
             assert len(action_sequences.shape) == 4  # problems, population, horizon, action_dim
-            K, population_size, horizon, _ = action_sequences.shape
+            K = action_sequences.shape[0]
             latent0, belief0 = self._posterior_batch(K)
             if np.shape(initial_states)[0] != K:
                 raise ValueError(f"{np.shape(initial_states)[0]} initial states for {K} problems")
             self._fresh()
-            actions = action_sequences.to(self.device, torch.float32).contiguous()
             if _offset is None:
                 _offset = self._call_offset()
                 self._offset += K - 1  # problem k uses the offset of the k-th of K consecutive calls
-            cfg = self._rollout_cfg(population_size, horizon, num_particles, _offset)
-            eps = None if _eps is None else _eps.to(self.device, torch.float32).contiguous()
-            returns = torch.empty(K, population_size, dtype=torch.float32, device=self.device)
-            ws = self._workspace(self.lib.b200pets_latent_eval_batch_workspace_bytes(self.staged.handle, C.byref(cfg), K))
-            with torch.cuda.device(self.device):
-                _lib.check(self.lib.b200pets_latent_eval_sequences_batch(
-                    self.staged.handle, C.byref(cfg), K, _lib.ptr(latent0), _lib.ptr(belief0), _lib.ptr(actions),
-                    _lib.ptr(eps), _lib.ptr(returns), _lib.ptr(_row_returns), _lib.ptr(ws), ws.numel(), _lib.stream_ptr()),
-                    "latent_eval_sequences_batch")
-            return returns
+            return self._evaluate(action_sequences, latent0, belief0, num_particles, _offset, _eps, _row_returns)
 
     def shuffle_member_assignment(self, *args, **kwargs):
         raise NotImplementedError("the latent model has no ensemble members")
 
     def cem_plan(self, optimizer, x0: torch.Tensor, num_particles: int, noise: Optional[torch.Tensor] = None,
-                 eps: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """``optimizer`` (a CEMOptimizer) over :meth:`evaluate_action_sequences` as one ``b200pets_latent_cem_plan``
-        call; ``noise [it, N, H, A]`` / ``eps [it, H, B, L]`` replace the population / model draws."""
-        self._fresh()
-        H, A = x0.shape
-        latent0, belief0 = self.staged.posterior()
-        rcfg = self._rollout_cfg(optimizer.population_size, H, num_particles, self._next_offset())
-        ccfg = optimizer._cem_cfg()
-        need = self.lib.b200pets_latent_cem_plan_workspace_bytes(self.staged.handle, C.byref(rcfg), C.byref(ccfg))
-        ws = self._workspace(need)
-        sol = torch.empty(H * A, dtype=torch.float32, device=self.device)
-        z = None if noise is None else noise.to(self.device, torch.float32).contiguous()
-        if eps is not None:
-            eps = eps.to(self.device, torch.float32).contiguous()
-        optimizer.last_values = None
-        if optimizer.record_values:
-            optimizer.last_values = torch.empty(optimizer.num_iterations, optimizer.population_size, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.b200pets_latent_cem_plan(
-                self.staged.handle, C.byref(rcfg), C.byref(ccfg), _lib.ptr(latent0), _lib.ptr(belief0), _lib.ptr(x0),
-                _lib.ptr(optimizer.lower_bound), _lib.ptr(optimizer.upper_bound), _lib.ptr(z), _lib.ptr(eps), _lib.ptr(sol),
-                _lib.ptr(optimizer.last_values), _lib.ptr(ws), ws.numel(), _lib.stream_ptr()), "latent_cem_plan")
-        return sol.view(H, A)
-
-    def cem_plan_batch(self, optimizer, x0: torch.Tensor, num_particles: int, noise: Optional[torch.Tensor] = None,
-                       eps: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """:meth:`cem_plan` for the K posteriors from the warm starts ``x0 [K, H, A]`` as one
-        ``b200pets_latent_cem_plan_batch`` call; problem k plans with counter value first + k, the one its own single
-        plan would take k calls later.  ``noise [K, it, N, H, A]`` / ``eps [K, it, H, B, L]``; with ``record_values``
-        ``last_values`` is ``[K, it, N]``."""
+                 eps: Optional[torch.Tensor] = None, *, batch: bool = False) -> torch.Tensor:
+        """``optimizer`` (a CEMOptimizer) over :meth:`evaluate_action_sequences` from the warm starts ``x0 [K, H, A]`` as
+        one ``b200pets_latent_cem_plan_batch`` call: K = 1 from the model's posterior, or with ``batch`` from the K
+        posteriors.  Problem k plans with counter value first + k, the one its own single plan would take k calls later.
+        ``noise [K, it, N, H, A]`` / ``eps [K, it, H, B, L]`` replace the population / model draws; with
+        ``record_values`` ``last_values`` is ``[K, it, N]``."""
         K, H, A = x0.shape
-        latent0, belief0 = self._posterior_batch(K)
-        self._fresh()
+        if batch:
+            latent0, belief0 = self._posterior_batch(K)
+            self._fresh()
+        else:
+            self._fresh()
+            latent0, belief0 = (t.view(1, -1) for t in self.staged.posterior())
         rcfg = self._rollout_cfg(optimizer.population_size, H, num_particles, self._next_offset())
         self._offset += K - 1
         ccfg = optimizer._cem_cfg()

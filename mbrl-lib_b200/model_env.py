@@ -97,20 +97,21 @@ class ModelEnv:
         return self._ws
 
     def _obs_to_device(self, initial_state: np.ndarray) -> torch.Tensor:
-        """host fp64/fp32 observation -> fp32 device vector through a pinned staging buffer."""
-        D = initial_state.shape[0]
-        if self._obs_pin is None or self._obs_pin.numel() != D:
-            self._obs_pin = torch.empty(D, dtype=torch.float32).pin_memory()
-            self._obs_dev = torch.empty(D, dtype=torch.float32, device=self.device)
+        """host fp64/fp32 observations of any shape ([D] or [K, D]) -> fp32 device tensor of that shape through a pinned
+        staging buffer."""
+        host = np.ascontiguousarray(initial_state, dtype=np.float32)
+        if self._obs_pin is None or self._obs_pin.numel() != host.size:
+            self._obs_pin = torch.empty(host.size, dtype=torch.float32).pin_memory()
+            self._obs_dev = torch.empty(host.size, dtype=torch.float32, device=self.device)
             with torch.cuda.device(self.device):
                 self._obs_evt = torch.cuda.Event()
         else:
             self._obs_evt.synchronize()  # the previous async H2D copy must have read the pinned buffer before we overwrite it
-        self._obs_pin.copy_(torch.from_numpy(np.ascontiguousarray(initial_state, dtype=np.float32)))
+        self._obs_pin.copy_(torch.from_numpy(host).reshape(-1))
         with torch.cuda.device(self.device):  # copy and event on the model's device / stream, whatever the current one is
             self._obs_dev.copy_(self._obs_pin, non_blocking=True)
             self._obs_evt.record()
-        return self._obs_dev
+        return self._obs_dev.view(host.shape)
 
     def shuffle_member_assignment(self, population: int, horizon: int, num_particles: int, offset: int,
                                   first_sequence: int = 0, global_population: int = 0) -> torch.Tensor:

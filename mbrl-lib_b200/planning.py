@@ -7,11 +7,12 @@
   host synchronisation of ours (the reference syncs on ``.item()`` / ``best_values[0] > best_value``).
 * When ``obj_fun`` is the ``evaluate_action_sequences`` closure built by
   :func:`create_trajectory_optim_agent_for_model`, ``CEMOptimizer`` runs the whole optimisation as one
-  C call (``b200pets_cem_plan``): every iteration's sample -> rollout -> refit is enqueued back to back.
+  C call (``b200pets_cem_plan_batch``, one observation being the batch of one): every iteration's sample -> rollout ->
+  refit is enqueued back to back.
   With a reward or termination callable the kernels do not know it runs the per-iteration loop instead, the
   objective applying the callable to windows of the rollout (``ModelEnv.evaluate_action_sequences``).
 * Over PlaNet's latent model (:class:`mbrl_lib_b200.latent.LatentModelEnv`) the fused plan is one
-  ``b200pets_latent_cem_plan`` call; iCEM and MPPI evaluate through its ``evaluate_action_sequences``.  For K
+  ``b200pets_latent_cem_plan_batch`` call; iCEM and MPPI evaluate through its ``evaluate_action_sequences``.  For K
   observations the environment's K posteriors plan as one ``b200pets_latent_cem_plan_batch`` call, and MPPI plans
   entry k from posterior k.
 * ``TrajectoryOptimizer`` / ``TrajectoryOptimizerAgent`` / ``create_trajectory_optim_agent_for_model``:
@@ -116,7 +117,6 @@ class CEMOptimizer(Optimizer):
         self._seed = int(torch.initial_seed()) & 0xFFFFFFFFFFFFFFFF
         self._ws = None
         self._plan_ws = None
-        self._plan_batch_ws = None
         self.record_values = False
         self.last_values = None
 
@@ -142,7 +142,13 @@ class CEMOptimizer(Optimizer):
         # the fused plan runs every iteration inside one C call, which cannot call back into Python: with a reward or
         # termination callable the kernels do not know, the loop below evaluates through the objective instead
         if isinstance(obj_fun, _FusedObjective) and callback is None and not obj_fun.model_env.has_external_callables():
-            return self._optimize_fused(obj_fun, x0, _noise, _model_noise)
+            # the plan of one observation is the batch of one
+            noise = None if _noise is None else _noise[None]
+            model_noise = None if _model_noise is None else tuple(None if t is None else t[None] for t in _model_noise)
+            sol = self._optimize_fused(obj_fun, x0[None], noise, model_noise)
+            if self.last_values is not None:
+                self.last_values = self.last_values[0]
+            return sol[0]
         shape = tuple(x0.shape)
         dims = int(np.prod(shape))
         b = self._buffers(shape)
@@ -182,7 +188,7 @@ class CEMOptimizer(Optimizer):
         x0 = x0.to(self.device, torch.float32).contiguous()
         if isinstance(obj_funs, _FusedBatchObjective):
             if callback is None and not obj_funs.model_env.has_external_callables():
-                return self._optimize_fused_batch(obj_funs, x0, _noise, _model_noise)
+                return self._optimize_fused(obj_funs, x0, _noise, _model_noise)
             obj_funs = obj_funs.entries()
         if len(obj_funs) != x0.shape[0]:
             raise ValueError(f"{len(obj_funs)} objectives for {x0.shape[0]} warm starts")
@@ -203,13 +209,19 @@ class CEMOptimizer(Optimizer):
         return torch.stack([torch.stack([torch.randperm(B, device=self.device) for _ in range(n)])
                             for _ in range(self.num_iterations)])
 
-    def _optimize_fused_batch(self, obj: _FusedBatchObjective, x0, noise, model_noise) -> torch.Tensor:
+    def _optimize_fused(self, obj, x0, noise, model_noise) -> torch.Tensor:
+        """One device-resident plan (``b200pets_cem_plan_batch``, or the latent model's) for the K observations of a
+        :class:`_FusedBatchObjective`, or for the one observation of a :class:`_FusedObjective` as K = 1.  ``x0 [K, H, A]``;
+        ``noise [K, it, N, H, A]`` and ``model_noise`` (perms, eps), each ``[K, ...]``, replace the draws.  Returns
+        ``[K, H, A]``; with ``record_values`` ``last_values`` is ``[K, it, N]``."""
         env = obj.model_env
-        if getattr(env, "is_latent", False):  # the K posteriors: b200pets_latent_cem_plan_batch, model noise = eps only
-            return env.cem_plan_batch(self, x0, obj.num_particles, noise, None if model_noise is None else model_noise[1])
+        batch = isinstance(obj, _FusedBatchObjective)
+        if getattr(env, "is_latent", False):  # b200pets_latent_cem_plan_batch, model noise = eps only
+            return env.cem_plan(self, x0, obj.num_particles, noise, None if model_noise is None else model_noise[1],
+                                batch=batch)
         env._fresh()
         K, H, A = x0.shape
-        obs = np.asarray(obj.obs)
+        obs = np.asarray(obj.obs) if batch else np.asarray(obj.obs)[None]
         if obs.ndim != 2 or obs.shape[0] != K:
             raise ValueError(f"observations must be [K={K}, obs_dim], got {tuple(obs.shape)}")
         prop = env._propagation()
@@ -226,57 +238,23 @@ class CEMOptimizer(Optimizer):
         env._offset += K - 1
         ccfg = self._cem_cfg()
         need = self.lib.b200pets_cem_plan_batch_workspace_bytes(env.staged.handle, C.byref(rcfg), C.byref(ccfg), K)
-        if self._plan_batch_ws is None or self._plan_batch_ws.numel() < need:
-            self._plan_batch_ws = torch.empty(max(need, 1), dtype=torch.uint8, device=self.device)
-        obs0 = torch.from_numpy(np.ascontiguousarray(obs, dtype=np.float32)).to(self.device)
+        if self._plan_ws is None or self._plan_ws.numel() < need:
+            self._plan_ws = torch.empty(max(need, 1), dtype=torch.uint8, device=self.device)
+        obs0 = env._obs_to_device(obs)
         sol = torch.empty(K, H * A, dtype=torch.float32, device=self.device)
         z = None if noise is None else noise.to(self.device, torch.float32).contiguous()
         if perms is not None:
             perms = perms.to(torch.int64).contiguous()
         self.last_values = None
-        if self.record_values:
+        if self.record_values:  # per-iteration objective values of the fused plan (diagnostics / tests)
             self.last_values = torch.empty(K, self.num_iterations, self.population_size, device=self.device)
         with torch.cuda.device(self.device):
             _lib.check(self.lib.b200pets_cem_plan_batch(
                 env.staged.handle, C.byref(rcfg), C.byref(ccfg), K, _lib.ptr(obs0), _lib.ptr(x0), _lib.ptr(self.lower_bound),
                 _lib.ptr(self.upper_bound), _lib.ptr(z), _lib.ptr(eps), _lib.ptr(perms), _lib.ptr(sol),
-                _lib.ptr(self.last_values), _lib.ptr(self._plan_batch_ws), self._plan_batch_ws.numel(), _lib.stream_ptr()),
+                _lib.ptr(self.last_values), _lib.ptr(self._plan_ws), self._plan_ws.numel(), _lib.stream_ptr()),
                 "cem_plan_batch")
         return sol.view(K, H, A)
-
-    def _optimize_fused(self, obj: _FusedObjective, x0, noise, model_noise) -> torch.Tensor:
-        env = obj.model_env
-        if getattr(env, "is_latent", False):  # PlaNet's latent model: b200pets_latent_cem_plan, model noise = eps only
-            return env.cem_plan(self, x0, obj.num_particles, noise, None if model_noise is None else model_noise[1])
-        env._fresh()
-        H, A = x0.shape
-        prop = env._propagation()
-        perms = eps = None
-        if model_noise is not None:
-            perms, eps = model_noise
-        if perms is None:
-            perms = self._plan_perms(env, prop, H, obj.num_particles)
-        rcfg = _lib.RolloutCfg(self.population_size, H, obj.num_particles, _lib.PREC[env.precision_for(prop)], _lib.PROP[prop],
-                               _lib.TS1_PERMS if perms is not None else _lib.TS1_TILE_SHUFFLE, env._seed,
-                               env._next_offset())
-        ccfg = self._cem_cfg()
-        need = self.lib.b200pets_cem_plan_workspace_bytes(env.staged.handle, C.byref(rcfg), C.byref(ccfg))
-        if self._plan_ws is None or self._plan_ws.numel() < need:
-            self._plan_ws = torch.empty(need, dtype=torch.uint8, device=self.device)
-        obs0 = env._obs_to_device(obj.obs)
-        sol = torch.empty(H * A, dtype=torch.float32, device=self.device)
-        z = None if noise is None else noise.to(self.device, torch.float32).contiguous()
-        if perms is not None:
-            perms = perms.to(torch.int64).contiguous()
-        self.last_values = None
-        if self.record_values:  # per-iteration objective values of the fused plan (diagnostics / tests)
-            self.last_values = torch.empty(self.num_iterations, self.population_size, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.b200pets_cem_plan(
-                env.staged.handle, C.byref(rcfg), C.byref(ccfg), _lib.ptr(obs0), _lib.ptr(x0), _lib.ptr(self.lower_bound),
-                _lib.ptr(self.upper_bound), _lib.ptr(z), _lib.ptr(eps), _lib.ptr(perms), _lib.ptr(sol),
-                _lib.ptr(self.last_values), _lib.ptr(self._plan_ws), self._plan_ws.numel(), _lib.stream_ptr()), "cem_plan")
-        return sol.view(H, A)
 
 
 class ICEMOptimizer(Optimizer):

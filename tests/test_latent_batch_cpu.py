@@ -178,17 +178,29 @@ def test_abi_refusals_need_no_device():
         return lib.b200pets_latent_cem_plan_batch(h, C.byref(c), C.byref(cc), K, dummy, dummy, x0, dummy, dummy, None, None,
                                                   dummy, None, dummy, ws, None)
 
-    for call in (ev, plan):
-        assert call(cfg(), K=0) == -1 and "num_problems" in lib.b200pets_last_error().decode()
+    # the single entry points: the same refusals, less the problem count
+    def ev1(c, K=None, ws=1 << 30, latent0=dummy, returns=dummy):
+        return lib.b200pets_latent_eval_sequences(h, C.byref(c), latent0, dummy, dummy, None, returns, None, dummy, ws, None)
+
+    def plan1(c, K=None, ws=1 << 30, x0=dummy, cc=ccfg):
+        return lib.b200pets_latent_cem_plan(h, C.byref(c), C.byref(cc), dummy, dummy, x0, dummy, dummy, None, None, dummy,
+                                            None, dummy, ws, None)
+
+    for call in (ev, plan, ev1, plan1):
+        if call in (ev, plan):
+            assert call(cfg(), K=0) == -1 and "num_problems" in lib.b200pets_last_error().decode()
         assert call(cfg(first_sequence=10)) == -2 and "sharded" in lib.b200pets_last_error().decode()
         assert call(cfg(global_population=100)) == -2
         assert call(cfg(precision=_lib.PREC["bf16_tc"])) == -2 and "fp32" in lib.b200pets_last_error().decode()
         assert call(cfg(population=0)) == -1
         assert call(cfg(), ws=0) == -1 and "workspace too small" in lib.b200pets_last_error().decode()
-    assert ev(cfg(), latent0=None) == -1 and "null" in lib.b200pets_last_error().decode()
-    assert ev(cfg(), returns=None) == -1
-    assert plan(cfg(), x0=None) == -1 and "null" in lib.b200pets_last_error().decode()
-    assert plan(cfg(), cc=_lib.CemCfg(3, 51, 0.1, 1, 1)) == -1 and "elites" in lib.b200pets_last_error().decode()
+    for call in (ev, ev1):
+        assert call(cfg(), latent0=None) == -1 and "null" in lib.b200pets_last_error().decode()
+        assert call(cfg(), returns=None) == -1
+    for call in (plan, plan1):
+        assert call(cfg(), x0=None) == -1 and "null" in lib.b200pets_last_error().decode()
+        assert call(cfg(), cc=_lib.CemCfg(3, 51, 0.1, 1, 1)) == -1 and "elites" in lib.b200pets_last_error().decode()
+        assert call(cfg(), cc=_lib.CemCfg(3, 0, 0.1, 1, 1)) == -1 and "elites" in lib.b200pets_last_error().decode()
     assert lib.b200pets_latent_eval_sequences_batch(None, C.byref(cfg()), 2, dummy, dummy, dummy, None, dummy, None, dummy,
                                                     1 << 30, None) == -1
     need1 = lib.b200pets_latent_eval_batch_workspace_bytes(h, C.byref(cfg()), 1)
