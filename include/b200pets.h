@@ -605,6 +605,33 @@ int b200pets_sequence_gather(const b200pets_replay_desc* desc, const void* const
                              const float* rew, const int64_t* starts, int32_t batch, int32_t steps, float* obs_out,
                              float* act_out, float* rew_out, void* stream);
 
+/* ---- MBPO's SAC batches from a device-resident mirror of a replay buffer (mbrl_lib_b200/replay.py) ---------------
+ * The mirror holds one packed float row per transition, [obs | action | next_obs | reward | terminated] with
+ * W = 2 * obs_dim + act_dim + 2 floats (the staging rows b200pets_sac_update reads), in chunks of 2^chunk_shift rows
+ * (separate allocations; chunks[c] holds rows [c << chunk_shift, (c + 1) << chunk_shift), NULL while unallocated). */
+typedef struct {
+  int32_t obs_dim, act_dim;
+  int64_t rows;         /* gather: rows held (indices outside [0, rows) are skipped); scatter: the ring's capacity */
+  int32_t chunk_shift;  /* in [0, B200PETS_REPLAY_MAX_CHUNK_SHIFT] */
+} b200pets_transition_desc;
+
+/* What SAC.update_parameters converts from memory.sample's rows (sac.py:86-95), as one launch:
+ *   chunks [dev] array of device pointers; indices [dev] int64[batch]; out [dev] float[batch][W]: row b = row indices[b]
+ * An index outside [0, rows), or in an unallocated chunk, leaves its output row as it was: the caller draws the
+ * indices below num_stored.  Refused: NULL pointers, batch < 1, non-positive sizes, a chunk_shift out of range. */
+int b200pets_transition_gather(const b200pets_transition_desc* desc, float* const* chunks, const int64_t* indices,
+                               int32_t batch, float* out, void* stream);
+
+/* MBPO's per-step sac_buffer.add_batch calls (mbpo.py:53-60, replay_buffer.py:588-597) written into the mirror from
+ * b200pets_mbpo_compact's packed output: row j goes to position (first + j) mod rows, which is where consecutive
+ * add_batch calls of at most `rows` rows each put it.  obs, next_obs [dev] float[count][obs_dim]; act [dev]
+ * float[count][act_dim]; reward [dev] float[count]; terminated [dev] uint8[count] (stored as 1.0 / 0.0).  The chunks
+ * the positions fall in must be allocated.  Refused: NULL pointers, count < 1 or count > rows (later rows would
+ * overwrite earlier ones in an unspecified order), first outside [0, rows), bad sizes. */
+int b200pets_transition_scatter(const b200pets_transition_desc* desc, float* const* chunks, int64_t first, int64_t count,
+                                const float* obs, const float* act, const float* next_obs, const float* reward,
+                                const uint8_t* terminated, void* stream);
+
 /* ---- Training the dynamics model (mbrl/models/model_trainer.py:70-262) ------------------------------------
  * OneDTransitionRewardModel(GaussianMLP) trained with torch.optim.Adam, fp32 throughout. */
 
@@ -728,6 +755,15 @@ int b200pets_sac_update(b200pets_sac_t sac, int32_t batch, int64_t updates, int3
                         const int64_t* adam_steps, const float* transitions, const float* eps, uint64_t seed,
                         uint64_t offset, float* alpha, float* stats, void* workspace, size_t workspace_bytes,
                         void* stream);
+
+/* n SAC updates back to back on `stream`, with no host involvement: update i is b200pets_sac_update with updates =
+ * first_update + i, adam_steps[k] + i, transitions + i * batch * W, eps + i * 2 * batch * act_dim (when eps is not
+ * NULL), offset = first_offset + i and stats + 8 * i, so it equals the i-th of n consecutive b200pets_sac_update calls
+ * bit for bit.  One workspace serves all n.  Refused: n < 1, and what b200pets_sac_update refuses. */
+int b200pets_sac_update_many(b200pets_sac_t sac, int32_t n, int32_t batch, int64_t first_update, int32_t reverse_mask,
+                             const int64_t* adam_steps, const float* transitions, const float* eps, uint64_t seed,
+                             uint64_t first_offset, float* alpha, float* stats, void* workspace, size_t workspace_bytes,
+                             void* stream);
 
 /* Self test of the wgmma building block: D[128][n] = A[128][k] * B[n][k]^T with bf16 operands staged in the
  * no-swizzle canonical layouts, the weight ring and the accumulator fragments the rollout kernel uses.  a, b [dev] float

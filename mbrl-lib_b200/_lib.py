@@ -84,6 +84,11 @@ class ReplayDesc(C.Structure):
 
 
 REPLAY_MAX_CHUNK_SHIFT = 30
+
+
+class TransitionDesc(C.Structure):
+    _fields_ = [("obs_dim", C.c_int32), ("act_dim", C.c_int32), ("rows", C.c_int64), ("chunk_shift", C.c_int32)]
+
 SAC_MAX_ACTIONS = 32
 SAC_NUM_PARAMS, SAC_NUM_CRITIC_PARAMS = 20, 12
 
@@ -189,6 +194,8 @@ _SIGNATURES = {
     "b200pets_latent_seq_backward": (C.c_int, [C.POINTER(LatentTrainDesc), C.POINTER(_P), C.c_int32, C.c_int32, _P, _P, _P,
                                                _P, _P, _P, C.POINTER(LatentTape), _P, _P]),
     "b200pets_sequence_gather": (C.c_int, [C.POINTER(ReplayDesc), _P, _P, _P, _P, C.c_int32, C.c_int32, _P, _P, _P, _P]),
+    "b200pets_transition_gather": (C.c_int, [C.POINTER(TransitionDesc), _P, _P, C.c_int32, _P, _P]),
+    "b200pets_transition_scatter": (C.c_int, [C.POINTER(TransitionDesc), _P, C.c_int64, C.c_int64, _P, _P, _P, _P, _P, _P]),
     "b200pets_train_preprocess": (C.c_int, [C.POINTER(PrepDesc), C.c_int64, _P, _P, _P, _P, _P, _P, C.POINTER(C.c_int32),
                                             C.c_int32, _P, _P, _P]),
     "b200pets_trainer_create": (C.c_int, [C.POINTER(TrainDesc), C.POINTER(_P), C.POINTER(_P), C.POINTER(_P), C.POINTER(_P)]),
@@ -206,6 +213,8 @@ _SIGNATURES = {
     "b200pets_sac_workspace_bytes": (C.c_size_t, [_P, C.c_int32]),
     "b200pets_sac_update": (C.c_int, [_P, C.c_int32, C.c_int64, C.c_int32, C.POINTER(C.c_int64), _P, _P, C.c_uint64,
                                       C.c_uint64, _P, _P, _P, C.c_size_t, _P]),
+    "b200pets_sac_update_many": (C.c_int, [_P, C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.POINTER(C.c_int64), _P, _P,
+                                           C.c_uint64, C.c_uint64, _P, _P, _P, C.c_size_t, _P]),
 }
 
 _lib = None

@@ -1178,6 +1178,26 @@ int b200pets_sac_update(b200pets_sac_t sac, int32_t batch, int64_t updates, int3
   return launch_sac_update(sac->dev, a, (cudaStream_t)stream);
 }
 
+int b200pets_sac_update_many(b200pets_sac_t sac, int32_t n, int32_t batch, int64_t first_update, int32_t reverse_mask,
+                             const int64_t* adam_steps, const float* transitions, const float* eps, uint64_t seed,
+                             uint64_t first_offset, float* alpha, float* stats, void* workspace, size_t workspace_bytes,
+                             void* stream) {
+  if (n < 1) return b200pets_set_error(B200PETS_EINVAL, "sac_update_many: n %d < 1", n);
+  if (!sac || !adam_steps || !transitions) return b200pets_set_error(B200PETS_EINVAL, "sac_update_many: NULL pointer");
+  // n enqueued launches of the one-update kernel: each is a cooperative grid, so one update cannot start before the
+  // previous one's writes are done, and every update keeps the single call's arithmetic
+  const size_t W = 2 * (size_t)sac->dev.D + sac->dev.A + 2;
+  for (int32_t i = 0; i < n; ++i) {
+    const int64_t steps[3] = {adam_steps[0] + i, adam_steps[1] + i, adam_steps[2] + i};
+    const int rc = b200pets_sac_update(sac, batch, first_update + i, reverse_mask, steps,
+                                       transitions + (size_t)i * batch * W,
+                                       eps ? eps + (size_t)i * 2 * batch * sac->dev.A : nullptr, seed, first_offset + i,
+                                       alpha, stats ? stats + 8 * (size_t)i : nullptr, workspace, workspace_bytes, stream);
+    if (rc) return rc;
+  }
+  return B200PETS_OK;
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // PlaNet's latent model (latent.cu)
 // ---------------------------------------------------------------------------------------------------------

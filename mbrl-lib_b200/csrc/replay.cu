@@ -104,7 +104,83 @@ __global__ void __launch_bounds__(kThreads) sequence_gather_kernel(const GatherA
   }
 }
 
+// ---- MBPO's SAC transitions (mbrl_lib_b200/replay.py DeviceTransitionMirror) ---------------------------------------
+// One packed float row per transition, [obs | action | next_obs | reward | terminated] (W = 2D + A + 2 floats), in
+// chunks of 2^chunk_shift rows.  Both kernels move floats only: consecutive threads take consecutive floats of the
+// flattened [rows][W] range, so a warp reads and writes whole rows.
+struct TransitionArgs {
+  long long rows;  // gather: indices outside [0, rows) are skipped; scatter: positions wrap at rows (the capacity)
+  int W, D, A, chunk_shift;
+  float* const* chunks;
+};
+
+__global__ void __launch_bounds__(kThreads) transition_gather_kernel(const TransitionArgs a, const long long* __restrict__ idx,
+                                                                     int batch, float* __restrict__ out) {
+  const long long n = (long long)batch * a.W, mask = (1LL << a.chunk_shift) - 1;
+  for (long long e = (long long)blockIdx.x * kThreads + threadIdx.x; e < n; e += (long long)gridDim.x * kThreads) {
+    const long long b = e / a.W, col = e - b * a.W;
+    const long long row = idx[b];
+    if (row < 0 || row >= a.rows) continue;  // the host draws indices below num_stored; never read past the store
+    const float* chunk = a.chunks[row >> a.chunk_shift];
+    if (chunk) out[e] = chunk[(row & mask) * a.W + col];
+  }
+}
+
+// row j of the packed rollout output goes to position (first + j) mod rows, its columns from the five arrays
+__global__ void __launch_bounds__(kThreads) transition_scatter_kernel(const TransitionArgs a, long long first, long long count,
+                                                                      const float* __restrict__ obs, const float* __restrict__ act,
+                                                                      const float* __restrict__ next_obs,
+                                                                      const float* __restrict__ reward,
+                                                                      const uint8_t* __restrict__ terminated) {
+  const long long n = count * a.W, mask = (1LL << a.chunk_shift) - 1;
+  for (long long e = (long long)blockIdx.x * kThreads + threadIdx.x; e < n; e += (long long)gridDim.x * kThreads) {
+    const long long j = e / a.W;
+    const int col = (int)(e - j * a.W);
+    const long long pos = (first + j) % a.rows;
+    float v;
+    if (col < a.D) v = obs[j * a.D + col];
+    else if (col < a.D + a.A) v = act[j * a.A + (col - a.D)];
+    else if (col < 2 * a.D + a.A) v = next_obs[j * a.D + (col - a.D - a.A)];
+    else if (col == 2 * a.D + a.A) v = reward[j];
+    else v = terminated[j] ? 1.0f : 0.0f;
+    float* chunk = a.chunks[pos >> a.chunk_shift];
+    if (chunk) chunk[(pos & mask) * a.W + col] = v;
+  }
+}
+
 int g_sms[64];  // SM count per device ordinal, read once
+
+int sm_count(const char* who, int* out) {
+  int dev = 0;
+  CUDA_TRY(cudaGetDevice(&dev));
+  if (dev < 0 || dev >= 64) return b200pets_set_error(B200PETS_EUNSUPPORTED, "%s: device ordinal %d", who, dev);
+  if (g_sms[dev] == 0) CUDA_TRY(cudaDeviceGetAttribute(&g_sms[dev], cudaDevAttrMultiProcessorCount, dev));
+  *out = g_sms[dev];
+  return B200PETS_OK;
+}
+
+int transition_args(const b200pets_transition_desc* desc, float* const* chunks, const char* who, TransitionArgs* a) {
+  if (desc->obs_dim < 1 || desc->act_dim < 1 || desc->rows < 1)
+    return b200pets_set_error(B200PETS_EINVAL, "%s: obs_dim %d, act_dim %d and rows %lld must be positive", who,
+                              desc->obs_dim, desc->act_dim, (long long)desc->rows);
+  if (desc->chunk_shift < 0 || desc->chunk_shift > B200PETS_REPLAY_MAX_CHUNK_SHIFT)
+    return b200pets_set_error(B200PETS_EINVAL, "%s: chunk_shift %d outside [0, %d]", who, desc->chunk_shift,
+                              B200PETS_REPLAY_MAX_CHUNK_SHIFT);
+  if (desc->obs_dim > (1 << 24) || desc->act_dim > (1 << 24))
+    return b200pets_set_error(B200PETS_EUNSUPPORTED, "%s: rows wider than 2^26 floats", who);
+  a->rows = desc->rows;
+  a->D = desc->obs_dim;
+  a->A = desc->act_dim;
+  a->W = 2 * desc->obs_dim + desc->act_dim + 2;
+  a->chunk_shift = desc->chunk_shift;
+  a->chunks = chunks;
+  return B200PETS_OK;
+}
+
+unsigned grid_for(long long elems, int sms) {
+  const long long blocks = (elems + kThreads - 1) / kThreads, most = (long long)sms * kCtasPerSm;
+  return (unsigned)(blocks < most ? blocks : most);
+}
 
 }  // namespace
 
@@ -156,6 +232,39 @@ int b200pets_sequence_gather(const b200pets_replay_desc* desc, const void* const
     sequence_gather_kernel<uint8_t><<<grid, kThreads, 0, s>>>(a);
   else
     sequence_gather_kernel<float><<<grid, kThreads, 0, s>>>(a);
+  CUDA_TRY(cudaGetLastError());
+  return B200PETS_OK;
+}
+
+int b200pets_transition_gather(const b200pets_transition_desc* desc, float* const* chunks, const int64_t* indices,
+                               int32_t batch, float* out, void* stream) {
+  if (!desc || !chunks || !indices || !out) return b200pets_set_error(B200PETS_EINVAL, "transition_gather: NULL argument");
+  if (batch < 1) return b200pets_set_error(B200PETS_EINVAL, "transition_gather: batch %d < 1", batch);
+  TransitionArgs a{};
+  if (const int rc = transition_args(desc, chunks, "transition_gather", &a)) return rc;
+  int sms = 0;
+  if (const int rc = sm_count("transition_gather", &sms)) return rc;
+  const long long elems = (long long)batch * a.W;
+  transition_gather_kernel<<<grid_for(elems, sms), kThreads, 0, (cudaStream_t)stream>>>(
+      a, reinterpret_cast<const long long*>(indices), batch, out);
+  CUDA_TRY(cudaGetLastError());
+  return B200PETS_OK;
+}
+
+int b200pets_transition_scatter(const b200pets_transition_desc* desc, float* const* chunks, int64_t first, int64_t count,
+                                const float* obs, const float* act, const float* next_obs, const float* reward,
+                                const uint8_t* terminated, void* stream) {
+  if (!desc || !chunks || !obs || !act || !next_obs || !reward || !terminated)
+    return b200pets_set_error(B200PETS_EINVAL, "transition_scatter: NULL argument");
+  TransitionArgs a{};
+  if (const int rc = transition_args(desc, chunks, "transition_scatter", &a)) return rc;
+  if (count < 1 || count > a.rows || first < 0 || first >= a.rows)
+    return b200pets_set_error(B200PETS_EINVAL, "transition_scatter: needs 1 <= count <= rows and 0 <= first < rows "
+                              "(first %lld, count %lld, rows %lld)", (long long)first, (long long)count, a.rows);
+  int sms = 0;
+  if (const int rc = sm_count("transition_scatter", &sms)) return rc;
+  transition_scatter_kernel<<<grid_for(count * a.W, sms), kThreads, 0, (cudaStream_t)stream>>>(
+      a, first, count, obs, act, next_obs, reward, terminated);
   CUDA_TRY(cudaGetLastError());
   return B200PETS_OK;
 }

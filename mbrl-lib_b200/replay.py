@@ -150,6 +150,7 @@ class WriteTracker:
         self.rows = len(buffer.obs)  # capacity, plus max_trajectory_length for a buffer that stores trajectories
         self._dirty = np.zeros(self.rows, dtype=bool)
         self._dirty[:int(buffer.num_stored)] = True
+        self._pending = buffer.num_stored > 0  # whether _dirty may have a set bit (take() skips the scan when not)
         self._seen = self._state()
         self._stale = False
         self._hooks = {}
@@ -170,6 +171,7 @@ class WriteTracker:
         cur = int(self.buffer.cur_idx)
         if 0 <= cur < self.rows:
             self._dirty[cur] = True
+            self._pending = True
         out = orig(*args, **kwargs)
         self._seen = self._state()
         return out
@@ -183,6 +185,7 @@ class WriteTracker:
             self._dirty[cur:cur + (cap - cur)] = True
             first, cur = cap - cur, 0
         self._dirty[cur:cur + (n - first)] = True
+        self._pending = True
         out = orig(*args, **kwargs)
         self._seen = self._state()
         return out
@@ -190,6 +193,7 @@ class WriteTracker:
     def _on_load(self, orig, *args, **kwargs):
         out = orig(*args, **kwargs)
         self._dirty[:int(self.buffer.num_stored)] = True
+        self._pending = True
         self._seen = self._state()
         return out
 
@@ -205,9 +209,18 @@ class WriteTracker:
             self._dirty[:int(self.buffer.num_stored)] = True
             self._seen = self._state()
             self._stale = False
+            self._pending = True
+        if not self._pending:
+            return np.empty(0, dtype=np.int64)
         rows = np.flatnonzero(self._dirty)
         self._dirty[rows] = False
+        self._pending = False
         return rows
+
+    def clear(self, rows: np.ndarray):
+        """Count ``rows`` as copied (rows the caller wrote to the device copy itself)."""
+        self._dirty[rows] = False
+        self._pending = bool(self._dirty.any())
 
     def mark_stale(self):
         """Make the next :meth:`take` a resync (a copy that failed part-way)."""
@@ -459,3 +472,196 @@ class SequenceGather:
             out = SequenceBatch(self._obs[:B], self._act[:B], self._rew[:B])
             m.gather(self._starts[:B], T, *out)
         return out
+
+
+# ---- MBPO's SAC transitions in device memory --------------------------------------------------------------------------
+
+_TRANSITION_DTYPES = (np.dtype(np.float32), np.dtype(np.float64))
+_TRANSITION_MIRRORS: Dict[int, "weakref.ref[DeviceTransitionMirror]"] = {}  # id of a mirrored buffer -> its mirror
+
+
+class DeviceTransitionMirror:
+    """A copy in device memory of what ``SAC.update_parameters`` reads from an mbrl-lib ``ReplayBuffer``
+    (pytorch_sac_pranz24/sac.py:76-97): ``obs``, ``action``, ``next_obs``, ``reward`` and ``terminated``, one packed
+    float32 row per transition in the layout ``b200pets_sac_update`` reads, ``[obs | action | next_obs | reward |
+    terminated]`` (W = 2 D + A + 2 floats).  float64 buffers are converted as ``torch.FloatTensor`` converts them
+    (round to nearest).  Made by :func:`mirror_transitions_to_device`.
+
+    Rows live in chunks of ``2 ** chunk_shift`` rows, each allocated the first time a row in it is written, so the
+    device memory follows the rows written rather than the capacity.  A :class:`WriteTracker` records what ``add``,
+    ``add_batch`` and ``load`` write, and :meth:`flush` copies it; ``mbpo.rollout_model_and_populate_sac_buffer`` writes
+    its rows device-to-device (:meth:`scatter`).  Writes no wrapper sees need :meth:`resync`."""
+
+    def __init__(self, buffer, device, max_bytes: Optional[int] = None, _rows_per_chunk: Optional[int] = None):
+        for name in ("obs", "action", "next_obs", "reward"):
+            a = getattr(buffer, name)
+            if a.dtype not in _TRANSITION_DTYPES:
+                raise NotImplementedError(f"the transition mirror stores float32 or float64 arrays, not {name} {a.dtype}")
+        if getattr(buffer, "trajectory_indices", None) is not None:
+            raise NotImplementedError("the transition mirror covers buffers without max_trajectory_length")
+        dev = _cuda_device(device)
+        self.obs_dim = int(np.prod(buffer.obs.shape[1:], dtype=np.int64))
+        self.act_dim = int(np.prod(buffer.action.shape[1:], dtype=np.int64))
+        self.width = 2 * self.obs_dim + self.act_dim + 2
+        self.rows = int(buffer.capacity)
+        row_bytes = 4 * self.width
+        if max_bytes is not None and self.rows * row_bytes > max_bytes:
+            raise MemoryError(f"mirroring {self.rows} rows of {row_bytes} bytes takes up to {self.rows * row_bytes} "
+                              f"bytes of device memory, more than max_bytes = {max_bytes}")
+        self.buffer, self.device, self.max_bytes = buffer, dev, max_bytes
+        rows_per_chunk = _rows_per_chunk or max(1, _CHUNK_BYTES // row_bytes)
+        self.chunk_shift = min(int(rows_per_chunk).bit_length() - 1, max(0, (self.rows - 1).bit_length()))
+        self._chunks = [None] * ((self.rows + (1 << self.chunk_shift) - 1) >> self.chunk_shift)
+        self._slot_rows = max(1, min(self.rows, _STAGING_SLOT_BYTES // row_bytes))
+        with torch.cuda.device(dev):
+            self._chunk_table = torch.zeros(len(self._chunks), dtype=torch.int64, device=dev)
+        self.rows_held = 0  # rows [0, rows_held) are current on the device (the buffer's num_stored at the last flush)
+        self._staging = None
+        self._events = None
+        self._slot = 0
+        self._rows_copied = 0  # rows copied by the last flush (tests)
+        self._writes = WriteTracker(buffer, owner=self)  # the buffer's wrappers keep this mirror alive
+
+    def allocated_bytes(self) -> int:
+        """Device memory the allocated chunks take."""
+        return sum(4 * self.width * int(t.shape[0]) for t in self._chunks if t is not None)
+
+    # ---- copies ----------------------------------------------------------------------------------------------------
+    def flush(self) -> int:
+        """Copy the rows written since the last flush to the device on the current stream (a resync when ``cur_idx`` /
+        ``num_stored`` changed outside the wrappers).  Returns the number of rows copied."""
+        return self._copy(self._writes.take())
+
+    def resync(self) -> int:
+        """Re-copy rows ``[0, num_stored)``: for code that writes the buffer's arrays directly, which no wrapper sees."""
+        return self._copy(self._writes.take(resync=True))
+
+    def _copy(self, rows: np.ndarray) -> int:
+        try:
+            with torch.cuda.device(self.device):
+                for lo, hi in row_runs(rows, self.chunk_shift):
+                    self._copy_run(lo, hi)
+        except BaseException:
+            self._writes.mark_stale()
+            raise
+        self.rows_held = min(int(self.buffer.num_stored), self.rows)
+        self._rows_copied = int(rows.size)
+        return self._rows_copied
+
+    def _chunk(self, c: int) -> torch.Tensor:
+        t = self._chunks[c]
+        if t is None:
+            n = min(1 << self.chunk_shift, self.rows - (c << self.chunk_shift))
+            t = torch.empty(n, self.width, dtype=torch.float32, device=self.device)
+            self._chunks[c] = t
+            self._chunk_table[c] = t.data_ptr()
+        return t
+
+    def _copy_run(self, lo: int, hi: int):
+        """Rows [lo, hi) of one chunk, through two pinned staging slots."""
+        if self._staging is None:
+            self._staging = [torch.empty(self._slot_rows, self.width, dtype=torch.float32, pin_memory=True)
+                             for _ in range(2)]
+            self._events = [torch.cuda.Event() for _ in range(2)]
+        c = lo >> self.chunk_shift
+        chunk, base = self._chunk(c), c << self.chunk_shift
+        for s in range(lo, hi, self._slot_rows):
+            e = min(hi, s + self._slot_rows)
+            k = self._slot
+            self._slot ^= 1
+            self._events[k].synchronize()  # the slot's previous copy has left it
+            stage = self._staging[k][:e - s]
+            pack_rows(self.buffer, slice(s, e), stage.numpy(), self.obs_dim, self.act_dim)
+            chunk[s - base:e - base].copy_(stage, non_blocking=True)
+            self._events[k].record()
+
+    def device_rows(self, lo: int, hi: int) -> torch.Tensor:
+        """Rows [lo, hi) of the device store (tests; one chunk per call)."""
+        c = lo >> self.chunk_shift
+        base = c << self.chunk_shift
+        if (hi - 1) >> self.chunk_shift != c:
+            raise ValueError("rows of one chunk only")
+        return self._chunk(c)[lo - base:hi - base]
+
+    def desc(self, rows: int) -> _lib.TransitionDesc:
+        d = _lib.TransitionDesc()
+        d.obs_dim, d.act_dim, d.rows, d.chunk_shift = self.obs_dim, self.act_dim, int(rows), self.chunk_shift
+        return d
+
+    # ---- device-side reads and writes ------------------------------------------------------------------------------
+    def gather(self, indices: torch.Tensor, out: torch.Tensor):
+        """``b200pets_transition_gather``: rows ``indices`` (int64 [B] on the device, each below the rows held) into
+        ``out`` [B, W] float32, on the current stream.  Call :meth:`flush` first."""
+        B = int(indices.shape[0])
+        if tuple(out.shape) != (B, self.width) or out.dtype != torch.float32 or not out.is_contiguous() or \
+                out.device != self.device:
+            raise ValueError(f"gather output {tuple(out.shape)} {out.dtype} on {out.device}: expected contiguous float32 "
+                             f"{(B, self.width)} on {self.device}")
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.load().b200pets_transition_gather(C.byref(self.desc(self.rows_held)),
+                                                               _lib.ptr(self._chunk_table), _lib.ptr(indices), B,
+                                                               _lib.ptr(out), _lib.stream_ptr()), "transition_gather")
+
+    def scatter(self, first: int, obs, act, next_obs, reward, terminated):
+        """``b200pets_transition_scatter``: the packed device rows (float32 [n, D], [n, A], [n, D], [n], uint8 [n]) to
+        positions ``(first + j) mod capacity``, on the current stream, allocating the chunks they fall in.  n must not
+        exceed the capacity.  The caller clears the positions' dirty bits once the host buffer holds the same rows."""
+        n = int(reward.shape[0])
+        pos = (first + np.arange(n, dtype=np.int64)) % self.rows
+        for c in np.unique(pos >> self.chunk_shift):
+            self._chunk(int(c))
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.load().b200pets_transition_scatter(
+                C.byref(self.desc(self.rows)), _lib.ptr(self._chunk_table), int(first), n, _lib.ptr(obs), _lib.ptr(act),
+                _lib.ptr(next_obs), _lib.ptr(reward), _lib.ptr(terminated), _lib.stream_ptr()), "transition_scatter")
+        return pos
+
+    def close(self):
+        """Restore the buffer's methods and free the device and pinned memory."""
+        self._writes.close()
+        if self._events is not None:
+            for ev in self._events:
+                ev.synchronize()
+        key = id(self.buffer)
+        if key in _TRANSITION_MIRRORS and _TRANSITION_MIRRORS[key]() is self:
+            del _TRANSITION_MIRRORS[key]
+        self._chunks, self._staging, self._events = [], None, None
+        self._chunk_table = None
+        self.rows_held = 0
+
+
+def pack_rows(buffer, rows, out: np.ndarray, D: int, A: int):
+    """``buffer``'s rows ``rows`` as SAC staging rows ``[obs | action | next_obs | reward | terminated]`` in ``out``
+    [n, 2D + A + 2] float32: numpy's float32 conversion, which rounds to nearest as ``torch.FloatTensor`` does."""
+    n = out.shape[0]
+    out[:, :D] = buffer.obs[rows].reshape(n, D)
+    out[:, D:D + A] = buffer.action[rows].reshape(n, A)
+    out[:, D + A:2 * D + A] = buffer.next_obs[rows].reshape(n, D)
+    out[:, 2 * D + A] = buffer.reward[rows]
+    out[:, 2 * D + A + 1] = buffer.terminated[rows]
+
+
+def mirror_transitions_to_device(buffer, device, max_bytes: Optional[int] = None, *,
+                                 _rows_per_chunk: Optional[int] = None) -> DeviceTransitionMirror:
+    """Mirror what ``SAC.update_parameters`` reads from an mbrl-lib ``ReplayBuffer`` (float32 or float64 arrays, no
+    ``max_trajectory_length``) in ``device`` memory; see :class:`DeviceTransitionMirror`.  From then on
+    ``mbrl_lib_b200.SAC.update_parameters`` and ``mbpo.update_agent`` gather their batches from the mirror on the
+    device, and ``mbpo.rollout_model_and_populate_sac_buffer`` writes its rollouts into it.  ``max_bytes``: refuse
+    (``MemoryError``, before allocating anything) a buffer whose full capacity would take more device memory.  The
+    buffer keeps the mirror alive until :meth:`DeviceTransitionMirror.close`.  Mirroring a buffer again on the same
+    device returns its mirror."""
+    m = find_transition_mirror(buffer)
+    if m is not None:
+        if m.device == _cuda_device(device):
+            return m
+        raise ValueError(f"this buffer is already mirrored on {m.device}; close() that mirror first")
+    m = DeviceTransitionMirror(buffer, device, max_bytes, _rows_per_chunk=_rows_per_chunk)
+    _TRANSITION_MIRRORS[id(buffer)] = weakref.ref(m)
+    return m
+
+
+def find_transition_mirror(buffer) -> Optional[DeviceTransitionMirror]:
+    """The transition mirror of ``buffer``, or None."""
+    found = _TRANSITION_MIRRORS.get(id(buffer))
+    m = found() if found is not None else None
+    return m if m is not None and m.buffer is buffer else None

@@ -9,6 +9,10 @@ of the statistics.  The networks, ``torch.optim.Adam`` optimizers and ``log_alph
 updates their tensors and the optimizers' ``exp_avg`` / ``exp_avg_sq`` in place, and this class advances each
 optimizer's ``step``, so ``state_dict()`` and checkpoints stay truthful and move both ways with the reference.
 
+When the buffer has a transition mirror on the agent's device (``replay.mirror_transitions_to_device``), the batch's
+indices are drawn on the host as ``ReplayBuffer.sample`` draws them and its rows are gathered in HBM instead.
+``update_many`` runs several updates as one ``b200pets_sac_update_many`` call, for ``mbpo.update_agent``.
+
 Draws.  The reparameterisation noise of an update comes from Philox inside the kernel, keyed by a seed drawn from torch's
 default generator at construction (``torch.manual_seed`` makes a run reproducible) and by the object's update counter.
 It is not the stream ``Normal.rsample`` would draw from torch's generator, so the agent trains with other noise than the
@@ -29,7 +33,7 @@ import torch.nn.functional as F
 from torch.distributions import Normal
 from torch.optim import Adam
 
-from . import _lib
+from . import _lib, replay
 
 LOG_SIG_MAX = 2
 LOG_SIG_MIN = -20
@@ -263,11 +267,35 @@ class SAC:
         if getattr(self, "_ws", None) is None or self._ws.numel() < need:
             self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
 
+    def _index_buffers(self, rows):
+        if rows > getattr(self, "_idx_rows", 0):
+            self._idx_host = torch.empty(rows, dtype=torch.int64).pin_memory()
+            self._idx_dev = torch.empty(rows, dtype=torch.int64, device=self.device)
+            self._idx_rows = rows
+
+    def mirror_of(self, memory):
+        """The transition mirror (``replay.mirror_transitions_to_device``) of ``memory`` that this agent gathers from,
+        or None: a mirror on another device is not read (the host packs the batch instead)."""
+        m = replay.find_transition_mirror(memory)
+        if m is None or m.device != self.device:
+            return None
+        if (m.obs_dim, m.act_dim) != (self._desc.obs_dim, self._desc.act_dim):
+            raise ValueError(f"the mirror holds {m.obs_dim} observation and {m.act_dim} action columns; this agent "
+                             f"reads {self._desc.obs_dim} and {self._desc.act_dim}")
+        return m
+
     def update_parameters(self, memory, batch_size, updates, logger=None, reverse_mask=False, _eps=None):
-        """One SAC update (sac.py:76-173).  ``_eps``: a [2][B][A] device tensor of reparameterisation draws (on s', then
-        on s) used instead of the in-kernel ones, for tests."""
-        state_batch, action_batch, next_state_batch, reward_batch, mask_batch, _ = memory.sample(batch_size).astuple()
-        B = len(state_batch)
+        """One SAC update (sac.py:76-173).  When ``memory`` has a transition mirror on this agent's device, the batch's
+        indices are drawn as ``ReplayBuffer.sample`` draws them and the rows are gathered on the device.  ``_eps``: a
+        [2][B][A] device tensor of reparameterisation draws (on s', then on s) used instead of the in-kernel ones, for
+        tests."""
+        m = self.mirror_of(memory)
+        if m is None:
+            state_batch, action_batch, next_state_batch, reward_batch, mask_batch, _ = memory.sample(batch_size).astuple()
+            B = len(state_batch)
+        else:
+            idx = memory._rng.choice(memory.num_stored, size=batch_size)  # ReplayBuffer.sample's draw
+            B = len(idx)
         D, A = self._desc.obs_dim, self._desc.act_dim
         lib = _lib.load()
         opts = self._optimizers()
@@ -276,15 +304,24 @@ class SAC:
         self._buffers(B)
         if self.alpha is not self._alpha_dev:  # args.alpha, or a temperature the caller set
             self._alpha_dev.fill_(float(self.alpha))
-        stage = self._stage_host[:B].numpy()
-        stage[:, :D] = state_batch
-        stage[:, D:D + A] = action_batch
-        stage[:, D + A:2 * D + A] = next_state_batch
-        stage[:, 2 * D + A] = reward_batch
-        stage[:, 2 * D + A + 1] = mask_batch
+        if m is None:
+            stage = self._stage_host[:B].numpy()
+            stage[:, :D] = state_batch
+            stage[:, D:D + A] = action_batch
+            stage[:, D + A:2 * D + A] = next_state_batch
+            stage[:, 2 * D + A] = reward_batch
+            stage[:, 2 * D + A + 1] = mask_batch
+        else:
+            self._index_buffers(B)
+            self._idx_host[:B].numpy()[:] = idx
         with torch.cuda.device(self.device):
             stream = torch.cuda.current_stream()
-            self._stage_dev[:B].copy_(self._stage_host[:B], non_blocking=True)
+            if m is None:
+                self._stage_dev[:B].copy_(self._stage_host[:B], non_blocking=True)
+            else:
+                m.flush()
+                self._idx_dev[:B].copy_(self._idx_host[:B], non_blocking=True)
+                m.gather(self._idx_dev[:B], self._stage_dev[:B])
             eps = None if _eps is None else _eps.contiguous()
             _lib.check(lib.b200pets_sac_update(h, B, int(updates), 1 if reverse_mask else 0, (C.c_int64 * 3)(*steps),
                                                _lib.ptr(self._stage_dev), _lib.ptr(eps), self._seed, self._updates_done,
@@ -296,9 +333,14 @@ class SAC:
         for o, ps in opts:
             for p in ps:
                 o.state[p]["step"] += 1
-        qf1, qf2, pol, alpha_loss, alpha, reward_mean, entropy, _ = self._stats_host.tolist()
         if self.automatic_entropy_tuning is True:
             self.alpha = self._alpha_dev
+        return self.log_stats(self._stats_host.tolist(), updates, logger)
+
+    def log_stats(self, stats, updates, logger=None):
+        """The seven ``logger.log`` calls of one update (sac.py:165-172) from its statistics row; returns the update's
+        ``(qf1_loss, qf2_loss, policy_loss, alpha_loss, alpha)``."""
+        qf1, qf2, pol, alpha_loss, alpha, reward_mean, entropy, _ = stats
         if logger is not None:
             logger.log("train/batch_reward", reward_mean, updates)
             logger.log("train_critic/loss", qf1 + qf2, updates)
@@ -309,6 +351,71 @@ class SAC:
             logger.log("train_alpha/loss", alpha_loss, updates)
             logger.log("train_alpha/value", alpha, updates)
         return qf1, qf2, pol, alpha_loss, alpha
+
+    def update_many(self, batches, batch_size, first_update, reverse_mask=False, _eps=None):
+        """len(batches) consecutive updates as one ``b200pets_sac_update_many`` call: update i has ``updates =
+        first_update + i`` and reads the rows ``indices`` of ``memory`` for ``batches[i] = (memory, indices)`` (int
+        arrays of ``batch_size`` rows).  Consecutive batches of one mirrored buffer are gathered on the device by one
+        launch; the others are packed on the host and copied once.  Equals the updates of as many ``update_parameters``
+        calls drawing the same indices, bit for bit.  Returns the statistics, float32 [n, 8] (``update_parameters``'
+        order; ``log_stats`` turns a row into its log calls).  ``_eps``: [n][2][B][A] device draws, for tests."""
+        n, B = len(batches), int(batch_size)
+        D, A = self._desc.obs_dim, self._desc.act_dim
+        lib = _lib.load()
+        opts = self._optimizers()
+        steps = [self._adam_state(o, ps) for o, ps in opts] + ([] if len(opts) == 3 else [0])
+        h = self._sac_handle(opts)
+        self._buffers(B)
+        W = 2 * D + A + 2
+        if n * B > getattr(self, "_many_rows", 0):
+            self._many_host = torch.empty(n * B, W, dtype=torch.float32).pin_memory()
+            self._many_dev = torch.empty(n * B, W, dtype=torch.float32, device=self.device)
+            self._many_rows = n * B
+        if n > getattr(self, "_many_stats_rows", 0):
+            self._many_stats_dev = torch.empty(n, 8, dtype=torch.float32, device=self.device)
+            self._many_stats_host = torch.empty(n, 8, dtype=torch.float32).pin_memory()
+            self._many_stats_rows = n
+        self._index_buffers(n * B)
+        if self.alpha is not self._alpha_dev:
+            self._alpha_dev.fill_(float(self.alpha))
+        runs = []  # (mirror or None, first update, end): consecutive updates with one source
+        for i, (memory, idx) in enumerate(batches):
+            if len(idx) != B:
+                raise ValueError(f"update {i} has {len(idx)} rows, not batch_size {B}")
+            m = self.mirror_of(memory)
+            if m is None:
+                replay.pack_rows(memory, idx, self._many_host[i * B:(i + 1) * B].numpy(), D, A)
+            else:
+                self._idx_host[i * B:(i + 1) * B].numpy()[:] = idx
+            if runs and runs[-1][0] is m:
+                runs[-1][2] = i + 1
+            else:
+                runs.append([m, i, i + 1])
+        with torch.cuda.device(self.device):
+            stream = torch.cuda.current_stream()
+            if any(m is None for m, _, _ in runs):
+                self._many_dev[:n * B].copy_(self._many_host[:n * B], non_blocking=True)
+            if any(m is not None for m, _, _ in runs):
+                self._idx_dev[:n * B].copy_(self._idx_host[:n * B], non_blocking=True)
+            for m, lo, hi in runs:
+                if m is not None:
+                    m.flush()
+                    m.gather(self._idx_dev[lo * B:hi * B], self._many_dev[lo * B:hi * B])
+            eps = None if _eps is None else _eps.contiguous()
+            _lib.check(lib.b200pets_sac_update_many(h, n, B, int(first_update), 1 if reverse_mask else 0,
+                                                    (C.c_int64 * 3)(*steps), _lib.ptr(self._many_dev), _lib.ptr(eps),
+                                                    self._seed, self._updates_done, _lib.ptr(self._alpha_dev),
+                                                    _lib.ptr(self._many_stats_dev), _lib.ptr(self._ws), self._ws.numel(),
+                                                    C.c_void_p(stream.cuda_stream)), "sac_update_many")
+            self._many_stats_host[:n].copy_(self._many_stats_dev[:n], non_blocking=True)
+            stream.synchronize()
+        self._updates_done += n
+        for o, ps in opts:
+            for p in ps:
+                o.state[p]["step"] += n
+        if self.automatic_entropy_tuning is True:
+            self.alpha = self._alpha_dev
+        return self._many_stats_host[:n].numpy().copy()
 
     def _close(self):
         if self._handle is not None:
