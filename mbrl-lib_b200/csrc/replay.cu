@@ -159,13 +159,16 @@ int sm_count(const char* who, int* out) {
   return B200PETS_OK;
 }
 
+int check_chunk_shift(int shift, const char* who) {
+  if (shift >= 0 && shift <= B200PETS_REPLAY_MAX_CHUNK_SHIFT) return B200PETS_OK;
+  return b200pets_set_error(B200PETS_EINVAL, "%s: chunk_shift %d outside [0, %d]", who, shift, B200PETS_REPLAY_MAX_CHUNK_SHIFT);
+}
+
 int transition_args(const b200pets_transition_desc* desc, float* const* chunks, const char* who, TransitionArgs* a) {
   if (desc->obs_dim < 1 || desc->act_dim < 1 || desc->rows < 1)
     return b200pets_set_error(B200PETS_EINVAL, "%s: obs_dim %d, act_dim %d and rows %lld must be positive", who,
                               desc->obs_dim, desc->act_dim, (long long)desc->rows);
-  if (desc->chunk_shift < 0 || desc->chunk_shift > B200PETS_REPLAY_MAX_CHUNK_SHIFT)
-    return b200pets_set_error(B200PETS_EINVAL, "%s: chunk_shift %d outside [0, %d]", who, desc->chunk_shift,
-                              B200PETS_REPLAY_MAX_CHUNK_SHIFT);
+  if (const int rc = check_chunk_shift(desc->chunk_shift, who)) return rc;
   if (desc->obs_dim > (1 << 24) || desc->act_dim > (1 << 24))
     return b200pets_set_error(B200PETS_EUNSUPPORTED, "%s: rows wider than 2^26 floats", who);
   a->rows = desc->rows;
@@ -196,9 +199,7 @@ int b200pets_sequence_gather(const b200pets_replay_desc* desc, const void* const
                               batch, steps);
   if (desc->dtype != B200PETS_DTYPE_U8 && desc->dtype != B200PETS_DTYPE_F32)
     return b200pets_set_error(B200PETS_EINVAL, "sequence_gather: unknown storage dtype %d", desc->dtype);
-  if (desc->chunk_shift < 0 || desc->chunk_shift > B200PETS_REPLAY_MAX_CHUNK_SHIFT)
-    return b200pets_set_error(B200PETS_EINVAL, "sequence_gather: chunk_shift %d outside [0, %d]", desc->chunk_shift,
-                              B200PETS_REPLAY_MAX_CHUNK_SHIFT);
+  if (const int rc = check_chunk_shift(desc->chunk_shift, "sequence_gather")) return rc;
   if (desc->frame_elems < 1 || desc->action_size < 1 || desc->rows < steps)
     return b200pets_set_error(B200PETS_EINVAL,
                               "sequence_gather: frame_elems %lld and action_size %d must be positive and rows %lld at "
@@ -207,10 +208,8 @@ int b200pets_sequence_gather(const b200pets_replay_desc* desc, const void* const
   if ((long long)batch * (steps - 1) > 0x7fffffffLL)
     return b200pets_set_error(B200PETS_EUNSUPPORTED, "sequence_gather: more than 2^31 - 1 frames (batch %d, steps %d)",
                               batch, steps);
-  int dev = 0;
-  CUDA_TRY(cudaGetDevice(&dev));
-  if (dev < 0 || dev >= 64) return b200pets_set_error(B200PETS_EUNSUPPORTED, "sequence_gather: device ordinal %d", dev);
-  if (g_sms[dev] == 0) CUDA_TRY(cudaDeviceGetAttribute(&g_sms[dev], cudaDevAttrMultiProcessorCount, dev));
+  int sms = 0;
+  if (const int rc = sm_count("sequence_gather", &sms)) return rc;
   GatherArgs a{};
   a.frame_elems = desc->frame_elems;
   a.rows = desc->rows;
@@ -226,7 +225,7 @@ int b200pets_sequence_gather(const b200pets_replay_desc* desc, const void* const
   a.act_out = act_out;
   a.rew_out = rew_out;
   const long long frames = (long long)batch * (steps - 1);
-  const unsigned grid = (unsigned)(frames < (long long)g_sms[dev] * kCtasPerSm ? frames : (long long)g_sms[dev] * kCtasPerSm);
+  const unsigned grid = (unsigned)(frames < (long long)sms * kCtasPerSm ? frames : (long long)sms * kCtasPerSm);
   cudaStream_t s = (cudaStream_t)stream;
   if (desc->dtype == B200PETS_DTYPE_U8)
     sequence_gather_kernel<uint8_t><<<grid, kThreads, 0, s>>>(a);

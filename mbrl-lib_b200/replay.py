@@ -245,49 +245,57 @@ def row_runs(rows: np.ndarray, chunk_shift: int):
     return [(int(r[0]), int(r[-1]) + 1) for r in np.split(rows, cut)]
 
 
-class DeviceReplayMirror:
-    """A copy in device memory of what PlaNet's sequence loss reads from an mbrl-lib ``ReplayBuffer``
-    (mbrl/models/planet.py:274-287): ``obs`` in the buffer's own element type (uint8 or float32), and ``action`` and
-    ``reward`` as float32, converted as ``.float()`` converts them.  ``next_obs``, ``terminated`` and ``truncated`` are
-    not mirrored.  Made by :func:`mirror_to_device`.
+class _ChunkedMirror:
+    """The device store both mirrors keep: ``rows`` rows of a buffer, each ``row_elems`` elements of ``storage``.
 
-    Frames live in chunks of ``2 ** chunk_shift`` rows, each allocated through torch's allocator the first time a row in
-    it is written, plus a device table of chunk pointers: PlaNet's buffer has room for a million frames, far more than
-    a run writes.  Actions and rewards are allocated for every row.
+    Rows live in chunks of ``2 ** chunk_shift`` rows, each allocated through torch's allocator the first time a row in
+    it is written, plus a device table of chunk pointers, so the device memory follows the rows written rather than the
+    capacity.
 
     A :class:`WriteTracker` records the rows the buffer's ``add``, ``add_batch`` and ``load`` write; :meth:`flush` copies
-    them.  Writes no wrapper sees (assignments to the buffer's arrays) need :meth:`resync`; a ``cur_idx`` or
-    ``num_stored`` that changed outside the wrappers makes :meth:`flush` resync by itself."""
+    them through two pinned staging slots, each filled by the subclass's :meth:`_fill`.  Writes no wrapper sees
+    (assignments to the buffer's arrays) need :meth:`resync`; a ``cur_idx`` or ``num_stored`` that changed outside the
+    wrappers makes :meth:`flush` resync by itself, and so does a copy that failed part-way."""
 
-    def __init__(self, buffer, device, _rows_per_chunk: Optional[int] = None):
-        obs = buffer.obs
-        if obs.dtype not in _STORAGE:
-            raise NotImplementedError(f"the replay mirror stores uint8 or float32 observations, not {obs.dtype}")
-        if not obs.flags.c_contiguous:
-            raise ValueError("the replay mirror copies rows of a C-contiguous obs array")
-        dev = _cuda_device(device)
-        self.buffer, self.device = buffer, dev
-        self.rows = len(obs)
-        self.frame_shape = tuple(int(n) for n in obs.shape[1:])
-        self.frame_elems = int(np.prod(self.frame_shape, dtype=np.int64))
-        self.action_size = int(np.prod(buffer.action.shape[1:], dtype=np.int64))
-        self.storage, self._dtype_name = _STORAGE[obs.dtype]
-        row_bytes = self.frame_elems * obs.itemsize
+    _registry: Dict[int, "weakref.ref[_ChunkedMirror]"]  # a subclass's _key(buffer) -> its mirror, one per subclass
+
+    def __init__(self, buffer, device: torch.device, rows: int, row_elems: int, storage: torch.dtype,
+                 _rows_per_chunk: Optional[int] = None):
+        self.buffer, self.device = buffer, device
+        self.rows, self._row_elems, self.storage = rows, row_elems, storage
+        row_bytes = row_elems * storage.itemsize
         rows_per_chunk = _rows_per_chunk or max(1, _CHUNK_BYTES // row_bytes)
         # a power of two, and no more rows than the whole store needs
         self.chunk_shift = min(int(rows_per_chunk).bit_length() - 1, max(0, (self.rows - 1).bit_length()))
         self._chunks = [None] * ((self.rows + (1 << self.chunk_shift) - 1) >> self.chunk_shift)
         self._slot_rows = max(1, min(self.rows, _STAGING_SLOT_BYTES // row_bytes))
-        with torch.cuda.device(dev):
-            self._chunk_table = torch.zeros(len(self._chunks), dtype=torch.int64, device=dev)
-            self.act = torch.zeros(self.rows, self.action_size, device=dev)
-            self.rew = torch.zeros(self.rows, device=dev)
+        with torch.cuda.device(device):
+            self._chunk_table = torch.zeros(len(self._chunks), dtype=torch.int64, device=device)
         self.rows_held = 0  # rows [0, rows_held) are current on the device (the buffer's num_stored at the last flush)
         self._staging = None
         self._events = None
         self._slot = 0
         self._rows_copied = 0  # rows copied by the last flush (tests)
         self._writes = WriteTracker(buffer, owner=self)  # the buffer's wrappers keep this mirror alive
+
+    @classmethod
+    def _registered(cls, buffer):
+        """The live mirror of this kind whose buffer is ``buffer``, or None."""
+        found = cls._registry.get(cls._key(buffer))
+        m = found() if found is not None else None
+        return m if m is not None and m.buffer is buffer else None
+
+    @classmethod
+    def _get_or_make(cls, buffer, device, **kwargs):
+        """``buffer``'s mirror of this kind on ``device``: the one already made, or a new one, registered."""
+        m = cls._registered(buffer)
+        if m is not None:
+            if m.device == _cuda_device(device):
+                return m
+            raise ValueError(f"this buffer is already mirrored on {m.device}; close() that mirror first")
+        m = cls(buffer, device, **kwargs)
+        cls._registry[cls._key(buffer)] = weakref.ref(m)
+        return m
 
     # ---- copies ----------------------------------------------------------------------------------------------------
     def flush(self) -> int:
@@ -316,30 +324,96 @@ class DeviceReplayMirror:
         t = self._chunks[c]
         if t is None:
             n = min(1 << self.chunk_shift, self.rows - (c << self.chunk_shift))
-            t = torch.empty(n, self.frame_elems, dtype=self.storage, device=self.device)
+            t = torch.empty(n, self._row_elems, dtype=self.storage, device=self.device)
             self._chunks[c] = t
             self._chunk_table[c] = t.data_ptr()
         return t
 
     def _copy_run(self, lo: int, hi: int):
-        """Rows [lo, hi) of one chunk."""
-        b = self.buffer
+        """Rows [lo, hi) of one chunk, through two pinned staging slots."""
         if self._staging is None:
-            self._staging = [torch.empty(self._slot_rows, self.frame_elems, dtype=self.storage, pin_memory=True)
+            self._staging = [torch.empty(self._slot_rows, self._row_elems, dtype=self.storage, pin_memory=True)
                              for _ in range(2)]
             self._events = [torch.cuda.Event() for _ in range(2)]
         c = lo >> self.chunk_shift
         chunk, base = self._chunk(c), c << self.chunk_shift
-        frames = b.obs.reshape(self.rows, self.frame_elems)
         for s in range(lo, hi, self._slot_rows):
             e = min(hi, s + self._slot_rows)
             k = self._slot
             self._slot ^= 1
             self._events[k].synchronize()  # the slot's previous copy has left it
             stage = self._staging[k][:e - s]
-            np.copyto(stage.numpy(), frames[s:e])
+            self._fill(stage.numpy(), s, e)
             chunk[s - base:e - base].copy_(stage, non_blocking=True)
             self._events[k].record()
+        self._run_copied(lo, hi)
+
+    def _fill(self, stage: np.ndarray, s: int, e: int):
+        """Put the buffer's rows [s, e) into ``stage`` [e - s, row_elems] as the device store holds them."""
+        raise NotImplementedError
+
+    def _run_copied(self, lo: int, hi: int):
+        """What else a subclass copies with rows [lo, hi), once their staging copies are queued."""
+
+    def device_rows(self, lo: int, hi: int) -> torch.Tensor:
+        """Rows [lo, hi) of the device store (tests; one chunk per call)."""
+        c = lo >> self.chunk_shift
+        base = c << self.chunk_shift
+        if (hi - 1) >> self.chunk_shift != c:
+            raise ValueError("rows of one chunk only")
+        return self._chunk(c)[lo - base:hi - base]
+
+    def close(self):
+        """Restore the buffer's methods and free the device and pinned memory."""
+        self._writes.close()
+        if self._events is not None:
+            for ev in self._events:
+                ev.synchronize()
+        key = self._key(self.buffer)
+        if key in self._registry and self._registry[key]() is self:
+            del self._registry[key]
+        self._chunks, self._staging, self._events = [], None, None
+        self._chunk_table = None
+        self.rows_held = 0
+
+
+class DeviceReplayMirror(_ChunkedMirror):
+    """A copy in device memory of what PlaNet's sequence loss reads from an mbrl-lib ``ReplayBuffer``
+    (mbrl/models/planet.py:274-287): ``obs`` in the buffer's own element type (uint8 or float32), and ``action`` and
+    ``reward`` as float32, converted as ``.float()`` converts them.  ``next_obs``, ``terminated`` and ``truncated`` are
+    not mirrored.  Made by :func:`mirror_to_device`.
+
+    Frames live in the chunked store (:class:`_ChunkedMirror`): PlaNet's buffer has room for a million frames, far more
+    than a run writes.  Actions and rewards are allocated for every row."""
+
+    _registry = _MIRRORS
+
+    def __init__(self, buffer, device, _rows_per_chunk: Optional[int] = None):
+        obs = buffer.obs
+        if obs.dtype not in _STORAGE:
+            raise NotImplementedError(f"the replay mirror stores uint8 or float32 observations, not {obs.dtype}")
+        if not obs.flags.c_contiguous:
+            raise ValueError("the replay mirror copies rows of a C-contiguous obs array")
+        dev = _cuda_device(device)
+        rows = len(obs)
+        self.frame_shape = tuple(int(n) for n in obs.shape[1:])
+        self.frame_elems = int(np.prod(self.frame_shape, dtype=np.int64))
+        self.action_size = int(np.prod(buffer.action.shape[1:], dtype=np.int64))
+        storage, self._dtype_name = _STORAGE[obs.dtype]
+        with torch.cuda.device(dev):  # before the store's tracker wraps the buffer's writers
+            self.act = torch.zeros(rows, self.action_size, device=dev)
+            self.rew = torch.zeros(rows, device=dev)
+        super().__init__(buffer, dev, rows, self.frame_elems, storage, _rows_per_chunk)
+
+    @staticmethod
+    def _key(buffer) -> int:
+        return _address(buffer.obs)  # find_mirror starts from get_all()'s views, which share the obs data
+
+    def _fill(self, stage: np.ndarray, s: int, e: int):
+        np.copyto(stage, self.buffer.obs.reshape(self.rows, self.frame_elems)[s:e])
+
+    def _run_copied(self, lo: int, hi: int):
+        b = self.buffer
         act = torch.from_numpy(np.ascontiguousarray(b.action[lo:hi]).reshape(hi - lo, self.action_size)).float()
         rew = torch.from_numpy(np.ascontiguousarray(b.reward[lo:hi])).float()
         self.act[lo:hi].copy_(act)
@@ -347,11 +421,7 @@ class DeviceReplayMirror:
 
     def device_obs(self, lo: int, hi: int) -> torch.Tensor:
         """Rows [lo, hi) of the device store's frames (tests; one chunk per call)."""
-        c = lo >> self.chunk_shift
-        base = c << self.chunk_shift
-        if (hi - 1) >> self.chunk_shift != c:
-            raise ValueError("rows of one chunk only")
-        return self._chunk(c)[lo - base:hi - base].view(hi - lo, *self.frame_shape)
+        return self.device_rows(lo, hi).view(hi - lo, *self.frame_shape)
 
     # ---- the gather ------------------------------------------------------------------------------------------------
     def desc(self) -> _lib.ReplayDesc:
@@ -377,18 +447,8 @@ class DeviceReplayMirror:
                 _lib.stream_ptr()), "sequence_gather")
 
     def close(self):
-        """Restore the buffer's methods and free the device and pinned memory."""
-        b = self.buffer
-        self._writes.close()
-        if self._events is not None:
-            for ev in self._events:
-                ev.synchronize()
-        key = _address(b.obs)
-        if key in _MIRRORS and _MIRRORS[key]() is self:
-            del _MIRRORS[key]
-        self._chunks, self._staging, self._events = [], None, None
-        self._chunk_table = self.act = self.rew = None
-        self.rows_held = 0
+        super().close()
+        self.act = self.rew = None
 
 
 def mirror_to_device(buffer, device, *, _rows_per_chunk: Optional[int] = None) -> DeviceReplayMirror:
@@ -397,15 +457,7 @@ def mirror_to_device(buffer, device, *, _rows_per_chunk: Optional[int] = None) -
     :class:`DeviceReplayMirror`.  From then on ``mbrl_lib_b200.ModelTrainer`` trains a PlaNet model from the mirror when
     it is handed a sequence sampler or iterator over ``buffer.get_all()``.  The buffer keeps the mirror alive until
     :meth:`DeviceReplayMirror.close`.  Mirroring a buffer again on the same device returns its mirror."""
-    found = _MIRRORS.get(_address(buffer.obs))
-    m = found() if found is not None else None
-    if m is not None and m.buffer is buffer:
-        if m.device == _cuda_device(device):
-            return m
-        raise ValueError(f"this buffer is already mirrored on {m.device}; close() that mirror first")
-    m = DeviceReplayMirror(buffer, device, _rows_per_chunk=_rows_per_chunk)
-    _MIRRORS[_address(buffer.obs)] = weakref.ref(m)
-    return m
+    return DeviceReplayMirror._get_or_make(buffer, device, _rows_per_chunk=_rows_per_chunk)
 
 
 def find_mirror(transitions) -> Optional[DeviceReplayMirror]:
@@ -480,17 +532,17 @@ _TRANSITION_DTYPES = (np.dtype(np.float32), np.dtype(np.float64))
 _TRANSITION_MIRRORS: Dict[int, "weakref.ref[DeviceTransitionMirror]"] = {}  # id of a mirrored buffer -> its mirror
 
 
-class DeviceTransitionMirror:
+class DeviceTransitionMirror(_ChunkedMirror):
     """A copy in device memory of what ``SAC.update_parameters`` reads from an mbrl-lib ``ReplayBuffer``
     (pytorch_sac_pranz24/sac.py:76-97): ``obs``, ``action``, ``next_obs``, ``reward`` and ``terminated``, one packed
     float32 row per transition in the layout ``b200pets_sac_update`` reads, ``[obs | action | next_obs | reward |
     terminated]`` (W = 2 D + A + 2 floats).  float64 buffers are converted as ``torch.FloatTensor`` converts them
     (round to nearest).  Made by :func:`mirror_transitions_to_device`.
 
-    Rows live in chunks of ``2 ** chunk_shift`` rows, each allocated the first time a row in it is written, so the
-    device memory follows the rows written rather than the capacity.  A :class:`WriteTracker` records what ``add``,
-    ``add_batch`` and ``load`` write, and :meth:`flush` copies it; ``mbpo.rollout_model_and_populate_sac_buffer`` writes
-    its rows device-to-device (:meth:`scatter`).  Writes no wrapper sees need :meth:`resync`."""
+    Rows live in the chunked store (:class:`_ChunkedMirror`); ``mbpo.rollout_model_and_populate_sac_buffer`` writes its
+    rows device-to-device (:meth:`scatter`)."""
+
+    _registry = _TRANSITION_MIRRORS
 
     def __init__(self, buffer, device, max_bytes: Optional[int] = None, _rows_per_chunk: Optional[int] = None):
         for name in ("obs", "action", "next_obs", "reward"):
@@ -503,85 +555,24 @@ class DeviceTransitionMirror:
         self.obs_dim = int(np.prod(buffer.obs.shape[1:], dtype=np.int64))
         self.act_dim = int(np.prod(buffer.action.shape[1:], dtype=np.int64))
         self.width = 2 * self.obs_dim + self.act_dim + 2
-        self.rows = int(buffer.capacity)
+        rows = int(buffer.capacity)
         row_bytes = 4 * self.width
-        if max_bytes is not None and self.rows * row_bytes > max_bytes:
-            raise MemoryError(f"mirroring {self.rows} rows of {row_bytes} bytes takes up to {self.rows * row_bytes} "
+        if max_bytes is not None and rows * row_bytes > max_bytes:
+            raise MemoryError(f"mirroring {rows} rows of {row_bytes} bytes takes up to {rows * row_bytes} "
                               f"bytes of device memory, more than max_bytes = {max_bytes}")
-        self.buffer, self.device, self.max_bytes = buffer, dev, max_bytes
-        rows_per_chunk = _rows_per_chunk or max(1, _CHUNK_BYTES // row_bytes)
-        self.chunk_shift = min(int(rows_per_chunk).bit_length() - 1, max(0, (self.rows - 1).bit_length()))
-        self._chunks = [None] * ((self.rows + (1 << self.chunk_shift) - 1) >> self.chunk_shift)
-        self._slot_rows = max(1, min(self.rows, _STAGING_SLOT_BYTES // row_bytes))
-        with torch.cuda.device(dev):
-            self._chunk_table = torch.zeros(len(self._chunks), dtype=torch.int64, device=dev)
-        self.rows_held = 0  # rows [0, rows_held) are current on the device (the buffer's num_stored at the last flush)
-        self._staging = None
-        self._events = None
-        self._slot = 0
-        self._rows_copied = 0  # rows copied by the last flush (tests)
-        self._writes = WriteTracker(buffer, owner=self)  # the buffer's wrappers keep this mirror alive
+        self.max_bytes = max_bytes
+        super().__init__(buffer, dev, rows, self.width, torch.float32, _rows_per_chunk)
+
+    @staticmethod
+    def _key(buffer) -> int:
+        return id(buffer)
+
+    def _fill(self, stage: np.ndarray, s: int, e: int):
+        pack_rows(self.buffer, slice(s, e), stage, self.obs_dim, self.act_dim)
 
     def allocated_bytes(self) -> int:
         """Device memory the allocated chunks take."""
         return sum(4 * self.width * int(t.shape[0]) for t in self._chunks if t is not None)
-
-    # ---- copies ----------------------------------------------------------------------------------------------------
-    def flush(self) -> int:
-        """Copy the rows written since the last flush to the device on the current stream (a resync when ``cur_idx`` /
-        ``num_stored`` changed outside the wrappers).  Returns the number of rows copied."""
-        return self._copy(self._writes.take())
-
-    def resync(self) -> int:
-        """Re-copy rows ``[0, num_stored)``: for code that writes the buffer's arrays directly, which no wrapper sees."""
-        return self._copy(self._writes.take(resync=True))
-
-    def _copy(self, rows: np.ndarray) -> int:
-        try:
-            with torch.cuda.device(self.device):
-                for lo, hi in row_runs(rows, self.chunk_shift):
-                    self._copy_run(lo, hi)
-        except BaseException:
-            self._writes.mark_stale()
-            raise
-        self.rows_held = min(int(self.buffer.num_stored), self.rows)
-        self._rows_copied = int(rows.size)
-        return self._rows_copied
-
-    def _chunk(self, c: int) -> torch.Tensor:
-        t = self._chunks[c]
-        if t is None:
-            n = min(1 << self.chunk_shift, self.rows - (c << self.chunk_shift))
-            t = torch.empty(n, self.width, dtype=torch.float32, device=self.device)
-            self._chunks[c] = t
-            self._chunk_table[c] = t.data_ptr()
-        return t
-
-    def _copy_run(self, lo: int, hi: int):
-        """Rows [lo, hi) of one chunk, through two pinned staging slots."""
-        if self._staging is None:
-            self._staging = [torch.empty(self._slot_rows, self.width, dtype=torch.float32, pin_memory=True)
-                             for _ in range(2)]
-            self._events = [torch.cuda.Event() for _ in range(2)]
-        c = lo >> self.chunk_shift
-        chunk, base = self._chunk(c), c << self.chunk_shift
-        for s in range(lo, hi, self._slot_rows):
-            e = min(hi, s + self._slot_rows)
-            k = self._slot
-            self._slot ^= 1
-            self._events[k].synchronize()  # the slot's previous copy has left it
-            stage = self._staging[k][:e - s]
-            pack_rows(self.buffer, slice(s, e), stage.numpy(), self.obs_dim, self.act_dim)
-            chunk[s - base:e - base].copy_(stage, non_blocking=True)
-            self._events[k].record()
-
-    def device_rows(self, lo: int, hi: int) -> torch.Tensor:
-        """Rows [lo, hi) of the device store (tests; one chunk per call)."""
-        c = lo >> self.chunk_shift
-        base = c << self.chunk_shift
-        if (hi - 1) >> self.chunk_shift != c:
-            raise ValueError("rows of one chunk only")
-        return self._chunk(c)[lo - base:hi - base]
 
     def desc(self, rows: int) -> _lib.TransitionDesc:
         d = _lib.TransitionDesc()
@@ -616,19 +607,6 @@ class DeviceTransitionMirror:
                 _lib.ptr(next_obs), _lib.ptr(reward), _lib.ptr(terminated), _lib.stream_ptr()), "transition_scatter")
         return pos
 
-    def close(self):
-        """Restore the buffer's methods and free the device and pinned memory."""
-        self._writes.close()
-        if self._events is not None:
-            for ev in self._events:
-                ev.synchronize()
-        key = id(self.buffer)
-        if key in _TRANSITION_MIRRORS and _TRANSITION_MIRRORS[key]() is self:
-            del _TRANSITION_MIRRORS[key]
-        self._chunks, self._staging, self._events = [], None, None
-        self._chunk_table = None
-        self.rows_held = 0
-
 
 def pack_rows(buffer, rows, out: np.ndarray, D: int, A: int):
     """``buffer``'s rows ``rows`` as SAC staging rows ``[obs | action | next_obs | reward | terminated]`` in ``out``
@@ -650,18 +628,9 @@ def mirror_transitions_to_device(buffer, device, max_bytes: Optional[int] = None
     (``MemoryError``, before allocating anything) a buffer whose full capacity would take more device memory.  The
     buffer keeps the mirror alive until :meth:`DeviceTransitionMirror.close`.  Mirroring a buffer again on the same
     device returns its mirror."""
-    m = find_transition_mirror(buffer)
-    if m is not None:
-        if m.device == _cuda_device(device):
-            return m
-        raise ValueError(f"this buffer is already mirrored on {m.device}; close() that mirror first")
-    m = DeviceTransitionMirror(buffer, device, max_bytes, _rows_per_chunk=_rows_per_chunk)
-    _TRANSITION_MIRRORS[id(buffer)] = weakref.ref(m)
-    return m
+    return DeviceTransitionMirror._get_or_make(buffer, device, max_bytes=max_bytes, _rows_per_chunk=_rows_per_chunk)
 
 
 def find_transition_mirror(buffer) -> Optional[DeviceTransitionMirror]:
     """The transition mirror of ``buffer``, or None."""
-    found = _TRANSITION_MIRRORS.get(id(buffer))
-    m = found() if found is not None else None
-    return m if m is not None and m.buffer is buffer else None
+    return DeviceTransitionMirror._registered(buffer)
