@@ -404,6 +404,49 @@ int b200pets_mppi_plan_batch(b200pets_model_t model, const b200pets_rollout_cfg*
                              const float* upper, const float* z, const float* eps, const int64_t* perms,
                              float* values_out, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Fused iCEM plan over the model: every iteration of one ICEMOptimizer.optimize driving
+ * ModelEnv.evaluate_action_sequences (trajectory_opt.py:391-487), enqueued on `stream` by one call, bit for bit the
+ * optimiser's chain of icem_sample, icem_append_elites, eval_sequences and cem_update (unbiased 0, use_std 0).
+ * Iteration i evaluates sizes[i] coloured-noise rows followed by its extra rows: none at i = 0 without carried elites
+ * (elite_in NULL); one copy of the current mu at the last iteration when i != 0; `keep` kept elites otherwise, rows
+ * keep_index[i][j] of the previous iteration's elite set (at i = 0: of elite_in, shifted by one step with a fresh end
+ * action).  The first population and each refit + next population are one launch each, so a plan is two launches per
+ * iteration (rollout, refit-and-resample); when the largest population is outside the single-CTA refit (more than 2048
+ * rows, fewer than 2 elites, or an elite set over 150 KB) the plan enqueues the chain's own kernels instead.
+ * Counters:
+ *   population noise and end actions of iteration i: Philox key sample_seed, offset sample_counter * 1024 + i (the
+ *     optimiser's seed and the counter of the optimize call);
+ *   rollout of iteration i: key rcfg->seed, offset (rcfg->offset + i) * 1024 (the environment's i-th evaluation), so a
+ *     plan takes one optimiser and num_iterations environment counter values.
+ * rcfg->population is not read: iteration i's population is sizes[i] plus its extra rows.
+ *   sizes [host] int32[num_iterations]: ICEMOptimizer.population_sizes();
+ *   obs0 [dev] float[D]; x0, lower, upper [dev] float[H*A];
+ *   elite_in [dev] float[elite_num][H][A] or NULL; keep_index [dev] int64[num_iterations][keep] or NULL (elite j);
+ *   perms [host] array of num_iterations device pointers, int64[H or 1][rows_i * P] each, or NULL (tile shuffle); the
+ *     array itself may be NULL;
+ *   solution [dev] float[H*A]; elite_out [dev] float[elite_num][H][A] (descending value);
+ *   values_out [dev] float[sum of rows_i] or NULL: iteration i's values after the NaN rule at the sum of the earlier
+ *     iterations' rows.
+ * Refused before the first launch: a NULL required pointer, num_iterations < 1, horizon < 2, keep outside
+ * [0, elite_num], elite_num outside [1, smallest population], a population b200pets_eval_sequences refuses, external
+ * reward / termination callables, a sharded rcfg, a workspace smaller than b200pets_icem_plan_workspace_bytes. */
+typedef struct {
+  int32_t num_iterations;
+  int32_t elite_num;
+  int32_t keep;               /* kept elites: min(keep_elite_size, elite_num) */
+  float alpha;
+  float exponent;             /* colored_noise_exponent */
+  int32_t return_mean_elites;
+  uint64_t sample_seed;       /* the optimiser's Philox key */
+  uint64_t sample_counter;    /* iteration i draws with offset sample_counter * 1024 + i */
+} b200pets_icem_cfg;
+size_t b200pets_icem_plan_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* rcfg,
+                                          const b200pets_icem_cfg* icfg, const int32_t* sizes);
+int b200pets_icem_plan(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_icem_cfg* icfg,
+                       const int32_t* sizes, const float* obs0, const float* x0, const float* lower, const float* upper,
+                       const float* elite_in, const int64_t* keep_index, const int64_t* const* perms, float* solution,
+                       float* elite_out, float* values_out, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- PlaNet's latent model (mbrl/models/planet.py, mbrl/algorithms/planet.py) --------------------------------
  * The prior transition and reward models PlaNet plans with, PlaNetModel.sample (planet.py:531-581), in fp32:
  *   e = relu(W_e [s, a] + b_e);  h' = GRUCell(e, h);  p = W_p2 relu(W_p1 h' + b_p1) + b_p2;

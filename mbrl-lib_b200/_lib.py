@@ -47,6 +47,12 @@ class MppiCfg(C.Structure):
                 ("sample_counter", C.c_uint64)]
 
 
+class IcemCfg(C.Structure):
+    _fields_ = [("num_iterations", C.c_int32), ("elite_num", C.c_int32), ("keep", C.c_int32), ("alpha", C.c_float),
+                ("exponent", C.c_float), ("return_mean_elites", C.c_int32), ("sample_seed", C.c_uint64),
+                ("sample_counter", C.c_uint64)]
+
+
 class LatentDesc(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("action_size", "latent_size", "belief_size", "hidden_size")] + \
                [("min_std", C.c_float)]
@@ -158,6 +164,9 @@ _SIGNATURES = {
     "b200pets_mppi_plan_batch_workspace_bytes": (C.c_size_t, [_P, C.POINTER(RolloutCfg), C.POINTER(MppiCfg), C.c_int32]),
     "b200pets_mppi_plan_batch": (C.c_int, [_P, C.POINTER(RolloutCfg), C.POINTER(MppiCfg), C.c_int32, _P, _P, _P, _P, _P, _P, _P,
                                            _P, _P, C.c_size_t, _P]),
+    "b200pets_icem_plan_workspace_bytes": (C.c_size_t, [_P, C.POINTER(RolloutCfg), C.POINTER(IcemCfg), C.POINTER(C.c_int32)]),
+    "b200pets_icem_plan": (C.c_int, [_P, C.POINTER(RolloutCfg), C.POINTER(IcemCfg), C.POINTER(C.c_int32), _P, _P, _P, _P, _P, _P,
+                                     C.POINTER(_P), _P, _P, _P, _P, C.c_size_t, _P]),
     "b200pets_peer_buffer_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "b200pets_peer_alloc": (C.c_int, [C.c_size_t, C.POINTER(C.c_void_p), C.c_char_p]),
     "b200pets_peer_open": (C.c_int, [C.c_char_p, C.POINTER(C.c_void_p)]),

@@ -30,6 +30,12 @@ int launch_cem_update_rows(int population, int dims, int elite_num, float alpha,
                            const float* population_in, const float* row_totals, int particles, float* values, float* mu,
                            float* dispersion, float* best_value, float* best_solution, void* workspace,
                            size_t workspace_bytes, void* stream);
+int launch_icem_refit_sample(int rows, int dims, int elite_num, float alpha, const float* row_totals, int particles, float* values,
+                             float* mu, float* var, float* best_value, float* best_solution, float* elites_out, void* workspace,
+                             size_t workspace_bytes, int refit, int sample, int n, int horizon, int act_dim, float exponent,
+                             int extra, int keep, int shift, const float* elite, const int64_t* index, const float* lb,
+                             const float* ub, unsigned long long seed, unsigned long long offset, unsigned int tag, float* pop,
+                             cudaStream_t stream);
 int launch_mppi_sample_batch(int num_problems, int population, int horizon, int act_dim, float beta, const float* mean,
                              const float* past, const float* lower, const float* upper, const float* z, long long z_stride,
                              unsigned long long seed, unsigned long long offset, unsigned long long offset_step, float* pop,
@@ -898,6 +904,162 @@ int b200pets_mppi_plan_batch(b200pets_model_t model, const b200pets_rollout_cfg*
       CUDA_TRY(cudaMemcpy2DAsync(values_out + (size_t)r * N, sizeof(float) * R * N, values, sizeof(float) * N, sizeof(float) * N, K,
                                  cudaMemcpyDeviceToDevice, stream));
   }
+  return B200PETS_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// fused iCEM plan: every iteration of one ICEMOptimizer.optimize over the model
+// ---------------------------------------------------------------------------------------------------------
+namespace {
+// what iteration i evaluates beyond its sizes[i] coloured-noise rows (trajectory_opt.py:442-466): nothing before any elite
+// exists, one copy of mu at the last of several iterations, the kept elites otherwise
+enum IcemExtra { kNoExtra = 0, kKeptElites = 1, kMuRow = 2 };
+int icem_extra(const b200pets_icem_cfg* icfg, int i, bool carried) {
+  if (i == 0 && !carried) return kNoExtra;
+  return (i == icfg->num_iterations - 1 && i != 0) ? kMuRow : kKeptElites;
+}
+int icem_extra_rows(const b200pets_icem_cfg* icfg, int mode) { return mode == kMuRow ? 1 : mode == kKeptElites ? icfg->keep : 0; }
+
+// the workspace of an iCEM plan, sized for its largest population (any iteration, carried elites or not)
+struct IcemLayout {
+  size_t pop, values, mu, var, best_sol, best_val, upd, eval, total;
+  size_t upd_bytes;
+  int rows_max;
+};
+IcemLayout icem_layout(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_icem_cfg* icfg, const int32_t* sizes) {
+  IcemLayout l{};
+  for (int i = 0; i < icfg->num_iterations; ++i) l.rows_max = max(l.rows_max, sizes[i] + max(icfg->keep, 1));
+  const size_t R = l.rows_max, dims = (size_t)rcfg->horizon * model->desc.act_dim;
+  b200pets_rollout_cfg r = *rcfg;
+  r.population = l.rows_max;
+  l.upd_bytes = al256(b200pets_cem_update_workspace_bytes(l.rows_max, (int)dims, icfg->elite_num));
+  size_t off = 0;
+  l.pop = off; off += al256(R * dims * 4);
+  l.values = off; off += al256(R * 4);
+  l.mu = off; off += al256(dims * 4);
+  l.var = off; off += al256(dims * 4);
+  l.best_sol = off; off += al256(dims * 4);
+  l.best_val = off; off += 256;  // best value, refit flag
+  l.upd = off; off += l.upd_bytes;
+  l.eval = off; off += al256(b200pets_eval_workspace_bytes(model, &r));
+  l.total = off;
+  return l;
+}
+}  // namespace
+
+size_t b200pets_icem_plan_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_icem_cfg* icfg,
+                                          const int32_t* sizes) {
+  if (!model || !rcfg || !icfg || !sizes || icfg->num_iterations < 1 || icfg->keep < 0) return 0;
+  return icem_layout(model, rcfg, icfg, sizes).total;
+}
+
+int b200pets_icem_plan(b200pets_model_t model, const b200pets_rollout_cfg* rcfg, const b200pets_icem_cfg* icfg, const int32_t* sizes,
+                       const float* obs0, const float* x0, const float* lower, const float* upper, const float* elite_in,
+                       const int64_t* keep_index, const int64_t* const* perms, float* solution, float* elite_out,
+                       float* values_out, void* workspace, size_t workspace_bytes, void* stream_) {
+  if (!model || !rcfg || !icfg || !sizes || !obs0 || !x0 || !lower || !upper || !solution || !elite_out || !workspace)
+    return b200pets_set_error(B200PETS_EINVAL, "icem_plan: null argument");
+  const int iters = icfg->num_iterations, E = icfg->elite_num, keep = icfg->keep, H = rcfg->horizon;
+  if (iters < 1) return b200pets_set_error(B200PETS_EINVAL, "icem_plan: num_iterations must be at least 1 (got %d)", iters);
+  if (H < 2)
+    return b200pets_set_error(B200PETS_EINVAL, "icem_plan: coloured noise needs a horizon of at least 2 (a one-step series has no "
+                                               "frequency above DC to normalise by)");
+  if (keep < 0 || keep > E) return b200pets_set_error(B200PETS_EINVAL, "icem_plan: %d kept elites of %d", keep, E);
+  { int rc = check_no_external(model); if (rc) return rc; }
+  if (rcfg->first_sequence != 0 || rcfg->global_population != 0)
+    return b200pets_set_error(B200PETS_EUNSUPPORTED, "icem_plan: the population cannot be sharded over GPUs (first_sequence %d, "
+                                                     "global_population %d)", rcfg->first_sequence, rcfg->global_population);
+  const bool carried = elite_in != nullptr;
+  std::vector<int> mode(iters), rows(iters);
+  std::vector<size_t> voff(iters);
+  size_t vsum = 0;
+  int min_rows = 0;
+  for (int i = 0; i < iters; ++i) {
+    if (sizes[i] < 1) return b200pets_set_error(B200PETS_EINVAL, "icem_plan: population %d of iteration %d", sizes[i], i);
+    mode[i] = icem_extra(icfg, i, carried);
+    rows[i] = sizes[i] + icem_extra_rows(icfg, mode[i]);
+    voff[i] = vsum;
+    vsum += rows[i];
+    min_rows = i == 0 ? rows[i] : min(min_rows, rows[i]);
+    b200pets_rollout_cfg rc_i = *rcfg;
+    rc_i.population = rows[i];
+    int rc = check_eval(model, &rc_i, "icem_plan");
+    if (rc) return rc;
+  }
+  if (E < 1 || E > min_rows)
+    return b200pets_set_error(B200PETS_EINVAL, "icem_plan: %d elites of a smallest population of %d", E, min_rows);
+  const IcemLayout l = icem_layout(model, rcfg, icfg, sizes);
+  if (workspace_bytes < l.total) return b200pets_set_error(B200PETS_EINVAL, "icem_plan: workspace too small (%zu < %zu)",
+                                                           workspace_bytes, l.total);
+  cudaStream_t stream = (cudaStream_t)stream_;
+  const b200pets_model_desc& d = model->desc;
+  const int A = d.act_dim, dims = H * A, P = rcfg->particles;
+  unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
+  float* pop = reinterpret_cast<float*>(ws + l.pop);
+  float* values = reinterpret_cast<float*>(ws + l.values);
+  float* mu = reinterpret_cast<float*>(ws + l.mu);
+  float* var = reinterpret_cast<float*>(ws + l.var);
+  float* best_sol = reinterpret_cast<float*>(ws + l.best_sol);
+  float* best_val = reinterpret_cast<float*>(ws + l.best_val);
+  void* upd_ws = ws + l.upd;
+  unsigned char* eval_ws = ws + l.eval;
+  // iteration i's values (after the NaN rule) and per-row totals: where b200pets_eval_sequences puts them for its population
+  auto vals = [&](int i) { return values_out ? values_out + voff[i] : values; };
+  auto totals = [&](int i) { return reinterpret_cast<float*>(eval_ws + al256((size_t)rows[i] * P * d.obs_dim * sizeof(float))); };
+  auto index = [&](int i) { return keep_index ? keep_index + (size_t)i * keep : nullptr; };
+  const unsigned long long sbase = icfg->sample_counter * 1024;
+
+  cem_init_kernel<<<(unsigned)((dims + 255) / 256), 256, 0, stream>>>(1, dims, x0, lower, upper, 0, mu, var, best_val);
+  CUDA_TRY(cudaGetLastError());
+  // refit of iteration it_next - 1 (if any) and the population of it_next (if any) in one launch
+  const bool merged = cem_refit_sample_supported(l.rows_max, dims, E);
+  auto next_pop = [&](int it_next, int refit) -> int {
+    const int r = refit ? rows[it_next - 1] : rows[0];
+    const int sample = it_next < iters;
+    return launch_icem_refit_sample(r, dims, E, icfg->alpha, refit ? totals(it_next - 1) : nullptr, P, refit ? vals(it_next - 1) : nullptr,
+                                    mu, var, best_val, best_sol, elite_out, upd_ws, l.upd_bytes, refit, sample,
+                                    sample ? sizes[it_next] : 0, H, A, icfg->exponent, sample ? mode[it_next] : kNoExtra, keep,
+                                    it_next == 0, it_next == 0 ? elite_in : elite_out, sample ? index(it_next) : nullptr, lower,
+                                    upper, icfg->sample_seed, sbase + (unsigned long long)it_next, (unsigned int)it_next, pop, stream);
+  };
+  if (merged) {
+    int rc = next_pop(0, 0);
+    if (rc) return rc;
+  }
+  const int nperm = rcfg->propagation == B200PETS_PROP_FIXED_MODEL ? 1 : H;
+  for (int i = 0; i < iters; ++i) {
+    const int n = sizes[i];
+    int rc;
+    if (!merged) {  // the optimiser's own chain: icem_sample, extra rows, rollout, particle mean, cem_update
+      rc = b200pets_icem_sample(n, H, A, icfg->exponent, mu, var, lower, upper, nullptr, nullptr, icfg->sample_seed, sbase + i, pop,
+                                stream);
+      if (rc) return rc;
+      if (mode[i] == kMuRow) {
+        CUDA_TRY(cudaMemcpyAsync(pop + (size_t)n * dims, mu, sizeof(float) * dims, cudaMemcpyDeviceToDevice, stream));
+      } else if (mode[i] == kKeptElites) {
+        rc = b200pets_icem_append_elites(keep, H, A, i == 0 ? elite_in : elite_out, index(i), i == 0, mu, var, nullptr,
+                                         icfg->sample_seed, sbase + i, pop + (size_t)n * dims, stream);
+        if (rc) return rc;
+      }
+    }
+    b200pets_rollout_cfg rc_i = *rcfg;
+    rc_i.population = rows[i];
+    rc_i.offset = (rcfg->offset + (unsigned long long)i) * 1024;
+    const long long B = (long long)rows[i] * P;
+    rc = eval_rows(model, &rc_i, 1, obs0, pop, (long long)rows[i] * dims, perms ? perms[i] : nullptr, (long long)nperm * B, nullptr,
+                   (long long)H * B * d.out_size, totals(i), eval_ws, stream, 1024);
+    if (rc) return rc;
+    if (merged) {
+      rc = next_pop(i + 1, 1);
+    } else {
+      rc = launch_particle_mean(rows[i], P, totals(i), vals(i), stream);  // model_env.py:190-191
+      if (rc) return rc;
+      rc = b200pets_cem_update(rows[i], dims, E, icfg->alpha, 0, 0, pop, vals(i), mu, var, best_val, best_sol, nullptr, elite_out,
+                               upd_ws, l.upd_bytes, stream);
+    }
+    if (rc) return rc;
+  }
+  CUDA_TRY(cudaMemcpyAsync(solution, icfg->return_mean_elites ? mu : best_sol, sizeof(float) * dims, cudaMemcpyDeviceToDevice, stream));
   return B200PETS_OK;
 }
 

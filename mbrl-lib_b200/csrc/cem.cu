@@ -60,15 +60,14 @@ __global__ void cem_sample_kernel(int n, int dims, const float* __restrict__ mu,
   pop[idx] = cem_sample_element(idx, dims, mu[d], disp[d], lb[d], ub[d], z, seed, offset, clipped, seq0);
 }
 
-// iCEM coloured noise: one thread per (sequence, action dim) synthesises the H samples of its series
-__global__ void icem_sample_kernel(int n, int H, int A, float exponent, const float* __restrict__ mu,
-                                   const float* __restrict__ var, const float* __restrict__ lb,
-                                   const float* __restrict__ ub, const float* __restrict__ sr,
-                                   const float* __restrict__ si, unsigned long long seed, unsigned long long offset,
-                                   float* __restrict__ pop) {
-  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= (long long)n * A) return;
-  const int ni = (int)(idx / A), ad = (int)(idx % A);
+// iCEM coloured noise: population element idx = (sequence * H + t) * A + action dim, sample t of its series (one thread
+// per element: the K frequencies of a sample are summed in order, so the split over t changes no bit).  mu / var are read
+// through L2: the fused plan's refit writes them in the same launch.
+__device__ __forceinline__ float icem_noise_element(long long idx, int H, int A, float exponent, const float* mu, const float* var,
+                                                    const float* __restrict__ lb, const float* __restrict__ ub,
+                                                    const float* __restrict__ sr, const float* __restrict__ si,
+                                                    unsigned long long seed, unsigned long long offset) {
+  const int ad = (int)(idx % A), t = (int)((idx / A) % H), ni = (int)(idx / ((long long)A * H));
   const int K = H / 2 + 1;
   // spectrum scale s_k = f_k^(-beta/2), f_0 := f_1 (low-frequency cut-off 1/H); theoretical sigma
   float sig2 = 0.f;
@@ -78,51 +77,58 @@ __global__ void icem_sample_kernel(int n, int H, int A, float exponent, const fl
     sig2 += w * w;
   }
   const float sigma = 2.0f * sqrtf(sig2) / (float)H;
-  for (int t = 0; t < H; ++t) {
-    float acc = 0.f;
-    for (int k = 0; k < K; ++k) {
-      const float s = powf((float)(k == 0 ? 1 : k) / (float)H, -exponent / 2.0f);
-      float zr, zi;
-      if (sr) {
-        zr = sr[((size_t)ni * A + ad) * K + k];
-        zi = si[((size_t)ni * A + ad) * K + k];
-      } else {
-        float g[4];
-        philox_normal4((uint32_t)ni, (uint32_t)(ad * K + k), RNG_STREAM_ICEM, (uint32_t)offset, seed, g);
-        zr = g[0];
-        zi = g[1];
-      }
-      const float re = zr * s;
-      float im = zi * s;
-      const bool nyq = (H % 2 == 0) && (k == K - 1);
-      if (k == 0 || nyq) im = 0.f;
-      const int ph = (int)(((long long)k * t) % H);
-      float sn, cs;
-      sincospif(2.0f * (float)ph / (float)H, &sn, &cs);
-      const float term = re * cs - im * sn;
-      acc += (k == 0 || nyq) ? term : 2.0f * term;
+  float acc = 0.f;
+  for (int k = 0; k < K; ++k) {
+    const float s = powf((float)(k == 0 ? 1 : k) / (float)H, -exponent / 2.0f);
+    float zr, zi;
+    if (sr) {
+      zr = sr[((size_t)ni * A + ad) * K + k];
+      zi = si[((size_t)ni * A + ad) * K + k];
+    } else {
+      float g[4];
+      philox_normal4((uint32_t)ni, (uint32_t)(ad * K + k), RNG_STREAM_ICEM, (uint32_t)offset, seed, g);
+      zr = g[0];
+      zi = g[1];
     }
-    const float y = acc / (float)H / sigma;
-    const int d = t * A + ad;
-    float v = fminf(y * sqrtf(var[d]) + mu[d], ub[d]);
-    v = fmaxf(v, lb[d]);
-    pop[((size_t)ni * H + t) * A + ad] = v;
+    const float re = zr * s;
+    float im = zi * s;
+    const bool nyq = (H % 2 == 0) && (k == K - 1);
+    if (k == 0 || nyq) im = 0.f;
+    const int ph = (int)(((long long)k * t) % H);
+    float sn, cs;
+    sincospif(2.0f * (float)ph / (float)H, &sn, &cs);
+    const float term = re * cs - im * sn;
+    acc += (k == 0 || nyq) ? term : 2.0f * term;
   }
+  const float y = acc / (float)H / sigma;
+  const int d = t * A + ad;
+  const float v = fminf(y * sqrtf(__ldcg(var + d)) + __ldcg(mu + d), ub[d]);
+  return fmaxf(v, lb[d]);
 }
 
-__global__ void icem_append_kernel(int keep, int H, int A, const float* __restrict__ elite,
-                                   const long long* __restrict__ index, int shift, const float* __restrict__ mu,
-                                   const float* __restrict__ var, const float* __restrict__ end_eps,
-                                   unsigned long long seed, unsigned long long offset, float* __restrict__ dst) {
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= keep * H * A) return;
+__global__ void icem_sample_kernel(int n, int H, int A, float exponent, const float* __restrict__ mu,
+                                   const float* __restrict__ var, const float* __restrict__ lb,
+                                   const float* __restrict__ ub, const float* __restrict__ sr,
+                                   const float* __restrict__ si, unsigned long long seed, unsigned long long offset,
+                                   float* __restrict__ pop) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (long long)n * H * A) return;
+  pop[idx] = icem_noise_element(idx, H, A, exponent, mu, var, lb, ub, sr, si, seed, offset);
+}
+
+// element idx of the kept elites appended to a population (trajectory_opt.py:442-466); elite / mu / var are read through
+// L2 for the same reason as in icem_noise_element
+__device__ __forceinline__ float icem_append_element(int idx, int H, int A, const float* elite,
+                                                     const long long* __restrict__ index, int shift, const float* mu,
+                                                     const float* var, const float* __restrict__ end_eps,
+                                                     unsigned long long seed, unsigned long long offset) {
   const int j = idx / (H * A), t = (idx / A) % H, ad = idx % A;
   const long long src = index ? index[j] : j;
   float v;
   if (!shift) {
-    v = elite[(src * H + t) * A + ad];
+    v = __ldcg(elite + (src * H + t) * A + ad);
   } else if (t < H - 1) {
-    v = elite[(src * H + t + 1) * A + ad];
+    v = __ldcg(elite + (src * H + t + 1) * A + ad);
   } else {  // trajectory_opt.py:451-459: fresh last action ~ N(mu[-1], sqrt(var[-1]))
     float e;
     if (end_eps) {
@@ -132,9 +138,18 @@ __global__ void icem_append_kernel(int keep, int H, int A, const float* __restri
       philox_normal4((uint32_t)j, (uint32_t)(ad >> 2), RNG_STREAM_ICEM | 1u, (uint32_t)offset, seed, g);
       e = g[ad & 3];
     }
-    v = mu[(H - 1) * A + ad] + sqrtf(var[(H - 1) * A + ad]) * e;
+    v = __ldcg(mu + (H - 1) * A + ad) + sqrtf(__ldcg(var + (H - 1) * A + ad)) * e;
   }
-  dst[idx] = v;
+  return v;
+}
+
+__global__ void icem_append_kernel(int keep, int H, int A, const float* __restrict__ elite,
+                                   const long long* __restrict__ index, int shift, const float* __restrict__ mu,
+                                   const float* __restrict__ var, const float* __restrict__ end_eps,
+                                   unsigned long long seed, unsigned long long offset, float* __restrict__ dst) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= keep * H * A) return;
+  dst[idx] = icem_append_element(idx, H, A, elite, index, shift, mu, var, end_eps, seed, offset);
 }
 
 __global__ void shift_kernel(int H, int A, int replan, const float* __restrict__ best,
@@ -548,28 +563,33 @@ struct NextPop {
   float* pop_out;
 };
 
+// The refit CTA refits and then publishes `tag` in *flag; every other CTA waits for it.  After this, the refit's outputs
+// are visible to the whole grid and nothing reads the old population any more.
+static __device__ __forceinline__ void refit_then_release(const SelArgs& s, const float* __restrict__ row_totals, int P,
+                                                          bool refit_cta, unsigned int* flag, unsigned int tag) {
+  if (refit_cta) {
+    select_small_body(s, row_totals, P);
+    __syncthreads();  // every read of the old population (elite rows, best row) is done
+    if (threadIdx.x == 0) {
+      __threadfence();
+      asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(flag), "r"(tag) : "memory");
+    }
+  } else {
+    if (threadIdx.x == 0) {
+      unsigned int v;
+      do {
+        asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(flag) : "memory");
+      } while (v != tag);
+    }
+    __syncthreads();
+  }
+}
+
 __global__ void __launch_bounds__(kSelThreads, 1)
 cem_refit_sample_kernel(const SelArgs s, const float* __restrict__ row_totals, int P, const NextPop q) {
   pdl_trigger();
   pdl_wait();
-  if (q.refit) {
-    if (blockIdx.x == 0) {
-      select_small_body(s, row_totals, P);
-      __syncthreads();  // every read of the old population (elite rows, best row) is done
-      if (threadIdx.x == 0) {
-        __threadfence();
-        asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(q.flag), "r"(q.tag) : "memory");
-      }
-    } else {
-      if (threadIdx.x == 0) {
-        unsigned int v;
-        do {
-          asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(q.flag) : "memory");
-        } while (v != q.tag);
-      }
-      __syncthreads();
-    }
-  }
+  if (q.refit) refit_then_release(s, row_totals, P, blockIdx.x == 0, q.flag, q.tag);
   if (!q.sample) return;
   const long long tot = (long long)q.n_pop * s.dims;
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < tot; idx += (long long)gridDim.x * blockDim.x) {
@@ -601,25 +621,8 @@ cem_refit_sample_batch_kernel(const SelArgs s0, const float* __restrict__ row_to
   SelArgs s = s0;
   s.pop += k * rb.pop; s.values += k * rb.values; s.mu += k * rb.dims; s.disp += k * rb.dims;
   s.best_value += k * rb.best; s.best_solution += k * rb.dims; s.elite_idx += k * rb.ws;
-  unsigned int* flag = q0.flag + k * rb.best;
-  if (q0.refit) {
-    if (slice == 0) {
-      select_small_body(s, row_totals ? row_totals + k * rb.rows : nullptr, P);
-      __syncthreads();  // every read of the old population (elite rows, best row) is done
-      if (threadIdx.x == 0) {
-        __threadfence();
-        asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(flag), "r"(q0.tag) : "memory");
-      }
-    } else {
-      if (threadIdx.x == 0) {
-        unsigned int v;
-        do {
-          asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(flag) : "memory");
-        } while (v != q0.tag);
-      }
-      __syncthreads();
-    }
-  }
+  if (q0.refit)
+    refit_then_release(s, row_totals ? row_totals + k * rb.rows : nullptr, P, slice == 0, q0.flag + k * rb.best, q0.tag);
   if (!q0.sample) return;
   const unsigned long long offset = q0.offset + (unsigned long long)k * rb.offset_step;
   const unsigned long long seed = rng_key(rb.seed, offset);
@@ -631,6 +634,45 @@ cem_refit_sample_batch_kernel(const SelArgs s0, const float* __restrict__ row_to
     pop_out[idx] = cem_sample_element(idx, s.dims, __ldcg(s.mu + d), __ldcg(s.disp + d), q0.lb[d], q0.ub[d], z, seed, offset,
                                       q0.clipped, q0.seq0);
   }
+}
+
+// iCEM's refit of iteration i AND the population of iteration i + 1 in one launch (ICEMOptimizer.optimize,
+// trajectory_opt.py:433-486), with the flag protocol of cem_refit_sample_kernel.  The refit is cem_update's with
+// unbiased = 0, use_std = 0 and the elite set written out; the population is n coloured-noise rows (icem_sample_kernel's
+// arithmetic) followed by the extra rows: `keep` kept elites (icem_append_kernel's arithmetic, from `elite`) or one copy
+// of the refitted mu.  refit = 0: sample only (the first population); sample = 0: refit only (the last iteration).
+struct IcemNextPop {
+  int refit, sample;
+  int n, H, A;
+  float exponent;
+  int extra;  // 0: none, 1: kept elites, 2: the mu row
+  int keep, shift;
+  const float* elite;       // [elite_num][H][A] the kept elites' source
+  const long long* index;   // [keep] or NULL (elite j)
+  const float* lb;
+  const float* ub;
+  unsigned long long seed, offset;  // seed keyed with rng_key
+  unsigned int* flag;
+  unsigned int tag;
+  float* pop_out;
+};
+
+__global__ void __launch_bounds__(kSelThreads, 1)
+icem_refit_sample_kernel(const SelArgs s, const float* __restrict__ row_totals, int P, const IcemNextPop q) {
+  pdl_trigger();
+  pdl_wait();
+  if (q.refit) refit_then_release(s, row_totals, P, blockIdx.x == 0, q.flag, q.tag);
+  if (!q.sample) return;
+  const long long stride = (long long)gridDim.x * blockDim.x, first = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const int HA = q.H * q.A;
+  for (long long idx = first; idx < (long long)q.n * HA; idx += stride)
+    q.pop_out[idx] = icem_noise_element(idx, q.H, q.A, q.exponent, s.mu, s.disp, q.lb, q.ub, nullptr, nullptr, q.seed, q.offset);
+  float* extra = q.pop_out + (size_t)q.n * HA;
+  const long long tot = q.extra == 1 ? (long long)q.keep * HA : q.extra == 2 ? HA : 0;
+  for (long long idx = first; idx < tot; idx += stride)
+    extra[idx] = q.extra == 2 ? __ldcg(s.mu + idx)
+                              : icem_append_element((int)idx, q.H, q.A, q.elite, q.index, q.shift, s.mu, s.disp, nullptr,
+                                                    q.seed, q.offset);
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -1164,7 +1206,7 @@ int b200pets_icem_sample(int32_t n, int32_t horizon, int32_t act_dim, float expo
   if (horizon < 2)
     return b200pets_set_error(B200PETS_EINVAL, "icem_sample: coloured noise needs a horizon of at least 2 (a one-step "
                                                "series has no frequency above DC to normalise by)");
-  long long tot = (long long)n * act_dim;
+  long long tot = (long long)n * horizon * act_dim;
   icem_sample_kernel<<<(unsigned)((tot + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
       n, horizon, act_dim, exponent, mu, var, lower, upper, sr, si, rng_key(seed, offset), offset, population_out);
   CUDA_TRY(cudaGetLastError());
@@ -1280,6 +1322,40 @@ int launch_cem_refit_sample(int num_problems, int population, int dims, int elit
   CUDA_TRY(cudaFuncSetAttribute(cem_refit_sample_batch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 150 * 1024));
   CUDA_TRY(launch_pdl(cem_refit_sample_batch_kernel, dim3((unsigned)num_problems * G), dim3(kSelThreads), esm, (cudaStream_t)stream, s,
                       row_totals, particles, q, rb));
+  return B200PETS_OK;
+}
+
+// internal (api.cu, fused iCEM plan): refit of the `rows`-row population of iteration i from its per-row totals (values
+// written to `values`, elites to elites_out) and / or iteration i + 1's population: n coloured-noise rows drawn with
+// Philox key `seed` (unkeyed) at `offset`, then the extra rows (icem_refit_sample_kernel).  The caller stays within
+// cem_refit_sample_supported for the largest population; workspace is cem_update's.
+int launch_icem_refit_sample(int rows, int dims, int elite_num, float alpha, const float* row_totals, int particles, float* values,
+                             float* mu, float* var, float* best_value, float* best_solution, float* elites_out, void* workspace,
+                             size_t workspace_bytes, int refit, int sample, int n, int horizon, int act_dim, float exponent,
+                             int extra, int keep, int shift, const float* elite, const int64_t* index, const float* lb,
+                             const float* ub, unsigned long long seed, unsigned long long offset, unsigned int tag, float* pop,
+                             cudaStream_t stream) {
+  const int k = elite_num;
+  if (!(rows <= kSmallN && (size_t)k * dims * sizeof(float) <= 150 * 1024)) return B200PETS_EUNSUPPORTED;
+  if (workspace_bytes < b200pets_cem_update_workspace_bytes(rows, dims, k))
+    return b200pets_set_error(B200PETS_EINVAL, "icem_plan: refit workspace too small");
+  SelArgs s{};
+  s.n = rows; s.dims = dims; s.k = k; s.alpha = alpha; s.unbiased = 0; s.use_std = 0; s.mode = 0;
+  s.pop = pop; s.pstride = dims; s.values = values; s.vstride = 1; s.mu = mu; s.disp = var;
+  s.best_value = best_value; s.best_solution = best_solution; s.elites_out = elites_out;
+  s.partial = reinterpret_cast<float*>(workspace);
+  s.elite_idx = reinterpret_cast<int*>(reinterpret_cast<float*>(workspace) + 33 * (size_t)dims);
+  IcemNextPop q{};
+  q.refit = refit; q.sample = sample; q.n = n; q.H = horizon; q.A = act_dim; q.exponent = exponent;
+  q.extra = extra; q.keep = keep; q.shift = shift; q.elite = elite; q.index = reinterpret_cast<const long long*>(index);
+  q.lb = lb; q.ub = ub; q.seed = rng_key(seed, offset); q.offset = offset;
+  q.flag = reinterpret_cast<unsigned int*>(best_value + 2); q.tag = tag; q.pop_out = pop;
+  const long long work = (long long)(n + max(keep, 1)) * dims;
+  unsigned G = sample ? (unsigned)min((long long)64, (work + kSelThreads - 1) / kSelThreads) : 1u;
+  if (G < 1) G = 1;
+  CUDA_TRY(cudaFuncSetAttribute(icem_refit_sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 150 * 1024));
+  CUDA_TRY(launch_pdl(icem_refit_sample_kernel, dim3(G), dim3(kSelThreads), (size_t)k * dims * sizeof(float), stream, s, row_totals,
+                      particles, q));
   return B200PETS_OK;
 }
 

@@ -15,6 +15,8 @@
   ``b200pets_latent_cem_plan_batch`` call; iCEM and MPPI evaluate through its ``evaluate_action_sequences``.  For K
   observations the environment's K posteriors plan as one ``b200pets_latent_cem_plan_batch`` call, and MPPI plans
   entry k from posterior k.
+* ``ICEMOptimizer`` over that closure (no callback, no callable the kernels do not know) runs the whole optimisation as
+  one C call too (``b200pets_icem_plan``), with the per-iteration loop's draws, counters, elites and result.
 * ``TrajectoryOptimizer`` / ``TrajectoryOptimizerAgent`` / ``create_trajectory_optim_agent_for_model``:
   reference semantics (warm-start shift, action cache, RuntimeError when the eval fn is unset).
 """
@@ -285,6 +287,9 @@ class ICEMOptimizer(Optimizer):
             self.keep_elite_size = self._round_up_to_module(self.keep_elite_size, self.population_size_module)
         self.lib = _lib.load()
         self._seed = int(torch.initial_seed()) & 0xFFFFFFFFFFFFFFFF
+        self._plan_ws = None
+        self.record_values = False
+        self.last_values: Optional[List[torch.Tensor]] = None
 
     @staticmethod
     def _round_up_to_module(value: int, module: int) -> int:
@@ -300,11 +305,20 @@ class ICEMOptimizer(Optimizer):
         return sizes
 
     def optimize(self, obj_fun, x0: Optional[torch.Tensor] = None, callback=None, *, _noise=None, **kwargs) -> torch.Tensor:
+        """trajectory_opt.py:391-487.  Over the model's objective (a non-latent ModelEnv without reward / termination
+        callables), with no callback and no injected noise, the whole optimisation is one device-resident call
+        (``b200pets_icem_plan``) that leaves the result, the elites, the counters and the torch generator exactly as the
+        per-iteration loop below would.  With ``record_values`` ``last_values`` holds each iteration's values."""
         H, A = x0.shape
         if H < 2:  # b200pets_icem_sample refuses it too; checked here before anything is launched
             raise ValueError(f"ICEMOptimizer needs a planning horizon of at least 2, got {H}: coloured noise over a "
                              "one-step series has no frequency above DC to normalise by")
         x0 = x0.to(self.device, torch.float32).contiguous()
+        # the fused plan cannot call back into Python: callbacks, injected noise and callables keep the loop
+        if (isinstance(obj_fun, _FusedObjective) and callback is None and _noise is None and self.num_iterations >= 1
+                and not getattr(obj_fun.model_env, "is_latent", False) and not obj_fun.model_env.has_external_callables()):
+            return self._optimize_fused(obj_fun, x0)
+        self.last_values = [] if self.record_values else None
         dims = H * A
         dev = self.device
         mu = x0.reshape(-1).clone()
@@ -355,8 +369,74 @@ class ICEMOptimizer(Optimizer):
                     _lib.ptr(var), _lib.ptr(best_val), _lib.ptr(best_sol), None, _lib.ptr(elites_new), _lib.ptr(ws), nbytes,
                     stream), "cem_update")
                 self.elite = elites_new.clone()
+                if self.last_values is not None:
+                    self.last_values.append(values)
         out = mu if self.return_mean_elites else best_sol
         return out.view(H, A).clone()
+
+    def _fused_draws(self, env, prop: str, horizon: int, num_particles: int, sizes: Optional[List[int]] = None):
+        """The torch generator draws of one :meth:`optimize` over the model, in the loop's order: per iteration the
+        permutation of the kept elites (whenever elites are kept) and then that evaluation's permutations
+        (``ModelEnv._eval_perms``).  Returns each iteration's evaluated population, the kept elites' indices
+        ``[iterations, keep]`` (None when no iteration keeps any) and each evaluation's permutations (None: members
+        drawn in the kernel)."""
+        keep = min(self.keep_elite_size, self.elite_num)
+        last = self.num_iterations - 1
+        rows, index, perms = [], [], []
+        for i, n in enumerate(self.population_sizes() if sizes is None else sizes):
+            extra, idx = 0, None
+            if self.elite is not None or i > 0:
+                if i == last and i != 0:
+                    extra = 1  # the current mean
+                else:
+                    extra = keep
+                    idx = torch.randperm(self.elite_num, device=self.device)[:keep]
+            rows.append(n + extra)
+            index.append(idx)
+            perms.append(env._eval_perms(prop, n + extra, horizon, num_particles))
+        drawn = [t for t in index if t is not None]
+        if keep == 0 or not drawn:
+            return rows, None, perms
+        # the rows of iterations that keep no elites are not read
+        return rows, torch.stack([drawn[0] if t is None else t for t in index]).to(torch.int64).contiguous(), perms
+
+    def _optimize_fused(self, obj: _FusedObjective, x0: torch.Tensor) -> torch.Tensor:
+        env = obj.model_env
+        obs = np.asarray(obj.obs)
+        if obs.ndim != 1:
+            raise NotImplementedError("pixel observations are outside the GaussianMLP hot path")
+        env._fresh()
+        H, A = x0.shape
+        P, iters = obj.num_particles, self.num_iterations
+        prop = env._propagation()
+        sizes = self.population_sizes()
+        rows, keep_index, perms = self._fused_draws(env, prop, H, P, sizes)
+        # iteration i evaluates with the environment's counter first + i, as the loop's i-th evaluation does
+        rcfg = _lib.RolloutCfg(0, H, P, _lib.PREC[env.precision_for(prop)], _lib.PROP[prop],
+                               _lib.TS1_PERMS if env.ts1 == "perms" else _lib.TS1_TILE_SHUFFLE, env._seed, env._offset + 1)
+        env._offset += iters
+        icfg = _lib.IcemCfg(iters, self.elite_num, min(self.keep_elite_size, self.elite_num), float(self.alpha),
+                            float(self.colored_noise_exponent), int(self.return_mean_elites), self._seed,
+                            _next_seed_offset(self))
+        sizes = (C.c_int32 * iters)(*sizes)
+        need = self.lib.b200pets_icem_plan_workspace_bytes(env.staged.handle, C.byref(rcfg), C.byref(icfg), sizes)
+        if self._plan_ws is None or self._plan_ws.numel() < need:
+            self._plan_ws = torch.empty(max(need, 1), dtype=torch.uint8, device=self.device)
+        perms = [None if p is None else p.to(torch.int64).contiguous() for p in perms]
+        perm_ptrs = (C.c_void_p * iters)(*[None if p is None else p.data_ptr() for p in perms])
+        obs0 = env._obs_to_device(obs)
+        sol = torch.empty(H, A, device=self.device)
+        elite = torch.empty(self.elite_num, H, A, device=self.device)
+        values = torch.empty(sum(rows), device=self.device) if self.record_values else None
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.b200pets_icem_plan(
+                env.staged.handle, C.byref(rcfg), C.byref(icfg), sizes, _lib.ptr(obs0), _lib.ptr(x0), _lib.ptr(self.lower_bound),
+                _lib.ptr(self.upper_bound), _lib.ptr(self.elite), _lib.ptr(keep_index), perm_ptrs, _lib.ptr(sol),
+                _lib.ptr(elite), _lib.ptr(values), _lib.ptr(self._plan_ws), self._plan_ws.numel(), _lib.stream_ptr()),
+                "icem_plan")
+        self.elite = elite
+        self.last_values = None if values is None else list(values.split(rows))
+        return sol
 
 
 
