@@ -142,11 +142,19 @@ __device__ __forceinline__ void philox_normal4(uint32_t c0, uint32_t c1, uint32_
 }
 
 // RNG stream tags (third counter word, high bits)
+// rollout_f32.cu / rollout_tc.cu, the Gaussian output noise of column o (the learned-reward column o = out - 1 included)
+// of row r at step t: philox_normal4(r, t, RNG_STREAM_EPS | (o >> 2), low word of off, rng_key(seed, off)), lane o & 3 (r: the
+// global row (seq0 + n) * P + p, under an explicit permutation the row perm[slot] holds, not the slot; t: the step of the
+// evaluation, 0 for b200pets_step, whose rows are r with P = 1; off: the call's offset, offset + k * offset_step for
+// problem k of a batched launch).  Under expectation each (row, t, o) draws once, after the member passes.
 #define RNG_STREAM_EPS 0x10000u
+// shuffle_member below, the member of tile-shuffle group gt at step t: (x * M) >> 32, a position in the elite list, with
+// x word 0 of philox4x32_10(gt, t, RNG_STREAM_MEMBER, low word of off, low word of s, high word of s ^ high word of gt),
+// s = rng_key(seed, off) (gt = p * C_glob + global sequence / 128, see "tile shuffle" below; t = 0 when the member is
+// drawn once per group (fixed_model); b200pets_step has gt = row / 128)
 #define RNG_STREAM_MEMBER 0x20000u
 #define RNG_STREAM_CEM 0x30000u
 #define RNG_STREAM_ICEM 0x40000u
-#define RNG_STREAM_PERM 0x50000u
 // latent.cu, the prior's draw of latent element j of row r at step t: philox_normal4(r, t, RNG_STREAM_LATENT | (j >> 2),
 // offset, rng_key(seed, offset)), lane j & 3 (r: row of the call, n * P + p; t: step of the call, 0 for one step)
 #define RNG_STREAM_LATENT 0x60000u

@@ -115,20 +115,29 @@ def check_rows(N, P, M, perm=None):
     return np.array(sorted(s))
 
 
-def _rel(got, ref):
+def _rel(got, ref, allow=0.0):
     got = np.asarray(got, np.float64).reshape(ref.shape[0], -1)
+    allow = np.reshape(allow, (ref.shape[0], -1)) if np.ndim(allow) else allow
     ref = ref.reshape(ref.shape[0], -1)
-    return (np.abs(got - ref) / np.maximum(1.0, np.abs(ref))).max(axis=1)
+    return (np.maximum(np.abs(got - ref) - allow, 0.0) / np.maximum(1.0, np.abs(ref))).max(axis=1)
 
 
-def compare_step(spec, ck, obs, act, members, eps, nobs, rew, done, bf16, sample=True):
+def compare_step(spec, ck, obs, act, members, eps, nobs, rew, done, bf16, sample=True, slack=None):
     """Worst relative error of next_obs and reward of these rows, the number of done flags that differ, and every row's
-    worst error ("rows")."""
+    worst error ("rows").  `slack` [rows, out] (in-kernel draws): how far each draw may be off; an element may then
+    differ from the reference by that times its sd beyond the bar (the checker's output moved by `slack` in place of
+    the draws, less its output at zero draws)."""
     ref_obs, ref_rew = ck.step(obs, act, members, eps, sample=sample, bf16=bf16)
+    a_obs = a_rew = 0.0
+    if slack is not None:
+        hi_obs, hi_rew = ck.step(obs, act, members, slack, sample=sample, bf16=bf16)
+        lo_obs, lo_rew = ck.step(obs, act, members, np.zeros_like(slack), sample=sample, bf16=bf16)
+        a_obs = np.abs(hi_obs - lo_obs)
+        a_rew = 0.0 if hi_rew is None else np.abs(hi_rew - lo_rew)
     if spec.reward_fn is not None:  # a known function on the kernel's own next_obs (it wins over a learned column)
-        ref_rew = known_reward(spec.reward_fn, act, nobs)
+        ref_rew, a_rew = known_reward(spec.reward_fn, act, nobs), 0.0
     bad_done = int((known_done(spec.term_fn, act, nobs) != done.astype(bool)).sum())
-    e_obs, e_rew = _rel(nobs, ref_obs), _rel(rew, ref_rew)
+    e_obs, e_rew = _rel(nobs, ref_obs, a_obs), _rel(rew, ref_rew, a_rew)
     return {"next_obs": float(e_obs.max()), "reward": float(e_rew.max()), "done": bad_done,
             "rows": np.maximum(e_obs, e_rew)}
 
@@ -143,10 +152,12 @@ def _worst(acc, err):
 
 
 # ---- trajectories --------------------------------------------------------------------------------------------------
-def run_trajectory(env, spec, inp, mode, windows, offset=SHUFFLE_OFFSET):
+def run_trajectory(env, spec, inp, mode, windows, offset=SHUFFLE_OFFSET, inject_eps=True, shard=(0, 0)):
     """b200pets_eval_trajectory over [0, H) as one window ("one") or H single-step windows ("steps").  Returns next_obs
     [H, B, D], reward [H, B], done [H, B], the row -> member map [H, B] (None for expectation) and a closure that runs
-    b200pets_eval_sequences with the same configuration and draws (per-row totals)."""
+    b200pets_eval_sequences with the same configuration and draws (per-row totals).  With `inject_eps` False the
+    kernels draw their own noise (a NULL eps); `shard` is (first sequence, global population) of a sharded evaluation
+    whose population is spec.population."""
     from mbrl_lib_b200 import _lib
 
     lib, h = env.lib, env.staged.handle
@@ -154,11 +165,11 @@ def run_trajectory(env, spec, inp, mode, windows, offset=SHUFFLE_OFFSET):
     B = N * P
     prop = spec.propagation
     perms = torch.from_numpy(inp["perms"]).to(DEV) if mode == "perms" else None
-    eps = None if spec.deterministic else torch.from_numpy(inp["eps"]).to(DEV)
+    eps = None if spec.deterministic or not inject_eps else torch.from_numpy(inp["eps"]).to(DEV)
     acts = torch.from_numpy(inp["actions"]).to(DEV)
     obs0 = torch.from_numpy(np.asarray(inp["obs0"], np.float32)).to(DEV)
     cfg = _lib.RolloutCfg(N, H, P, _lib.PREC[env.precision], _lib.PROP[prop],
-                          _lib.TS1_PERMS if perms is not None else _lib.TS1_TILE_SHUFFLE, env._seed, offset, 0, 0)
+                          _lib.TS1_PERMS if perms is not None else _lib.TS1_TILE_SHUFFLE, env._seed, offset, *shard)
     ws = torch.empty(lib.b200pets_trajectory_workspace_bytes(h, C.byref(cfg)), dtype=torch.uint8, device=DEV)
     nobs = torch.full((H, B, D), float("nan"), device=DEV)
     rew = torch.full((H, B), float("nan"), device=DEV)
@@ -173,7 +184,7 @@ def run_trajectory(env, spec, inp, mode, windows, offset=SHUFFLE_OFFSET):
     if mode == "perms":
         assign = np.stack([assignment_from_perm(inp["perms"][min(t, inp["perms"].shape[0] - 1)], M) for t in range(H)])
     elif mode == "shuffle":
-        assign = env.shuffle_member_assignment(N, H, P, offset).numpy()
+        assign = env.shuffle_member_assignment(N, H, P, offset, *shard).numpy()
     else:
         assign = None
 
@@ -191,8 +202,9 @@ def run_trajectory(env, spec, inp, mode, windows, offset=SHUFFLE_OFFSET):
     return nobs.cpu().numpy(), rew.cpu().numpy(), done.cpu().numpy(), assign, eval_rows
 
 
-def check_trajectory(spec, ck, inp, nobs, rew, done, assign, bf16, mode, eps=None):
-    """Teacher-forced comparison of every step: worst errors over steps and checked rows."""
+def check_trajectory(spec, ck, inp, nobs, rew, done, assign, bf16, mode, eps=None, slack=None):
+    """Teacher-forced comparison of every step: worst errors over steps and checked rows (`slack` [H, B, out]: see
+    compare_step)."""
     N, H, P, M = spec.population, spec.horizon, spec.particles, spec.num_models
     B = N * P
     eps = inp.get("eps") if eps is None else eps
@@ -205,7 +217,8 @@ def check_trajectory(spec, ck, inp, nobs, rew, done, assign, bf16, mode, eps=Non
         act = inp["actions"][rows // P, t]
         e = None if spec.deterministic else eps[t, rows]
         mem = None if assign is None else assign[t, rows]
-        _worst(acc, compare_step(spec, ck, obs, act, mem, e, nobs[t, rows], rew[t, rows], done[t, rows], bf16))
+        s = None if slack is None or spec.deterministic else slack[t, rows]
+        _worst(acc, compare_step(spec, ck, obs, act, mem, e, nobs[t, rows], rew[t, rows], done[t, rows], bf16, slack=s))
     assert np.isfinite(nobs).all() and np.isfinite(rew).all() and (done <= 1).all()
     return acc
 
