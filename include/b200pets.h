@@ -98,7 +98,22 @@ typedef struct {
   int32_t reward_fn;       /* B200PETS_REWARD_* */
   int32_t term_fn;         /* B200PETS_TERM_* */
   int32_t norm_mode;       /* 0 none, 1 fp32 stats, 2 fp64 stats (util/math.py:95-143) */
+  /* How the `perms` argument of the entry points that take one picks a row's member:
+   *   B200PETS_MEMBER_PERM (0): a permutation of the rows; member m owns slots [m*B/M, (m+1)*B/M)
+   *     (GaussianMLP, gaussian_mlp.py:202-212)
+   *   B200PETS_MEMBER_ROWS (1): per-row member indices in [0, M) (BasicEnsemble, basic_ensemble.py:103-126, 255-260),
+   *     any number of rows per member and B need not be a multiple of M.  perms keeps each entry point's shape
+   *     ([H][B] for random_model, [1][B] for fixed_model) and position in its argument list; it is required for those two
+   *     propagation methods (NULL: B200PETS_EINVAL), the tile shuffle never applies, and sharded configurations return
+   *     B200PETS_EUNSUPPORTED.  Rows are bucketed by member on the device (b200pets_member_slots) once per step of
+   *     random_model and once per evaluation of fixed_model; a row whose index is outside [0, M) is not evaluated and
+   *     its outputs (next observation, reward, reward total) are NaN and its done flags 0.  Both rollout kernels run it:
+   *     each member's rows form its own tiles. */
+  int32_t member_rule;
 } b200pets_model_desc;
+
+#define B200PETS_MEMBER_PERM 0
+#define B200PETS_MEMBER_ROWS 1
 
 int b200pets_version(void);
 const char* b200pets_last_error(void);
@@ -191,6 +206,14 @@ int b200pets_trajectory_returns(const b200pets_rollout_cfg* cfg, int32_t t0, int
 int64_t b200pets_shuffle_num_groups(const b200pets_rollout_cfg* cfg);
 int b200pets_shuffle_member_map(const b200pets_rollout_cfg* cfg, int32_t num_members, int32_t* members_out,
                                 void* stream);
+
+/* The member bucketing of B200PETS_MEMBER_ROWS models, as the rollouts run it: for each of num_problems problems,
+ * indices [dev] int64[num_problems][batch] -> slots_out [dev] int64[num_problems][batch], the rows grouped by member in
+ * member order and in row order within a member (rows whose index is outside [0, num_members) last), and offsets_out
+ * [dev] int32[num_problems][num_members + 1]: member m's rows are slots [offsets[m], offsets[m+1]), offsets[0] = 0 and
+ * offsets[num_members] = the number of in-range rows. */
+int b200pets_member_slots(int32_t num_problems, int64_t batch, int32_t num_members, const int64_t* indices,
+                          int64_t* slots_out, int32_t* offsets_out, void* stream);
 
 /* ModelEnv.step (mbrl/models/model_env.py:87-140) for a batch of B independent states.
  *   perm [dev] int64[B]; NULL is allowed for TS1 (tile shuffle) and expectation; TSinf requires the caller's

@@ -10,7 +10,7 @@ _LAZY = {
     "Agent": "planning", "Optimizer": "planning", "CEMOptimizer": "planning", "ICEMOptimizer": "planning", "MPPIOptimizer": "planning",
     "TrajectoryOptimizer": "planning", "TrajectoryOptimizerAgent": "planning",
     "create_trajectory_optim_agent_for_model": "planning", "complete_agent_cfg": "planning", "rollout_model_env": "planning",
-    "GaussianMLP": "models", "OneDTransitionRewardModel": "models", "EnsembleLinearLayer": "models",
+    "GaussianMLP": "models", "OneDTransitionRewardModel": "models", "EnsembleLinearLayer": "models", "BasicEnsemble": "models",
     "Normalizer": "models", "model_from_arrays": "models", "PlaNetModel": "models", "ModelTrainer": "trainer",
     "TransitionBatch": "replay", "TransitionIterator": "replay", "BootstrapIterator": "replay", "SAC": "sac",
 }

@@ -19,6 +19,7 @@ REWARD = {None: 0, "learned": 0, "cartpole": 1, "cartpole_pets": 2, "inverted_pe
 TERM = {"no_termination": 0, "cartpole": 1, "inverted_pendulum": 2, "hopper": 3, "walker2d": 4, "ant": 5,
         "humanoid": 6, "external": 255}
 PROP = {"random_model": 0, "fixed_model": 1, "expectation": 2}
+MEMBER_RULE = {"perm": 0, "rows": 1}  # how `perms` picks a row's member: GaussianMLP's permutation, BasicEnsemble's per-row index
 PREC = {"f32": 0, "bf16_tc": 1}
 DTYPE = {"float32": 0, "float64": 1, "uint8": 2}
 TS1_PERMS, TS1_TILE_SHUFFLE = 0, 1
@@ -28,7 +29,7 @@ class ModelDesc(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("ensemble_size", "num_members", "obs_dim", "act_dim", "in_size", "out_size",
                                          "hid_size", "num_hidden", "activation")] + [("leaky_slope", C.c_float)] + \
                [(n, C.c_int32) for n in ("obs_process", "learned_rewards", "target_is_delta", "deterministic",
-                                         "reward_fn", "term_fn", "norm_mode")]
+                                         "reward_fn", "term_fn", "norm_mode", "member_rule")]
 
 
 class RolloutCfg(C.Structure):
@@ -137,6 +138,7 @@ _SIGNATURES = {
                                             _P, _P]),
     "b200pets_shuffle_num_groups": (C.c_int64, [C.POINTER(RolloutCfg)]),
     "b200pets_shuffle_member_map": (C.c_int, [C.POINTER(RolloutCfg), C.c_int32, _P, _P]),
+    "b200pets_member_slots": (C.c_int, [C.c_int32, C.c_int64, C.c_int32, _P, _P, _P, _P]),
     "b200pets_cem_update_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32]),
     "b200pets_cem_update": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_int32, C.c_int32, _P, _P, _P, _P,
                                       _P, _P, _P, _P, _P, C.c_size_t, _P]),

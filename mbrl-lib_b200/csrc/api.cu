@@ -69,9 +69,113 @@ struct b200pets_model_s {
   size_t off_W[B200PETS_MAX_LAYERS], off_b[B200PETS_MAX_LAYERS];
   size_t off_members, off_norm_d, off_norm_f, off_lv, off_nodelta, off_img;
   bool tc_ok = false;
+  // b200pets_step's member bucketing space (per-row member models): b200pets_step has no workspace argument
+  void* step_bucket = nullptr;
+  size_t step_bucket_bytes = 0;
 };
 
 static inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
+
+// ---------------------------------------------------------------------------------------------------------
+// member bucketing of per-row member models (B200PETS_MEMBER_ROWS)
+// ---------------------------------------------------------------------------------------------------------
+constexpr int kMaxBucketMembers = 256;  // bounds the bucketing kernel's shared counters
+constexpr int kBucketThreads = 1024;
+
+namespace {
+// One CTA per problem: a stable counting sort of the rows by member index.  Bucket M holds the rows whose index is
+// outside [0, M) (never evaluated).  Pass 1 counts, pass 2 scatters blockDim rows at a time: a row's slot is its
+// bucket's cursor, plus the rows of its bucket in lower warps of the chunk, plus those in lower lanes of its warp.
+__global__ void __launch_bounds__(kBucketThreads) member_slots_kernel(long long B, int M, const long long* __restrict__ idx,
+                                                                      long long idx_stride, long long* __restrict__ slots,
+                                                                      int* __restrict__ offs) {
+  extern __shared__ int sh[];
+  const int MB = M + 1;
+  int* cursor = sh;     // [MB]
+  int* cnt = sh + MB;   // [warps][MB]
+  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5, nw = blockDim.x >> 5;
+  const long long k = blockIdx.x;
+  idx += k * idx_stride;
+  slots += k * B;
+  offs += k * MB;
+  auto bucket = [&](long long v) { return (v >= 0 && v < M) ? (int)v : M; };
+  for (int j = tid; j < MB; j += blockDim.x) cursor[j] = 0;
+  __syncthreads();
+  for (long long r = tid; r < B; r += blockDim.x) atomicAdd(&cursor[bucket(idx[r])], 1);
+  __syncthreads();
+  if (tid == 0) {
+    int s = 0;
+    for (int j = 0; j < MB; ++j) {
+      const int c = cursor[j];
+      cursor[j] = s;
+      s += c;
+    }
+  }
+  __syncthreads();
+  for (int j = tid; j < MB; j += blockDim.x) offs[j] = cursor[j];  // offs[M]: start of the out-of-range rows
+  for (long long base = 0; base < B; base += blockDim.x) {
+    const long long r = base + tid;
+    const bool in = r < B;
+    const int b = in ? bucket(idx[r]) : -1;
+    const unsigned peers = __match_any_sync(0xffffffffu, b);
+    const int rank = __popc(peers & ((1u << lane) - 1u));
+    for (int j = tid; j < nw * MB; j += blockDim.x) cnt[j] = 0;
+    __syncthreads();
+    if (in && rank == 0) cnt[w * MB + b] = __popc(peers);
+    __syncthreads();
+    for (int j = tid; j < MB; j += blockDim.x) {
+      int s = cursor[j];
+      for (int ww = 0; ww < nw; ++ww) {
+        const int c = cnt[ww * MB + j];
+        cnt[ww * MB + j] = s;
+        s += c;
+      }
+      cursor[j] = s;
+    }
+    __syncthreads();
+    if (in) slots[cnt[w * MB + b] + rank] = r;
+    __syncthreads();
+  }
+}
+
+// The outputs of the rows a bucketing left out (slots [offs[M], B) of each problem) are NaN, their done flags 0.
+__global__ void member_nan_rows_kernel(long long B, int M, const long long* __restrict__ slots, const int* __restrict__ offs,
+                                       int D, int T, float* obs, long long obs_stride, float* total, float* reward,
+                                       uint8_t* done, long long rows_stride, float* traj_obs, float* traj_reward,
+                                       uint8_t* traj_done) {
+  const long long k = blockIdx.y;
+  const long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= B || s < offs[k * (M + 1) + M]) return;
+  const long long r = slots[k * B + s];
+  const float nan = __int_as_float(0x7fc00000);
+  if (obs)
+    for (int d = 0; d < D; ++d) obs[k * obs_stride + r * D + d] = nan;
+  if (total) total[k * rows_stride + r] = nan;
+  if (reward) reward[r] = nan;
+  if (done) done[r] = 0;
+  for (int t = 0; t < T; ++t) {
+    if (traj_obs)
+      for (int d = 0; d < D; ++d) traj_obs[((size_t)t * B + r) * D + d] = nan;
+    if (traj_reward) traj_reward[(size_t)t * B + r] = nan;
+    if (traj_done) traj_done[(size_t)t * B + r] = 0;
+  }
+}
+}  // namespace
+
+static int launch_member_slots(int K, long long B, int M, const int64_t* idx, long long idx_stride, long long* slots, int* offs,
+                               cudaStream_t stream) {
+  const size_t smem = sizeof(int) * (size_t)(M + 1) * (1 + kBucketThreads / 32);  // <= 48 KB for M <= kMaxBucketMembers
+  member_slots_kernel<<<(unsigned)K, kBucketThreads, smem, stream>>>(B, M, reinterpret_cast<const long long*>(idx), idx_stride,
+                                                                     slots, offs);
+  CUDA_TRY(cudaGetLastError());
+  return B200PETS_OK;
+}
+
+// device bytes of the bucketing of K problems of B rows: slots [K][B] int64, offsets [K][M+1] int32
+static size_t bucket_bytes(const b200pets_model_s* mdl, size_t K, size_t B) {
+  if (mdl->desc.member_rule != B200PETS_MEMBER_ROWS) return 0;
+  return ((K * B * sizeof(long long) + 255) & ~(size_t)255) + ((K * (mdl->desc.num_members + 1) * sizeof(int) + 255) & ~(size_t)255);
+}
 
 namespace {
 
@@ -219,6 +323,11 @@ int b200pets_model_create(const b200pets_model_desc* desc, const float* const* w
     return b200pets_set_error(B200PETS_EINVAL, "model_create: out_size %d inconsistent with obs_dim %d / learned_rewards %d", d.out_size, d.obs_dim, d.learned_rewards);
   if (!d.learned_rewards && d.reward_fn == B200PETS_REWARD_LEARNED)
     return b200pets_set_error(B200PETS_EINVAL, "model_create: reward_fn required when rewards are not learned");
+  if (d.member_rule != B200PETS_MEMBER_PERM && d.member_rule != B200PETS_MEMBER_ROWS)
+    return b200pets_set_error(B200PETS_EINVAL, "model_create: unknown member_rule %d", d.member_rule);
+  if (d.member_rule == B200PETS_MEMBER_ROWS && d.num_members > kMaxBucketMembers)
+    return b200pets_set_error(B200PETS_EUNSUPPORTED, "model_create: per-row members bucket at most %d members (got %d)",
+                              kMaxBucketMembers, d.num_members);
 
   b200pets_model_s* mdl = new b200pets_model_s();
   mdl->desc = d;
@@ -296,6 +405,7 @@ int b200pets_model_refresh(b200pets_model_t model, const float* const* weights, 
 
 void b200pets_model_destroy(b200pets_model_t model) {
   if (!model) return;
+  cudaFree(model->step_bucket);
   cudaFree(model->blob);
   delete model;
 }
@@ -348,11 +458,38 @@ static int dispatch(const b200pets_model_s* mdl, int precision, const RolloutArg
 
 static size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 
-// evaluation workspace: observations [K][B][D], reward totals [K][B], dead flags [K][B]
+// A launch of a per-row member model (B200PETS_MEMBER_ROWS): bucket the K problems' member indices idx (problem k at
+// idx + k * bt.perm) into `bucket` (bucket_bytes), run the launch `a` over the members' slot ranges, then set the outputs
+// of rows with an out-of-range index to NaN.
+static int dispatch_member_rows(const b200pets_model_s* mdl, int precision, RolloutArgs a, const int64_t* idx, int K,
+                                BatchArgs bt, void* bucket, cudaStream_t stream) {
+  const int M = mdl->desc.num_members;
+  const long long B = a.B;
+  long long* slots = reinterpret_cast<long long*>(bucket);
+  int* offs = reinterpret_cast<int*>(reinterpret_cast<unsigned char*>(bucket) + al256((size_t)K * B * sizeof(long long)));
+  int rc = launch_member_slots(K, B, M, idx, bt.perm, slots, offs, stream);
+  if (rc) return rc;
+  a.slot_mode = 0;
+  a.perm = slots;
+  a.member_off = offs;
+  bt.perm = B;
+  bt.member_off = M + 1;
+  rc = dispatch(mdl, precision, a, K, bt, stream);
+  if (rc) return rc;
+  member_nan_rows_kernel<<<dim3((unsigned)((B + 255) / 256), (unsigned)K), 256, 0, stream>>>(
+      B, M, slots, offs, mdl->desc.obs_dim, a.t1 - a.t0, a.obs_out, bt.obs_state, a.total_state, a.reward_out, a.done_out,
+      bt.rows, a.traj_obs, a.traj_reward, a.traj_done);
+  CUDA_TRY(cudaGetLastError());
+  return B200PETS_OK;
+}
+
+// evaluation workspace: observations [K][B][D], reward totals [K][B], dead flags [K][B], then the member bucketing of
+// per-row member models (bucket_bytes)
 size_t b200pets_eval_batch_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* cfg, int32_t num_problems) {
   if (!model || !cfg || num_problems < 1) return 0;
   const size_t KB = (size_t)num_problems * cfg->population * cfg->particles;
-  return al256(KB * model->desc.obs_dim * sizeof(float)) + al256(KB * sizeof(float)) + al256(KB);
+  return al256(KB * model->desc.obs_dim * sizeof(float)) + al256(KB * sizeof(float)) + al256(KB) +
+         bucket_bytes(model, num_problems, (size_t)cfg->population * cfg->particles);
 }
 
 size_t b200pets_eval_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* cfg) {
@@ -365,7 +502,7 @@ static int check_eval(b200pets_model_t model, const b200pets_rollout_cfg* cfg, c
   const int N = cfg->population, H = cfg->horizon, P = cfg->particles;
   if (N <= 0 || H <= 0 || P <= 0) return b200pets_set_error(B200PETS_EINVAL, "%s: population, horizon, particles must be positive", what);
   const long long B = (long long)N * P;
-  if (B % d.num_members != 0)  // mbrl/models/gaussian_mlp.py:195-200
+  if (d.member_rule == B200PETS_MEMBER_PERM && B % d.num_members != 0)  // mbrl/models/gaussian_mlp.py:195-200
     return b200pets_set_error(B200PETS_EINVAL, "GaussianMLP ensemble requires batch size to be a multiple of the number of models. "
                                                "Current batch size is %lld for %d models.", B, d.num_members);
   return B200PETS_OK;
@@ -388,7 +525,7 @@ static int check_no_external(b200pets_model_t model) {
 static int rollout_steps(b200pets_model_t model, const b200pets_rollout_cfg* cfg, int t0, int t1, bool keep_obs,
                          const float* obs0, const float* actions, const int64_t* perms, const float* eps, float* obs_state,
                          float* total, uint8_t* dead, float* traj_obs, float* traj_reward, uint8_t* traj_done,
-                         cudaStream_t stream, int num_problems = 1, const BatchArgs& bt = BatchArgs{}) {
+                         void* bucket, cudaStream_t stream, int num_problems = 1, const BatchArgs& bt = BatchArgs{}) {
   const b200pets_model_desc& d = model->desc;
   const int N = cfg->population, H = cfg->horizon, P = cfg->particles;
   const long long B = (long long)N * P;
@@ -404,6 +541,12 @@ static int rollout_steps(b200pets_model_t model, const b200pets_rollout_cfg* cfg
   int precision = cfg->precision;
 
   const bool ts1 = cfg->propagation == B200PETS_PROP_RANDOM_MODEL;
+  // per-row members: the caller's indices, bucketed per step (random_model) or once (fixed_model)
+  const bool rows = d.member_rule == B200PETS_MEMBER_ROWS && cfg->propagation != B200PETS_PROP_EXPECTATION;
+  if (rows && !perms)
+    return b200pets_set_error(B200PETS_EINVAL, "per-row member models need the member indices of random_model / fixed_model");
+  if (rows && (a.seq0 != 0 || a.n_glob != N))
+    return b200pets_set_error(B200PETS_EUNSUPPORTED, "per-row member models cannot be sharded over GPUs");
   if (ts1 && perms) {
     // reference TS1: a fresh permutation of all rows every step => rows change member (and tile) between steps;
     // one launch per step, state carried through the workspace
@@ -418,7 +561,8 @@ static int rollout_steps(b200pets_model_t model, const b200pets_rollout_cfg* cfg
       s.traj_obs = traj_obs ? traj_obs + (size_t)(t - t0) * B * d.obs_dim : nullptr;
       s.traj_reward = traj_reward ? traj_reward + (size_t)(t - t0) * B : nullptr;
       s.traj_done = traj_done ? traj_done + (size_t)(t - t0) * B : nullptr;
-      int rc = dispatch(model, precision, s, num_problems, bt, stream);
+      int rc = rows ? dispatch_member_rows(model, precision, s, perms + (size_t)t * B, num_problems, bt, bucket, stream)
+                    : dispatch(model, precision, s, num_problems, bt, stream);
       if (rc) return rc;
     }
   } else {
@@ -434,7 +578,8 @@ static int rollout_steps(b200pets_model_t model, const b200pets_rollout_cfg* cfg
     } else {             // in-kernel member draw: per (tile, step) for TS1, per tile for TSinf
       a.slot_mode = ts1 ? 1 : 2; a.perm = nullptr;
     }
-    int rc = dispatch(model, precision, a, num_problems, bt, stream);
+    int rc = rows ? dispatch_member_rows(model, precision, a, perms, num_problems, bt, bucket, stream)
+                  : dispatch(model, precision, a, num_problems, bt, stream);
     if (rc) return rc;
   }
   return B200PETS_OK;
@@ -461,8 +606,9 @@ static int eval_rows(b200pets_model_t model, const b200pets_rollout_cfg* cfg, in
   bt.eps = eps_stride;
   bt.seed = cfg->seed;
   bt.offset_step = offset_step;
+  void* bucket = dead + al256(KB);
   return rollout_steps(model, cfg, 0, cfg->horizon, false, obs0, actions, perms, eps, obs_state, total, dead, nullptr, nullptr,
-                       nullptr, stream, K, bt);
+                       nullptr, bucket, stream, K, bt);
 }
 
 // b200pets_eval_sequences(_batch) past their own checks: K evaluations and one particle mean over their K * N sequences
@@ -506,11 +652,11 @@ __global__ void trajectory_returns_kernel(long long B, int T, int first, const f
 }  // namespace
 
 // trajectory workspace: reward totals [B], dead flags [B], then the carried observations [B][D] (the returns call does
-// not know D, so the per-row scalars come first)
+// not know D, so the per-row scalars come first), then the member bucketing of per-row member models (bucket_bytes)
 size_t b200pets_trajectory_workspace_bytes(b200pets_model_t model, const b200pets_rollout_cfg* cfg) {
   if (!model || !cfg) return 0;
   const size_t B = (size_t)cfg->population * cfg->particles;
-  return al256(B * sizeof(float)) + al256(B) + al256(B * model->desc.obs_dim * sizeof(float));
+  return al256(B * sizeof(float)) + al256(B) + al256(B * model->desc.obs_dim * sizeof(float)) + bucket_bytes(model, 1, B);
 }
 
 int b200pets_eval_trajectory(b200pets_model_t model, const b200pets_rollout_cfg* cfg, int32_t t0, int32_t t1,
@@ -526,8 +672,9 @@ int b200pets_eval_trajectory(b200pets_model_t model, const b200pets_rollout_cfg*
     return b200pets_set_error(B200PETS_EINVAL, "eval_trajectory: workspace too small");
   const size_t B = (size_t)cfg->population * cfg->particles;
   float* obs_state = reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(workspace) + al256(B * sizeof(float)) + al256(B));
+  void* bucket = reinterpret_cast<unsigned char*>(obs_state) + al256(B * model->desc.obs_dim * sizeof(float));
   return rollout_steps(model, cfg, t0, t1, t1 < cfg->horizon, obs0, actions, perms, eps, obs_state, nullptr, nullptr, next_obs,
-                       reward, done, (cudaStream_t)stream);
+                       reward, done, bucket, (cudaStream_t)stream);
 }
 
 int b200pets_trajectory_returns(const b200pets_rollout_cfg* cfg, int32_t t0, int32_t t1, const float* reward,
@@ -570,7 +717,10 @@ int b200pets_step(b200pets_model_t model, int32_t precision, int32_t propagation
   if (!model || !obs || !act || !next_obs) return b200pets_set_error(B200PETS_EINVAL, "step: null argument");
   const b200pets_model_desc& d = model->desc;
   if (batch <= 0) return b200pets_set_error(B200PETS_EINVAL, "step: empty batch");
-  if (batch % d.num_members != 0)  // mbrl/models/gaussian_mlp.py:195-200 (checked for every propagation method)
+  const bool rows = d.member_rule == B200PETS_MEMBER_ROWS && propagation != B200PETS_PROP_EXPECTATION;
+  if (rows && !perm)
+    return b200pets_set_error(B200PETS_EINVAL, "step: per-row member models need the member indices of random_model / fixed_model");
+  if (d.member_rule == B200PETS_MEMBER_PERM && batch % d.num_members != 0)  // mbrl/models/gaussian_mlp.py:195-200 (checked for every propagation method)
     return b200pets_set_error(B200PETS_EINVAL, "GaussianMLP ensemble requires batch size to be a multiple of the number of models. "
                                                "Current batch size is %lld for %d models.", (long long)batch, d.num_members);
   if (propagation == B200PETS_PROP_FIXED_MODEL && !perm)  // gaussian_mlp.py:208-211
@@ -592,7 +742,19 @@ int b200pets_step(b200pets_model_t model, int32_t precision, int32_t propagation
   } else {
     a.slot_mode = 1;
   }
-  return dispatch(model, precision, a, 1, BatchArgs{}, (cudaStream_t)stream_);
+  if (!rows) return dispatch(model, precision, a, 1, BatchArgs{}, (cudaStream_t)stream_);
+  // the step has no workspace argument: its bucketing space is kept on the model and grown on demand
+  cudaStream_t stream = (cudaStream_t)stream_;
+  const size_t need = bucket_bytes(model, 1, (size_t)batch);
+  if (model->step_bucket_bytes < need) {
+    CUDA_TRY(cudaStreamSynchronize(stream));  // earlier steps on this stream may still read the old space
+    CUDA_TRY(cudaFree(model->step_bucket));
+    model->step_bucket = nullptr;
+    model->step_bucket_bytes = 0;
+    CUDA_TRY(cudaMalloc(&model->step_bucket, need));
+    model->step_bucket_bytes = need;
+  }
+  return dispatch_member_rows(model, precision, a, perm, 1, BatchArgs{}, model->step_bucket, stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -1073,6 +1235,16 @@ __global__ void member_map_kernel(RolloutArgs a, int M, int H, long long groups,
   out[idx] = shuffle_member(a.seed, a.offset, a.slot_mode, shuffle_global_group(geom, g), t, M);
 }
 }  // namespace
+
+int b200pets_member_slots(int32_t num_problems, int64_t batch, int32_t num_members, const int64_t* indices,
+                          int64_t* slots_out, int32_t* offsets_out, void* stream) {
+  if (!indices || !slots_out || !offsets_out || num_problems < 1 || batch < 1 || num_members < 1)
+    return b200pets_set_error(B200PETS_EINVAL, "member_slots: bad argument");
+  if (num_members > kMaxBucketMembers)
+    return b200pets_set_error(B200PETS_EUNSUPPORTED, "member_slots: at most %d members (got %d)", kMaxBucketMembers, num_members);
+  return launch_member_slots(num_problems, batch, num_members, indices, batch, reinterpret_cast<long long*>(slots_out),
+                             offsets_out, (cudaStream_t)stream);
+}
 
 int64_t b200pets_shuffle_num_groups(const b200pets_rollout_cfg* cfg) {
   if (!cfg || cfg->population <= 0 || cfg->particles <= 0) return 0;

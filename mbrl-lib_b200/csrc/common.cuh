@@ -47,6 +47,9 @@ struct RolloutArgs {
   int seq0;             // tile shuffle: global index of this shard's first sequence (0 on one GPU)
   int n_glob;           // tile shuffle: global population (= N on one GPU); fixes the global group numbering
   const long long* perm;   // [B] for this launch or NULL
+  // slot_mode 0 with per-row members (B200PETS_MEMBER_ROWS): [M+1] slot offsets of the members, perm = slot -> row
+  // (member_slots_kernel); member m owns slots [member_off[m], member_off[m+1]).  NULL: the equal split above.
+  const int* member_off;
   const float* eps;        // [t1-t0][B][out] for this launch (row-id indexed) or NULL -> Philox
   int sample;              // 0: mean prediction
   unsigned long long seed, offset;
@@ -83,6 +86,7 @@ struct BatchArgs {
   long long rows;                  // total_state / dead_state [B]
   long long perm, eps;             // injected permutation / model noise
   unsigned long long seed, offset_step;
+  long long member_off;            // member slot offsets (RolloutArgs::member_off)
 };
 
 // Launch plans, chosen on the host from the model's shape and the device's opt-in shared memory (the launchers and
@@ -325,6 +329,27 @@ __device__ __forceinline__ long long shuffle_row(const RolloutArgs& a, const Shu
 
 __device__ __forceinline__ long long slot_to_rid(const RolloutArgs& a, long long slot) {  // slot_mode 0 only
   return a.perm ? a.perm[slot] : slot;
+}
+
+// Per-row members (RolloutArgs::member_off = off): member m owns ceil(count_m / rows) tiles of `rows` rows, in member
+// order, over its slots [off[m], off[m+1]).  Tile `tile` -> its member and first slot; returns its row count, 0 for a
+// surplus tile of the bound ceil(B / rows) + M - 1 the grids are sized for.  Every role of a kernel that walks tiles
+// derives its tile list from this one function.
+__device__ __forceinline__ int member_tile(const int* off, int M, long long tile, int rows, int* member, long long* slot0) {
+  long long rest = tile;
+  for (int mm = 0; mm < M; ++mm) {
+    const int cnt = off[mm + 1] - off[mm];
+    const long long nt = (cnt + rows - 1) / rows;
+    if (rest < nt) {
+      *member = mm;
+      *slot0 = off[mm] + rest * rows;
+      return (int)min((long long)rows, cnt - rest * rows);
+    }
+    rest -= nt;
+  }
+  *member = 0;
+  *slot0 = 0;
+  return 0;
 }
 
 // member of global group `gt` at step t: an independent uniform draw per (group, step) from Philox

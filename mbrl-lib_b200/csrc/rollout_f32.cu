@@ -124,6 +124,11 @@ __device__ __forceinline__ void rollout_f32_body(const ModelDev& m, const Rollou
     if (expectation) {
       slot0 = (long long)tile * TR;
       nv = (int)min((long long)TR, a.B - slot0);
+    } else if (a.member_off) {
+      // per-row members: member m owns ceil(count_m / TR) tiles, in member order; the grid has the bound
+      // ceil(B / TR) + M - 1 tiles, and tiles past the members' own have no rows
+      nv = member_tile(a.member_off + prob_off<BATCH>(bt, kp, &BatchArgs::member_off), m.M, tile, TR, &member, &slot0);
+      if (nv == 0) return;  // uniform over the CTA, before any barrier
     } else {
       const long long Bm = a.B / m.M;
       const int tpm = (int)((Bm + TR - 1) / TR);
@@ -331,6 +336,7 @@ __global__ void __launch_bounds__(kThreads) rollout_f32_batch_kernel(const __gri
 static long long f32_num_tiles(const ModelDev& m, const RolloutArgs& a, int TR) {
   if (a.propagation == B200PETS_PROP_EXPECTATION) return (a.B + TR - 1) / TR;
   if (a.slot_mode >= 1) return (long long)a.P * shuffle_geom(a.seq0, a.N, a.n_glob).C_loc * (B200PETS_GROUP_ROWS / TR);
+  if (a.member_off) return (a.B + TR - 1) / TR + m.M - 1;
   long long Bm = a.B / m.M;
   return (long long)m.M * ((Bm + TR - 1) / TR);
 }

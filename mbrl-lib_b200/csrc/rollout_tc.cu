@@ -298,11 +298,18 @@ __device__ __forceinline__ void rollout_tc_body(const ModelDev& m, const Rollout
     if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
+      // per-row members: the tile list comes from the bucketing kernel's offsets, the previous kernel's output
+      if (!expect && a.member_off) pdl_wait();
       for (long long u = blockIdx.x; u < num_tiles; u += gridDim.x) {
         long long tile = u / kSplit;
         long long kp = 0;  // problem of a batched launch
         if constexpr (BATCH) { kp = tile / bt->tiles; tile -= kp * bt->tiles; }
-        const int member = (shuffle || expect) ? 0 : (int)(tile / tpm);
+        int member = (shuffle || expect) ? 0 : (int)(tile / tpm);
+        if (!expect && a.member_off) {  // the consumers skip the same surplus tiles (member_tile)
+          long long slot0;
+          if (member_tile(a.member_off + prob_off<BATCH>(bt, kp, &BatchArgs::member_off), m.M, tile, kTileM, &member, &slot0) == 0)
+            continue;
+        }
         for (int t = a.t0; t < a.t1; ++t)
         for (int pass = 0; pass < passes; ++pass) {
           const int mem = expect ? pass : (shuffle ? shuffle_member(prob_seed<BATCH>(a, bt, kp), prob_offset<BATCH>(a, bt, kp), a.slot_mode,
@@ -382,6 +389,14 @@ __device__ __forceinline__ void rollout_tc_body(const ModelDev& m, const Rollout
       if (shuffle) {
         rid = shuffle_row(a, geom, tile, ti, &valid, &rid_glob);
         if (!valid) rid = 0;
+      } else if (!expect && a.member_off) {  // per-row members: the producer's tile list (member_tile)
+        int member;
+        long long slot0;
+        const int nv = member_tile(a.member_off + prob_off<BATCH>(bt, kp, &BatchArgs::member_off), m.M, tile, kTileM, &member, &slot0);
+        if (nv == 0) continue;  // uniform over the CTA; the producer streams nothing for it
+        valid = ti < nv;
+        rid = valid ? prob_rid<BATCH>(a, bt, kp, slot0 + ti) : 0;
+        rid_glob = rid + (long long)a.seq0 * a.P;
       } else {
         const int member = (int)(tile / tpm);
         const int c = (int)(tile % tpm);
@@ -777,6 +792,7 @@ static long long tc_launch_tiles(const ModelDev& m, const RolloutArgs& a) {
   if (a.propagation == B200PETS_PROP_EXPECTATION)  // every row through every member: plain 128-row tiles, no member binding
     return (a.B + kTileM - 1) / kTileM;
   if (a.slot_mode >= 1) return (long long)a.P * shuffle_geom(a.seq0, a.N, a.n_glob).C_loc;
+  if (a.member_off) return (a.B + kTileM - 1) / kTileM + m.M - 1;  // per-row members: the bound of member_tile
   long long Bm = a.B / m.M;
   return (long long)m.M * ((Bm + kTileM - 1) / kTileM);
 }

@@ -3,6 +3,8 @@
 Drop-in: same constructor ``(env, model, termination_fn, reward_fn=None, generator=None)``, same
 ``reset`` / ``step`` / ``evaluate_action_sequences`` signatures, shapes, return types and error behaviour.
 Extra keyword-only knobs choose the arithmetic (``precision``) and how TS1 draws members (``ts1``).
+Over a BasicEnsemble the rows' members are drawn where the reference draws them, ``torch.randint(E, (B,))`` on the
+environment's generator (basic_ensemble.py:122-127, 255-260), and ``ts1`` has no effect.
 Constructed over a PlaNet latent model, it returns the latent environment of :mod:`mbrl_lib_b200.latent`.
 """
 from __future__ import annotations
@@ -90,6 +92,14 @@ class ModelEnv:
         (exact reference rule, gaussian_mlp.py:202-212)."""
         groups = particles * ((population + 127) // 128)
         return groups < 2 * len(self.staged.members())
+
+    def _member_rows(self) -> bool:
+        """True over a BasicEnsemble: each row's member is an index drawn by :meth:`_draw_members`."""
+        return self.staged.member_rule == "rows"
+
+    def _draw_members(self, batch: int) -> torch.Tensor:
+        """One BasicEnsemble member draw for ``batch`` rows, on this environment's generator (basic_ensemble.py:126)."""
+        return torch.randint(len(self.staged.members()), (batch,), generator=self._rng, device=self.device)
 
     def _workspace(self, nbytes: int) -> torch.Tensor:
         if self._ws is None or self._ws.numel() < nbytes:
@@ -198,7 +208,9 @@ class ModelEnv:
         self._fresh()
         obs = torch.from_numpy(np.ascontiguousarray(initial_obs_batch.astype(np.float32))).to(self.device)
         state = {"obs": obs, "propagation_indices": None}
-        if self._propagation() == "fixed_model":
+        if self._propagation() == "fixed_model" and self._member_rows():
+            state["propagation_indices"] = self._draw_members(obs.shape[0])  # model.py:405, basic_ensemble.py:255-260
+        elif self._propagation() == "fixed_model":
             B, M = obs.shape[0], len(self.staged.members())
             if B % M != 0:  # gaussian_mlp.py:369-373
                 raise ValueError("To use GaussianMLP's ensemble propagation, the batch size must "
@@ -228,6 +240,8 @@ class ModelEnv:
                     perm = model_state.get("propagation_indices")
                     if perm is None:
                         raise ValueError("When using propagation='fixed_model', `propagation_indices` must be provided.")
+                elif prop == "random_model" and self._member_rows():
+                    perm = self._draw_members(B)
                 elif prop == "random_model" and (self.ts1 == "perms" or self._few_groups(B, 1)):
                     perm = torch.randperm(B, device=self.device)
             if perm is not None:
@@ -313,6 +327,8 @@ class ModelEnv:
     def _eval_perms(self, prop: str, population: int, horizon: int, num_particles: int) -> Optional[torch.Tensor]:
         """The permutations :meth:`evaluate_action_sequences` draws for one evaluation (None: members drawn in kernel)."""
         B = population * num_particles
+        if self._member_rows() and prop != "expectation":
+            return torch.stack([self._draw_members(B) for _ in range(horizon if prop == "random_model" else 1)])
         if prop == "fixed_model":
             if B % len(self.staged.members()) != 0:
                 raise ValueError("To use GaussianMLP's ensemble propagation, the batch size must "

@@ -128,6 +128,35 @@ class Normalizer:
         return (val - self.mean) / self.std
 
 
+class BasicEnsemble(nn.Module):
+    """mbrl-lib's ``BasicEnsemble`` (mbrl/models/basic_ensemble.py) as the kernels read it: ``members``, E one-member
+    GaussianMLPs of one shape, all of them used (``set_elite`` changes nothing, basic_ensemble.py:262-266).  Under
+    ``random_model`` every forward draws each row's member with ``torch.randint(E, (B,))``; under ``fixed_model`` the
+    rows keep the members of :meth:`sample_propagation_indices` for a whole rollout."""
+
+    def __init__(self, members: Sequence[GaussianMLP], propagation_method: Optional[str] = None):
+        super().__init__()
+        self.members = nn.ModuleList(members)
+        m0 = self.members[0]
+        self.in_size, self.out_size = m0.in_size, m0.out_size
+        self.num_members = len(self.members)
+        self.deterministic = m0.deterministic
+        self.propagation_method = propagation_method
+        self.device = m0.device
+
+    def __len__(self):
+        return len(self.members)
+
+    def set_elite(self, elite_indices: Sequence[int]):
+        pass  # every member is used (basic_ensemble.py:262-266)
+
+    def set_propagation_method(self, propagation_method: Optional[str] = None):
+        self.propagation_method = propagation_method
+
+    def sample_propagation_indices(self, batch_size: int, rng: torch.Generator) -> torch.Tensor:
+        return torch.randint(len(self), (batch_size,), generator=rng, device=self.device)  # basic_ensemble.py:255-260
+
+
 class OneDTransitionRewardModel:
     def __init__(self, model: GaussianMLP, target_is_delta: bool = True, normalize: bool = False,
                  normalize_double_precision: bool = False, learned_rewards: bool = True,
@@ -199,6 +228,34 @@ class OneDTransitionRewardModel:
         with torch.no_grad():
             model_in, target = self._process_batch(batch)
             return self.model.eval_score(model_in, target=target)
+
+
+def basic_ensemble_from_arrays(spec, arrays, device) -> OneDTransitionRewardModel:
+    """The model of :func:`model_from_arrays` with its stacked ensemble split into a :class:`BasicEnsemble` of
+    ``spec.ensemble_size`` one-member GaussianMLPs: member e holds slice e of every layer and the shared logvar bounds."""
+    from . import functions
+
+    members = []
+    for e in range(spec.ensemble_size):
+        mlp = GaussianMLP(spec.in_size, spec.out_size, device, num_layers=spec.num_layers, ensemble_size=1,
+                          hid_size=spec.hid_size, deterministic=spec.deterministic, activation=spec.activation)
+        with torch.no_grad():
+            for li, layer in enumerate(list(mlp.hidden_layers) + [None]):
+                lin = layer[0] if layer is not None else mlp.mean_and_logvar
+                lin.weight.copy_(torch.from_numpy(arrays["weights"][li][e:e + 1]))
+                lin.bias.copy_(torch.from_numpy(arrays["biases"][li][e:e + 1]))
+            if not spec.deterministic:
+                mlp.min_logvar.copy_(torch.from_numpy(arrays["min_logvar"]))
+                mlp.max_logvar.copy_(torch.from_numpy(arrays["max_logvar"]))
+        members.append(mlp)
+    wrapper = OneDTransitionRewardModel(
+        BasicEnsemble(members, spec.propagation), target_is_delta=spec.target_is_delta, normalize=spec.normalize is not None,
+        normalize_double_precision=spec.normalize == "float64", learned_rewards=spec.learned_rewards,
+        obs_process_fn=functions.OBS_PROCESS_FNS.get(spec.obs_process), no_delta_list=list(spec.no_delta_list))
+    if spec.normalize is not None:
+        wrapper.input_normalizer.mean = torch.from_numpy(arrays["norm_mean"]).to(device)
+        wrapper.input_normalizer.std = torch.from_numpy(arrays["norm_std"]).to(device)
+    return wrapper
 
 
 def model_from_arrays(spec, arrays, device) -> OneDTransitionRewardModel:

@@ -202,7 +202,11 @@ class CEMOptimizer(Optimizer):
                            int(self._clipped_normal))
 
     def _plan_perms(self, env, prop: str, horizon: int, num_particles: int) -> Optional[torch.Tensor]:
-        """The permutations one fused plan draws, ``[iterations, horizon or 1, N * P]`` (None: members drawn in kernel)."""
+        """The permutations one fused plan draws, ``[iterations, horizon or 1, N * P]`` (None: members drawn in kernel);
+        over a BasicEnsemble the per-row member indices of each iteration's evaluation."""
+        if prop != "expectation" and env._member_rows():
+            return torch.stack([env._eval_perms(prop, self.population_size, horizon, num_particles)
+                                for _ in range(self.num_iterations)])
         if prop not in ("random_model", "fixed_model") or not (
                 env.ts1 == "perms" or env._few_groups(self.population_size, num_particles)):
             return None
